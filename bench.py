@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- BASELINE.json's headline metric on the B200-native tiled-diffusion hot path.
+"""bench.py -- BASELINE.json's headline metric on the H100-native (sm_90a) tiled-diffusion hot path.
 
 Workload (config.workload): BASELINE configs[1] -- SD1.5 4096x4096 txt2img, MultiDiffusion,
 96x96 latent tiles, overlap 48 (the UI default), 50 sampler steps: latent [N=2, C=4, 512, 512]
@@ -23,7 +23,7 @@ reference; `kind: "port"`), on this box's host cores at the thread count that ru
 Other BASELINE configs (same JSON contract, DESIGN.md section 6):
     --config cfg3   Mixture of Diffusers step (td_blend_mixture heads the roofline object)
     --config cfg4   tiled VAE decode only, z [1,4,1024,1024] -> 8192 x 8192 RGB through tilevae.VAEHook (one step = one decode;
-                    roofline.bound = "tensor": the dominant tcgen05 convolution + the whole-decode TFLOP/s); --vae-slow
+                    roofline.bound = "tensor": the dominant wgmma convolution + the whole-decode TFLOP/s); --vae-slow
     --config cfg5   one DemoFusion.sample_one_step at the x4 phase of an SDXL 6144^2 upscale (latent [2,4,768,768])
     --gpus N        under torchrun: row-strip tile shard for cfg2 (weak scaling by default, strong rides along, in-run
                     parity_ok), tile round-robin for cfg4, window / view shard for cfg5
@@ -63,12 +63,12 @@ def load_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json, burst copy)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3), not measured"
 
 
 # ----------------------------------------------------------------------------- clocks
 class ClockSampler:
-    """nvidia-smi sampler running while the GPU is under load (recipe in B200_PROFILING.md)."""
+    """nvidia-smi sampler running while the GPU is under load (SM clock, its maximum, throttle reasons)."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -514,6 +514,25 @@ def timed_graph_loop(fn_step, steps, stream, chunk=1024):
     return replay
 
 
+DUMP_LIMIT = 64 << 20
+
+
+def dump_outputs(path: str, arrays: dict):
+    """DIR/<name>.npy in float32, one file per output of the timed path (compare two builds output for output).  Above
+    64 MB in all, every output is cut to the same share of its elements, picked by a fixed seed (sorted flat indices),
+    so two runs with the same arguments sample the same positions; the file is then 1-D."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    total = sum(t.numel() * 4 for t in arrays.values())
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy()
+        if total > DUMP_LIMIT:
+            k = max(1, a.size * DUMP_LIMIT // total)
+            idx = np.sort(np.random.Generator(np.random.PCG64(0)).choice(a.size, size=k, replace=False))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(path, name + ".npy"), a)
+
+
 def event_time_ms(fn, stream):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     torch.cuda.synchronize()
@@ -565,6 +584,9 @@ def gpu_arm(args, rank, world, local_rank):
         barrier()
         ms = event_time_ms(replay, stream)             # EXACTLY args.steps steps
         barrier()
+        if args.dump_outputs and rank == 0:            # what the last timed step handed back, before anything reuses the buffers
+            s = (args.steps - 1) % nsets
+            dump_outputs(args.dump_outputs, {"tiles": wl.tiles_in[s], "latent": wl._mod[2][s] if mod else wl.x_out[s]})
         t = torch.tensor([ms], device=dev)
         if world > 1:
             torch.distributed.all_reduce(t, op=torch.distributed.ReduceOp.MAX)
@@ -821,7 +843,7 @@ def strip_e2e(args, dev, stream, world, rank):
 
 
 def load_traffic(kernel: str):
-    """dram bytes per launch from the committed ncu --set full capture (profiles/traffic.json), or None."""
+    """dram bytes per launch from a saved profiler capture (profiles/traffic.json) when one is present, else None."""
     p = os.path.join(ROOT, "profiles", "traffic.json")
     try:
         return json.load(open(p)).get(kernel)
@@ -1027,7 +1049,14 @@ def vae_arm(args, rank, world, local_rank):
     torch.cuda.synchronize()
     if world > 1:
         torch.distributed.barrier()
-    ms = event_time_ms(lambda: [hook(z) for _ in range(steps)], stream)
+    last = {}
+
+    def timed():
+        for _ in range(steps):
+            last["image"] = hook(z)
+    ms = event_time_ms(timed, stream)
+    if args.dump_outputs and rank == 0:                 # the decoded image of the last timed step
+        dump_outputs(args.dump_outputs, last)
     t = torch.tensor([ms], device=dev)
     if world > 1:
         torch.distributed.all_reduce(t, op=torch.distributed.ReduceOp.MAX)
@@ -1057,12 +1086,11 @@ def vae_arm(args, rank, world, local_rank):
         return
 
     flops = vae_decode_flops(hook, lat, lat)
-    tf_burst, tf_sust = 1661.3, 1404.6
     try:
         pk = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         tf_burst, tf_sust, peak_src = float(pk["bf16_tflops"]), float(pk["bf16_tflops_sustained"]), "measured (MEASURED_PEAKS.json, cuBLAS bf16)"
     except Exception:
-        tf_burst, tf_sust, peak_src = 1590.0, 1400.0, "fallback (B200_PROFILING.md)"
+        tf_burst, tf_sust, peak_src = 989.0, 989.0, "H100 SXM data sheet (dense FP16 / BF16), not measured"
     # dominant kernel: the level-0 128 -> 128 3x3 convolution of a full tile (944 x 944), timed alone
     x = (torch.randn((1, 944, 944, 128), device=dev) * 0.5).half()
     w = (torch.randn((9, 128, 128), device=dev) * 0.03).half()
@@ -1087,13 +1115,13 @@ def vae_arm(args, rank, world, local_rank):
         "e2e": {"value": mp / e2e_sec, "unit": "MP/s", "h2d_bytes_per_step": z_host.numel() * 2, "d2h_bytes_per_step": out_host.numel() * 2,
                 "ms_per_step": e2e_sec * 1e3, "api": "VAEHook.__call__ (hooked decoder forward), pinned-host latent in, pinned-host image out"},
         "gpu_launches": None,
-        "roofline": {"bound": "tensor", "kernel": "conv_gemm_kernel (td_conv2d_nhwc, tcgen05 implicit GEMM), 128->128 3x3 on [1,944,944,128]",
+        "roofline": {"bound": "tensor", "kernel": "conv_gemm_kernel (td_conv2d_nhwc, wgmma implicit GEMM), 128->128 3x3 on [1,944,944,128]",
                      "achieved": conv_flops / t_conv / 1e12, "peak": tf_burst, "unit": "TFLOP/s", "frac": conv_flops / t_conv / 1e12 / tf_burst,
                      "traffic": load_traffic("conv_944_128_128"), "peak_source": peak_src + ", burst (kernel timed alone)", "algorithmic_flops": conv_flops,
                      "avg_launch_us": t_conv * 1e6,
                      "whole_decode": {"algorithmic_flops": flops, "achieved": flops / sec / 1e12, "peak": tf_sust,
                                       "frac": flops / sec / 1e12 / tf_sust, "peak_source": "sustained (inside a long step)"}},
-        "parity": {"what": "tcgen05 / channels-last backend vs cuDNN-module backend, same fp16 weights, z[:, :, :160, :160] (4 tiles)",
+        "parity": {"what": "wgmma / channels-last backend vs cuDNN-module backend, same fp16 weights, z[:, :, :160, :160] (4 tiles)",
                    "mean_rel": diff.mean().item() / scale, "max_rel": diff.max().item() / scale},
         "impl": "b200",
     }
@@ -1208,7 +1236,14 @@ def demofusion_arm(args, rank, world, local_rank):
     if world > 1:
         torch.distributed.barrier()
     calls[0] = 0
-    ms = event_time_ms(lambda: [d.sample_one_step(x, sigma, cond) for _ in range(steps)], stream)
+    last = {}
+
+    def timed():
+        for _ in range(steps):
+            last["latent"] = d.sample_one_step(x, sigma, cond)
+    ms = event_time_ms(timed, stream)
+    if args.dump_outputs and rank == 0:                 # the DemoFusion step's output latent of the last timed step
+        dump_outputs(args.dump_outputs, last)
     unet_calls = calls[0] // steps
     t = torch.tensor([ms], device=dev)
     if world > 1:
@@ -1267,7 +1302,7 @@ def demofusion_arm(args, rank, world, local_rank):
                                f"{d.num_tiles} local windows {c['window']}^2 stride {c['window'] - c['overlap']} (batches of {d.tile_bs}), scale {c['scale']}, "
                                f"{d.global_num_tiles} dilated views (mixture), gaussian filter k={2 * c['scale'] - 1}, identity UNet stand-in "
                                f"({unet_calls} calls / step)",
-                   "l2": f"{algo / 1e6:.0f} MB of algorithmic traffic per step (> the 126 MB L2); every intermediate is written once and read once",
+                   "l2": f"{algo / 1e6:.0f} MB of algorithmic traffic per step (> the 50 MB L2); every intermediate is written once and read once",
                    "parallelism": "single GPU" if world == 1 else f"windows + views sharded over {world} ranks, two all-gathers per step (NCCL)"},
         "clocks": clocks,
         "e2e": {"value": mp / e2e_sec, "unit": "MP/s", "h2d_bytes_per_step": canvas, "d2h_bytes_per_step": canvas, "ms_per_step": e2e_sec * 1e3,
@@ -1351,7 +1386,14 @@ def main():
                     "(default, the headline), cfg3 = Mixture of Diffusers hot path, cfg4 = tiled VAE decode only, cfg5 = DemoFusion step")
     ap.add_argument("--vae-latent", type=int, default=1024, help="cfg4: latent edge (1024 -> 8192^2 image)")
     ap.add_argument("--vae-slow", action="store_true", help="cfg4: slow mode (GroupNorm statistics merged over all tiles at every site)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps write the last step's outputs as DIR/<name>.npy in float32 (cfg2 / cfg3: tile batch "
+                         "and blended latent, one GPU; cfg4: decoded image; cfg5: output latent), a seeded sample above 64 MB in all; "
+                         "inputs are seeded, so two builds can be compared output for output")
     args = ap.parse_args()
+    torch.manual_seed(0)      # device-side synthetic inputs (tile outputs) are the same from run to run
+    if args.dump_outputs and (args.impl != "b200" or (args.config in ("cfg2", "cfg3") and args.gpus != 1)):
+        sys.exit("--dump-outputs covers the GPU arm: cfg2 / cfg3 on one GPU, cfg4 and cfg5")
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))

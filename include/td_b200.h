@@ -1,5 +1,5 @@
 /*
- * td_b200.h -- C-ABI of the B200-native tiled-diffusion / tiled-VAE hot path.
+ * td_b200.h -- C-ABI of the H100-native tiled-diffusion / tiled-VAE hot path.
  *
  * The reference (pkuliyi2015/multidiffusion-upscaler-for-automatic1111 @ 22798f6)
  * has NO FFI boundary: its hot path is eager PyTorch inside Python classes
@@ -48,7 +48,7 @@ typedef enum td_dtype { TD_F16 = 0, TD_BF16 = 1, TD_F32 = 2 } td_dtype;
 #define TD_FLAG_STRIP 128u       /* MultiDiffusion blend: strip CTAs (8 rows x full width), opt-in, see csrc/td_strip.cu */
 #define TD_FLAG_DBG_NO_TILES 0x100u /* measurement aid: skip all tile visits (launch + epilogue floor) */
 #define TD_FLAG_ROWS 0x400u      /* row-block form (csrc/td_rows.cu: one persistent CTA per SM, bulk-copy staging), opt-in: bit-identical,
-                                    measured slower than the default kernels on B200 (DESIGN.md section 4) */
+                                    the default kernels stay many small co-resident CTAs (DESIGN.md section 4) */
 
 #define TD_MAX_GRID_DIM 256   /* max tile rows / cols of a grid plan            */
 #define TD_MAX_BATCH_PTRS 128 /* max UNet output batch tensors per blend launch */
@@ -337,7 +337,7 @@ int td_depthwise_conv2d(const void* in, void* out, int planes, int H, int W, con
                         int k, int dtype, void* stream);
 
 /* ------------------------------------------------------------------------- *
- *  Tiled-VAE dense contractions on the tensor cores (tcgen05.mma, fp32 accumulators in TMEM).
+ *  Tiled-VAE dense contractions on the tensor cores (wgmma, fp32 accumulators in registers).
  *  The reference executes its conv / attention tasks at scripts/tilevae.py:618 through third-party
  *  ldm modules (queue built at :107-204; attention tile_utils/attn.py:49-72).
  * ------------------------------------------------------------------------- */

@@ -1,9 +1,9 @@
-"""B200-native tiled-diffusion + tiled-VAE hot path behind the reference's API.
+"""H100-native tiled-diffusion + tiled-VAE hot path behind the reference's API.
 
 Drop-in for `pkuliyi2015/multidiffusion-upscaler-for-automatic1111`'s tile-method
 delegates (`MultiDiffusion`, `MixtureOfDiffusers`) and `tilevae.VAEHook`: Python
 host classes with the reference's names and arguments, calling hand-written
-sm_100a CUDA kernels through the C-ABI in `include/td_b200.h`.
+sm_90a CUDA kernels through the C-ABI in `include/td_b200.h`.
 
 Importing this package loads `libtd_b200.so`; if it is missing the import fails
 (there is no CPU / PyTorch fallback).

@@ -1,8 +1,7 @@
-"""Build recipe for libtd_b200.so (hand-written sm_100a CUDA behind a C-ABI).
+"""Build recipe for libtd_b200.so (hand-written sm_90a CUDA behind a C-ABI).
 
-`nvcc` cross-compiles without a GPU, so this runs in the build container and the
-resulting .so travels with the repo snapshot to the B200 box (it is git-ignored,
-not gpurun-ignored).  Usage: `python -m multidiffusion_upscaler_for_automatic1111_b200.build`.
+`nvcc` cross-compiles without a GPU, so the library can be built on a machine without one; it is
+git-ignored and written next to this file.  Usage: `python -m multidiffusion_upscaler_for_automatic1111_b200.build`.
 """
 from __future__ import annotations
 
@@ -17,7 +16,7 @@ INCLUDE = os.path.join(os.path.dirname(PKG_DIR), "include")
 LIB_PATH = os.path.join(PKG_DIR, "libtd_b200.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "--shared", "-Xcompiler", "-fPIC,-ffp-contract=off",
     "-Xptxas", "-v",
@@ -58,7 +57,7 @@ def build_variant(out_path: str, defines) -> str:
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile every CUDA source for sm_100a into libtd_b200.so; returns its path."""
+    """Compile every CUDA source for sm_90a into libtd_b200.so; returns its path."""
     if not force and not needs_build():
         return LIB_PATH
     nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"

@@ -1,22 +1,24 @@
-// Tiled-VAE convolutions and attention GEMMs on the 5th-generation tensor cores (sm_100a):
+// Tiled-VAE convolutions and attention GEMMs on the Hopper tensor cores (sm_90a, wgmma):
 //   the conv / upsample / downsample / attention tasks the reference executes at scripts/tilevae.py:618 through
 //   third-party ldm modules (3x3 s1 p1 convs, 1x1 nin_shortcut / q / k / v / proj_out, nearest x2 + conv,
 //   pad(0,1,0,1) + 3x3 s2 conv; tile_utils/attn.py:49-72 QK^T and PV) as ONE implicit-GEMM kernel:
 //
 //       D[pixel, co] = alpha * sum_{tap, ci} A[pixel + offset(tap), ci] * W[tap][co][ci]  + bias  (+ residual)
 //
-// Design (B200-first):
+// Design:
 //   * activations NHWC fp16 / bf16 (channels innermost): a 3x3 tap is a shifted 4-D TMA box {64 ch, BW, BH, 1} of the
 //     SAME tensor -- signed start coordinates, out-of-bounds rows / columns zero-filled by the TMA unit = the
 //     convolution's zero padding, no im2col buffer, no halo handling in software.  BW x BH = 128 output pixels = the
-//     UMMA M dimension; a stride-2 convolution is the same box with element strides {1,2,2,1};
-//   * the box lands in shared memory as 128 rows x 128 bytes, 128-byte swizzled = the canonical K-major UMMA operand
-//     layout; weights [tap][Cout][Cin] load the same way ({64, BN, 1} boxes).  One elected thread issues
-//     tcgen05.mma.cta_group::1.kind::f16 (M = 128, N = BN <= 256, K = 16) four times per 64-channel stage;
-//   * fp32 accumulators live in TMEM (2 x BN columns: the epilogue of tile i overlaps the MMAs of tile i+1);
-//   * warp roles: warp 0 TMA producer, warp 1 MMA issuer, warp 2 TMEM allocator, warps 4-7 epilogue
-//     (tcgen05.ld -> alpha / bias / residual -> fp16 -> swizzled smem -> TMA store, which also clips partial tiles);
-//   * persistent: one CTA per SM walks the (pixel tile, Cout block) list, 4-stage smem ring (mbarrier full / empty).
+//     tile's M dimension; a stride-2 convolution is the same box with element strides {1,2,2,1};
+//   * the box lands in shared memory as 128 rows x 128 bytes, 128-byte swizzled = the K-major wgmma operand layout;
+//     weights [tap][Cout][Cin] load the same way ({64, BN, 1} boxes);
+//   * warp roles: warp 8 is the TMA producer (one elected thread), warps 0-3 and 4-7 are two consumer warpgroups that
+//     each issue wgmma.m64nBNk16 for 64 of the 128 pixel rows (four per 64-channel stage) and keep the 64 x BN fp32
+//     accumulator tile in registers (BN / 2 per thread, <= 128: 288 threads leave 224 registers each);
+//   * epilogue straight from the accumulator registers: alpha / bias / residual (/ frozen GroupNorm + SiLU) in fp32,
+//     one rounding to fp16 / bf16, stores clipped to the output tensor; it overlaps the producer's loads of the next
+//     tile;
+//   * persistent: one CTA per SM walks the (pixel tile, Cout block) list, up to 8-stage smem ring (mbarrier full / empty).
 // A plain GEMM (attention: S = Q K^T, O = P V, V^T = Wv X^T) is the 1x1 "image" with H = 1, W = M.
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -32,64 +34,39 @@
 #include "td_b200.h"
 #include "td_internal.h"
 #include "td_tma.cuh"
+#include "td_wgmma.cuh"
 
 namespace {
 
 using namespace td;
 
-constexpr int kConvThreads = 384;   // warp 0 TMA, 1 MMA, 2 TMEM alloc, 3 idle, 4-7 and 8-11: two epilogue groups
-constexpr int kConvBM = 128;              // output pixels per tile = UMMA M
+constexpr int kConvThreads = 288;         // warps 0-7: two consumer warpgroups, warp 8: TMA producer
+constexpr int kConvBM = 128;              // output pixels per tile
 constexpr int kConvBK = 64;               // channels per stage (128 bytes of fp16 = one swizzle row)
 constexpr int kConvStageA = kConvBM * kConvBK * 2;   // 16 KB
-constexpr int kConvStoreBuf = kConvBM * 128;         // 16 KB epilogue staging buffer (128 rows x 64 ch x 2 B)
 constexpr int kConvMaxStages = 8;
 
 struct ConvParams {
     int taps_x, taps_y;        // kw, kh
     int stride;                // 1 or 2
     int pad_left, pad_top;
-    int OW, OH, NI;            // output image and batch
+    int OW, OH, NI;            // grid of output pixels the tiles walk, and its "image" count
     int Cin_chunks;            // ceil(Cin / 64)
-    int Cout;                  // real output channels (bias / residual guard)
-    int BN;                    // Cout block = UMMA N (16..256, multiple of 16)
+    int Cout;                  // real output channels (bias / residual / store guard)
     int n_blocks;              // ceil(Cout / BN)
-    int BW, BH;                // pixel patch of one CTA tile: BW * BH == 128 * MT
-    int MT;                    // 128-pixel sub-tiles per CTA tile (1 or 2): they share the weight tile of a k-step, which
-                               // halves the weight bytes an SM pulls per FLOP (the kernel is bound by L2 -> SM bytes)
-    int BWs, BHs;              // sub-tile shape (store box): 16 x 8 image rows, or 128 x 1 for a GEMM
-    int sub_dx, sub_dy;        // origin of sub-tile mt inside the patch: (mt * sub_dx, mt * sub_dy)
-    int acc_stages;            // accumulator stages in TMEM: 512 / (MT * BN) capped at 2
+    int BW, BH;                // pixel patch of one tile: BW * BH == 128 (16 x 8 image rows, 8 x 16, or 128 x 1 for a GEMM)
     int tiles_x, tiles_y;
     int num_tiles;             // NI * tiles_y * tiles_x * n_blocks
     int stages;
-    int chunk_cols;            // columns per store chunk: min(64, BN)
     int is_bf16;
     int bias_per_row;          // bias indexed by output pixel (GEMM row) instead of channel
     int post_act;              // with post_scale / post_shift: 1 = SiLU after the per-channel affine
-    int pair;                  // 1: CTA pair (cluster of 2) on ONE 256-pixel patch with tcgen05.mma.cta_group::2 -- each CTA stages its
-                               // own 128-pixel sub-tile and HALF of the weight tile, the pair's tensor cores read both halves:
-                               // 32 KB instead of 48 KB into each SM per k-step at BN = 256
-    int cluster;               // CTAs per cluster (1, 2 or 4): consecutive pixel tiles share the weight tile by TMA multicast
-    int m_tiles;               // NI * tiles_y * tiles_x
-    int m_groups;              // ceil(m_tiles / cluster)
     float alpha;
-    int dual;                  // 1: two outputs -- map_d receives the result BEFORE the post affine / activation (the residual source of
-                               // the next block), map_d2 the result after it (the next block's normalised input)
     int up2;                   // 1: nearest-2x upsample folded into the 3x3 convolution -- four 2x2 convolutions of the LOW-resolution
-                               // image, one per output parity (py, px) = "image" index & 3; weights [16 taps, Cout, Cin]; the
-                               // output map is 5-D {c, x, y, px, py} over the high-resolution tensor
-    long long res_pitch;       // residual: elements between pixels (0: none)
+                               // image, one per output parity (py, px) = "image" index (py * 2 + px); weights [16 taps, Cout, Cin];
+                               // tile pixel (x, y) of parity (py, px) is output pixel (2 x + px, 2 y + py)
+    long long y_pitch, y2_pitch, res_pitch;   // elements between pixels
 };
-
-__device__ __forceinline__ uint32_t elect_one() {
-    uint32_t pred = 0;
-    asm volatile(
-        "{\n\t.reg .b32 %%rx;\n\t.reg .pred %%px;\n\t"
-        "elect.sync %%rx|%%px, %1;\n\t"
-        "@%%px mov.s32 %0, 1;\n\t}"
-        : "+r"(pred) : "r"(0xffffffffu));
-    return pred;
-}
 
 __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map, int c0, int c1, int c2, int c3, uint64_t* bar) {
     asm volatile(
@@ -101,117 +78,12 @@ __device__ __forceinline__ void tma_load_3d_u32(uint32_t dst, const CUtensorMap*
         "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
         ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(c2), "r"(smem_u32(bar)) : "memory");
 }
-// weight slice of this CTA, written into the same shared-memory offset of every CTA of the cluster (and completing
-// bytes on each CTA's own full barrier)
-__device__ __forceinline__ void tma_load_3d_mcast(uint32_t dst, const CUtensorMap* map, int c0, int c1, int c2, uint64_t* bar, uint16_t mask) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%2, %3, %4}], [%5], %6;"
-        ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(c2), "r"(smem_u32(bar)), "h"(mask) : "memory");
-}
-// CTA-pair forms: the copy lands in the executing CTA's shared memory, its bytes complete on the LEADER CTA's barrier
-// (shared::cluster address with the pair's rank bit cleared, as CUTLASS's Sm100MmaPeerBitMask does)
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-__device__ __forceinline__ void tma_load_4d_2sm(uint32_t dst, const CUtensorMap* map, int c0, int c1, int c2, int c3, uint32_t leader_bar) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];"
-        ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(leader_bar) : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_2sm(uint32_t dst, const CUtensorMap* map, int c0, int c1, int c2, uint32_t leader_bar) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
-        ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(c2), "r"(leader_bar) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar_cluster_addr) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(bar_cluster_addr) : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_rank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, int c0, int c1, int c2, int c3, uint32_t src) {
-    asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%1, %2, %3, %4}], [%5];"
-                 ::"l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(src) : "memory");
-}
-__device__ __forceinline__ void tma_store_5d(const CUtensorMap* map, int c0, int c1, int c2, int c3, int c4, uint32_t src) {
-    asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%1, %2, %3, %4, %5}], [%6];"
-                 ::"l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4), "r"(src) : "memory");
-}
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N> __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
-__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// the same arrive delivered to the barrier at this offset in every CTA of `mask` (frees the stage cluster-wide)
-__device__ __forceinline__ void tc_commit_mcast(uint64_t* bar, uint16_t mask) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"(mask) : "memory");
-}
-__device__ __forceinline__ void tc_commit_2sm_mcast(uint64_t* bar, uint16_t mask) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"(mask) : "memory");
-}
-// the pair's MMA: M = 256 (128 rows from each CTA's A tile), N = BN (BN / 2 weight rows from each CTA), issued by the leader
-__device__ __forceinline__ void tc_mma_f16_2sm(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; kind::f16 covers fp16 and bf16 inputs with fp32 accumulation
-__device__ __forceinline__ void tc_mma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// 32 lanes x 16 consecutive fp32 columns of this warp's TMEM lane quarter
-__device__ __forceinline__ void tc_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// K-major operand, 128-byte swizzle: rows of 128 bytes, 8-row groups 1024 bytes apart (SBO), descriptor version 1
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
-    uint64_t d = (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
-    d |= (uint64_t)1 << 16;                 // leading byte offset (unused for swizzled K-major): 16 B
-    d |= (uint64_t)(1024 >> 4) << 32;       // stride byte offset: 8 rows x 128 B
-    d |= (uint64_t)1 << 46;                 // descriptor version (sm_100)
-    d |= (uint64_t)2 << 61;                 // SWIZZLE_128B
-    return d;
-}
-// instruction descriptor: fp32 accumulate, A / B both K-major, M = 128, N = n
-__device__ __forceinline__ uint32_t umma_idesc(int n, int is_bf16, int m = kConvBM) {
-    uint32_t d = 0;
-    d |= 1u << 4;                           // D format: F32
-    d |= (is_bf16 ? 1u : 0u) << 7;          // A format
-    d |= (is_bf16 ? 1u : 0u) << 10;         // B format
-    d |= (uint32_t)(n >> 3) << 17;          // N / 8
-    d |= (uint32_t)(m >> 4) << 24;          // M / 16
-    return d;
-}
-
-__device__ __forceinline__ void named_bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 
 __device__ __forceinline__ uint32_t pack2(float a, float b, int is_bf16) {
     if (is_bf16) {
@@ -229,326 +101,144 @@ __device__ __forceinline__ float unpack_hi(uint32_t w, int is_bf16) {
 }
 
 struct TileCoord { int img, py, px, nb; };
-// Work list: group g = (Cout block fastest, then pixel-tile group); the CTAs of a cluster take the `cluster` consecutive
-// pixel tiles of one group (same Cout block: they share the weight tile).  A pixel tile past the end is a dummy: its
-// loads are out of bounds (zero fill), its store is clipped away.
-__device__ __forceinline__ TileCoord decode_tile(const ConvParams& p, int g, int crank) {
+// work list: Cout block fastest, then pixel tile (consecutive CTAs read the same activation box from L2)
+__device__ __forceinline__ TileCoord decode_tile(const ConvParams& p, int g) {
     TileCoord c;
     c.nb = g % p.n_blocks;
-    int m = p.pair ? g / p.n_blocks : (g / p.n_blocks) * p.cluster + crank;   // a pair works on ONE patch
+    int m = g / p.n_blocks;
     c.px = m % p.tiles_x; m /= p.tiles_x;
     c.py = m % p.tiles_y;
-    c.img = m / p.tiles_y;          // >= NI for a dummy tile
+    c.img = m / p.tiles_y;
     return c;
 }
 
-// PAIR selects the CTA-pair form at compile time: every tcgen05 instruction of one kernel must carry the same
-// .cta_group (mixing ::1 and ::2 in one kernel is rejected at launch: "cluster misconfiguration").
-template <bool PAIR>
-__global__ void __launch_bounds__(kConvThreads, 1)
-conv_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-                 const __grid_constant__ CUtensorMap map_d, const __grid_constant__ CUtensorMap map_d2,
-                 const __grid_constant__ CUtensorMap map_r, const __grid_constant__ ConvParams p,
-                 const float* __restrict__ bias, const uint16_t* __restrict__ residual, const float* __restrict__ post_scale,
-                 const float* __restrict__ post_shift) {
-    extern __shared__ unsigned char conv_smem_raw[];
-    __shared__ __align__(8) uint64_t full_bar[kConvMaxStages], empty_bar[kConvMaxStages], acc_full[2], acc_empty[2];
-    __shared__ __align__(8) uint64_t res_bar[2];          // residual tile landed in the staging buffer (one per epilogue group)
-    __shared__ __align__(16) float cst[2][3][64];         // per epilogue group: bias / post scale / post shift of the current chunk
-    __shared__ uint32_t tmem_base_slot;
-    const uint32_t smem0 = (smem_u32(conv_smem_raw) + 1023u) & ~1023u;      // SWIZZLE_128B needs 1024-byte alignment
-    const int stage_b = (p.pair ? p.BN / 2 : p.BN) * 128;                   // pair: half of the weight tile per CTA
-    const uint32_t stage_a = (uint32_t)(p.MT * kConvStageA);
-    const uint32_t stage_bytes = stage_a + (uint32_t)stage_b;
-    const uint32_t acc_cols = (uint32_t)(p.MT * p.BN);                      // TMEM columns of one accumulator stage
-    const uint32_t store0 = smem0 + (uint32_t)p.stages * stage_bytes;       // two staging buffers for the TMA store
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int crank = p.cluster > 1 ? (int)cluster_rank() : 0;
-    const uint16_t cmask = (uint16_t)((1u << p.cluster) - 1u);
-    const int cid = blockIdx.x / p.cluster, nclusters = gridDim.x / p.cluster;
-    const int num_groups = p.m_groups * p.n_blocks;
+// one output element pair (channels co, co + 1) of pixel row `off` (elements): fp32 -> dtype, clipped at Cout
+__device__ __forceinline__ void store_pair(uint16_t* base, long long off, int co, int cout, float a, float b, int is_bf16) {
+    const uint32_t w = pack2(a, b, is_bf16);
+    if (co + 1 < cout) *reinterpret_cast<uint32_t*>(base + off + co) = w;
+    else base[off + co] = (uint16_t)(w & 0xffffu);
+}
 
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(&map_a); tma_prefetch_desc(&map_b); tma_prefetch_desc(&map_d);
-        if (p.dual) tma_prefetch_desc(&map_d2);
-        if (residual != nullptr) tma_prefetch_desc(&map_r);
-        // a stage is free when the MMAs of EVERY CTA of the cluster have read it (peers multicast into it)
-        for (int s = 0; s < p.stages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], p.pair ? 1u : (uint32_t)p.cluster); }
-        // pair: the leader's MMA thread waits for the epilogues of BOTH CTAs (the peer's threads arrive remotely)
-        for (int s = 0; s < 2; ++s) { mbar_init(&acc_full[s], 1); mbar_init(&acc_empty[s], p.pair ? 512u : 256u); mbar_init(&res_bar[s], 1); }
+template <int BN, bool BF16>
+__global__ void __launch_bounds__(kConvThreads, 1)
+conv_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const __grid_constant__ ConvParams p,
+                 const float* __restrict__ bias, const uint16_t* __restrict__ residual, const float* __restrict__ post_scale,
+                 const float* __restrict__ post_shift, uint16_t* __restrict__ y, uint16_t* __restrict__ y2) {
+    extern __shared__ unsigned char conv_smem_raw[];
+    __shared__ __align__(8) uint64_t full_bar[kConvMaxStages], empty_bar[kConvMaxStages];
+    const uint32_t smem0 = (smem_u32(conv_smem_raw) + 1023u) & ~1023u;      // SWIZZLE_128B needs 1024-byte alignment
+    constexpr uint32_t stage_bytes = (uint32_t)(kConvStageA + BN * 128);
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < p.stages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }   // one arrive per consumer warpgroup
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         fence_proxy_async();
     }
-    if (warp == 2) {   // TMEM: 512 columns = two accumulator stages of up to 256 columns (pair: the same warp of both CTAs)
-        if constexpr (PAIR) {
-            asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_slot)), "r"(512u) : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-        } else {
-            asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_slot)), "r"(512u) : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-        }
-    }
-    tc_fence_before();
-    if (p.cluster > 1) cluster_sync_all(); else __syncthreads();     // barrier inits visible cluster-wide before any remote arrive
-    tc_fence_after();
-    const uint32_t tmem_base = tmem_base_slot;
+    __syncthreads();
     const int ksteps = p.taps_x * p.taps_y * p.Cin_chunks;
 
-    if (warp == 0) {
+    if (warp == 8) {
         // ===================== TMA producer =====================
-        if (elect_one()) {
+        if (lane == 0) {
+            tma_prefetch_desc(&map_a); tma_prefetch_desc(&map_b);
             int stage = 0; uint32_t phase = 0;
-            const int slice_rows = p.BN / p.cluster;
-            for (int g = cid; g < num_groups; g += nclusters) {
-                const TileCoord c = decode_tile(p, g, crank);
-                // pair: this CTA stages sub-tile `crank` of the patch
+            for (int g = blockIdx.x; g < p.num_tiles; g += gridDim.x) {
+                const TileCoord c = decode_tile(p, g);
                 // up2: output parity (py, px) shifts the 2x2 window by one low-resolution pixel and selects its 4 folded taps
-                const int par = p.up2 ? (c.img & 3) : 0;
-                const int img = p.up2 ? (c.img >> 2) : c.img;
-                const int x0 = (c.px * p.BW + (p.pair ? crank * p.MT * p.sub_dx : 0)) * p.stride - p.pad_left + (par & 1);
-                const int y0 = (c.py * p.BH + (p.pair ? crank * p.MT * p.sub_dy : 0)) * p.stride - p.pad_top + (par >> 1);
+                const int par = p.up2 ? c.img : 0;
+                const int img = p.up2 ? 0 : c.img;
+                const int x0 = c.px * p.BW * p.stride - p.pad_left + (par & 1);
+                const int y0 = c.py * p.BH * p.stride - p.pad_top + (par >> 1);
                 int tap = par * 4;
                 for (int ty = 0; ty < p.taps_y; ++ty)
                     for (int tx = 0; tx < p.taps_x; ++tx, ++tap)
                         for (int kc = 0; kc < p.Cin_chunks; ++kc) {
                             mbar_wait(&empty_bar[stage], phase ^ 1u);
                             const uint32_t sa = smem0 + (uint32_t)stage * stage_bytes;
-                            if constexpr (PAIR) {
-                                // both CTAs' copies complete on the leader's barrier, which expects the bytes of the pair
-                                const uint32_t lbar = smem_u32(&full_bar[stage]) & kPeerBitMask;
-                                if (crank == 0) mbar_arrive_expect_tx(&full_bar[stage], 2u * stage_bytes);
-                                tma_load_4d_2sm(sa, &map_a, kc * kConvBK, x0 + tx, y0 + ty, img, lbar);
-                                tma_load_3d_2sm(sa + stage_a, &map_b, kc * kConvBK, c.nb * p.BN + crank * (p.BN / 2), tap, lbar);
-                                if (++stage == p.stages) { stage = 0; phase ^= 1u; }
-                                continue;
-                            }
                             mbar_arrive_expect_tx(&full_bar[stage], stage_bytes);
-                            if constexpr (!PAIR) {
-                                tma_load_4d(sa, &map_a, kc * kConvBK, x0 + tx, y0 + ty, img, &full_bar[stage]);
-                                if (p.cluster == 1)
-                                    tma_load_3d_u32(sa + stage_a, &map_b, kc * kConvBK, c.nb * p.BN, tap, &full_bar[stage]);
-                                else
-                                    tma_load_3d_mcast(sa + stage_a + (uint32_t)(crank * slice_rows * 128), &map_b, kc * kConvBK,
-                                                      c.nb * p.BN + crank * slice_rows, tap, &full_bar[stage], cmask);
-                                if (++stage == p.stages) { stage = 0; phase ^= 1u; }
-                            }
+                            tma_load_4d(sa, &map_a, kc * kConvBK, x0 + tx, y0 + ty, img, &full_bar[stage]);
+                            tma_load_3d_u32(sa + kConvStageA, &map_b, kc * kConvBK, c.nb * BN, tap, &full_bar[stage]);
+                            if (++stage == p.stages) { stage = 0; phase ^= 1u; }
                         }
             }
         }
-    } else if (warp == 1 && (!p.pair || crank == 0)) {
-        // ===================== MMA issuer (one thread; pair: of the leader CTA) =====================
-        if (elect_one()) {
-            const uint32_t idesc = umma_idesc(p.BN, p.is_bf16, p.pair ? 2 * kConvBM : kConvBM);
-            int stage = 0; uint32_t phase = 0;
-            int as = 0; uint32_t aphase = 0;
-            for (int g = cid; g < num_groups; g += nclusters) {
-                mbar_wait(&acc_empty[as], aphase ^ 1u);              // epilogue has drained this accumulator stage
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)as * acc_cols;
-                for (int ks = 0; ks < ksteps; ++ks) {
-                    mbar_wait(&full_bar[stage], phase);
-                    tc_fence_after();
-                    const uint32_t sa = smem0 + (uint32_t)stage * stage_bytes;
-                    const uint64_t db = umma_desc_sw128(sa + stage_a);
-                    for (int mt = 0; mt < p.MT; ++mt) {             // the sub-tiles of the patch share this k-step's weight tile
-                        const uint64_t da = umma_desc_sw128(sa + (uint32_t)(mt * kConvStageA));
-#pragma unroll
-                        for (int k = 0; k < kConvBK / 16; ++k) {    // +32 bytes along K inside the swizzle row = +2 in the address field
-                            if constexpr (PAIR) tc_mma_f16_2sm(d_tmem + (uint32_t)(mt * p.BN), da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), idesc, (ks | k) != 0 ? 1u : 0u);
-                            else tc_mma_f16(d_tmem + (uint32_t)(mt * p.BN), da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), idesc, (ks | k) != 0 ? 1u : 0u);
-                        }
-                    }
-                    if constexpr (PAIR) tc_commit_2sm_mcast(&empty_bar[stage], 3);   // frees the stage in both CTAs of the pair
-                    else {
-                        if (p.cluster == 1) tc_commit(&empty_bar[stage]);   // frees the smem stage when these MMAs have read it
-                        else tc_commit_mcast(&empty_bar[stage], cmask);     // ... in every CTA of the cluster
-                    }
-                    if (++stage == p.stages) { stage = 0; phase ^= 1u; }
-                }
-                if constexpr (PAIR) tc_commit_2sm_mcast(&acc_full[as], 3);   // accumulators of both CTAs complete -> both epilogues
-                else tc_commit(&acc_full[as]);                               // accumulator complete -> epilogue
-                if (++as == p.acc_stages) { as = 0; aphase ^= 1u; }
-            }
-        }
-    } else if (warp >= 4) {
-        // ===================== epilogue: TMEM -> registers -> smem -> TMA store =====================
-        // Two groups of four warps (TMEM lane quarters 0-3 each) split the (sub-tile, 64-column chunk) units of a tile
-        // between them: with one group the epilogue of a 256 x 128 tile (TMEM -> fma / residual / SiLU -> fp16 -> smem)
-        // took longer than its MMAs whenever K is short (128 -> 128 3x3: 13.8 us against 9.8 us, measured per tile)
-        const int q = warp & 3;                       // TMEM lane quarter of this warp
-        const int eg = (warp - 4) >> 2;               // epilogue group
-        const int row = q * 32 + lane;                // accumulator row = pixel index inside the tile
-        const int et = (threadIdx.x - 128) & 127;     // 0..127 inside the group
-        const int bar_id = 1 + eg;
-        const uint32_t sbuf = store0 + (uint32_t)eg * kConvStoreBuf;   // one staging buffer per group
-        const uint32_t sbuf2 = store0 + (uint32_t)(2 + eg) * kConvStoreBuf;   // ... and one more for the second output (dual)
-        int as = 0; uint32_t aphase = 0;
-        uint32_t rphase = 0;                          // parity of this group's residual-load barrier
-        const bool has_res = residual != nullptr;
-        for (int g = cid; g < num_groups; g += nclusters) {
-            const TileCoord c = decode_tile(p, g, crank);
-            mbar_wait(&acc_full[as], aphase);
-            tc_fence_after();
-            const int nchunks = p.BN / p.chunk_cols;
-            const int units = p.MT * nchunks;
-            const int last_u = units - 1 - ((units - 1 - eg) & 1);      // this group's last unit (< eg: none)
-            if (last_u < eg) {                                          // nothing to read: hand the stage straight back
-                tc_fence_before();
-                if (p.pair) mbar_arrive_cluster(smem_u32(&acc_empty[as]) & kPeerBitMask);
-                else mbar_arrive(&acc_empty[as]);
-            }
-            for (int u = eg; u < units; u += 2) {
-                const int mt0 = u / nchunks, ch = u - mt0 * nchunks;
-                {
-                const int mt = p.pair ? crank * p.MT + mt0 : mt0;   // pair: this CTA holds sub-tiles [crank * MT, (crank + 1) * MT) of the patch
-                const int pidx = mt * kConvBM + row;          // pixel index inside the patch (= shared-memory row of the A box)
-                const int ly = pidx / p.BW, lx = pidx - ly * p.BW;
-                const int ox = c.px * p.BW + lx, oy = c.py * p.BH + ly;
-                const bool pix_ok = ox < p.OW && oy < p.OH && c.img < p.NI;
-                const long long pix = ((long long)c.img * p.OH + oy) * p.OW + ox;
-                {
-                    const int col0 = c.nb * p.BN + ch * p.chunk_cols;
-                    const int ng = p.chunk_cols / 16;
-                    const int sx = c.px * p.BW + mt * p.sub_dx, sy = c.py * p.BH + mt * p.sub_dy;
-                    // the group's staging buffer must have been read by its previous TMA store; then the residual tile of this
-                    // unit is fetched INTO it by TMA (same box, same swizzle as the output: every thread later reads and
-                    // overwrites only its own row) -- per-thread 128-byte global loads of a row-per-thread layout cost 32 L1
-                    // requests per instruction and were the longest stall of the residual epilogue
-                    if (et == 0) {
-                        bulk_wait_read<0>();
-                        if (has_res) {
-                            mbar_arrive_expect_tx(&res_bar[eg], (uint32_t)(kConvBM * p.chunk_cols * 2));
-                            tma_load_4d(sbuf, &map_r, col0, sx, sy, c.img, &res_bar[eg]);
-                        }
-                    }
-                    // per-channel constants of the chunk -> shared memory, once per unit instead of once per thread and group:
-                    // threads 0-15 bias, 16-31 post scale, 32-47 post shift (4 channels each; 0 / 1 / 0 where absent)
-                    if (et < 48 && (et & 15) * 4 < p.chunk_cols) {
-                        const int kind = et >> 4, c4 = (et & 15) * 4;
-                        const float* src = kind == 0 ? ((bias != nullptr && !p.bias_per_row) ? bias : nullptr) : (kind == 1 ? post_scale : post_shift);
-                        float4 val = kind == 1 ? make_float4(1.f, 1.f, 1.f, 1.f) : make_float4(0.f, 0.f, 0.f, 0.f);
-                        if (src != nullptr) {
-                            const int cc = col0 + c4;
-                            if (cc + 4 <= p.Cout) val = __ldg(reinterpret_cast<const float4*>(src + cc));
-                            else {
-                                if (cc + 0 < p.Cout) val.x = __ldg(src + cc + 0);
-                                if (cc + 1 < p.Cout) val.y = __ldg(src + cc + 1);
-                                if (cc + 2 < p.Cout) val.z = __ldg(src + cc + 2);
-                            }
-                        }
-                        *reinterpret_cast<float4*>(&cst[eg][kind][c4]) = val;
-                    }
-                    // all TMEM loads of the chunk in flight before the single wait (up to 64 columns = 64 registers)
-                    uint32_t racc[4][16];
-                    __syncwarp();
-                    const uint32_t tcol = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)as * acc_cols + (uint32_t)(mt0 * p.BN + ch * p.chunk_cols);
-                    tc_ld16(tcol, racc[0]);
-                    if (ng > 1) tc_ld16(tcol + 16u, racc[1]);
-                    if (ng > 2) { tc_ld16(tcol + 32u, racc[2]); tc_ld16(tcol + 48u, racc[3]); }
-                    named_bar_sync(bar_id, 128);          // constants visible; staging buffer known free
-                    if (has_res) { mbar_wait(&res_bar[eg], rphase); rphase ^= 1u; }
-                    tc_wait_ld();
-#pragma unroll
-                    for (int g16 = 0; g16 < 4; ++g16) {
-                        if (g16 >= ng) break;
-                        const uint32_t (&r)[16] = racc[g16];
-                        float v[16];
-                        const int cb = col0 + g16 * 16;
-                        // shared-memory addresses of this thread's two 16-byte pieces of the group (output staging layout)
-                        uint32_t a0, a1;
-                        if (p.chunk_cols == 64) {      // 128-byte rows, 128-byte swizzle: chunk index XOR (row & 7)
-                            a0 = (uint32_t)row * 128u + ((uint32_t)((2 * g16) ^ (row & 7)) << 4);
-                            a1 = (uint32_t)row * 128u + ((uint32_t)((2 * g16 + 1) ^ (row & 7)) << 4);
-                        } else {                       // narrow outputs: dense rows of chunk_cols * 2 bytes, no swizzle
-                            a0 = (uint32_t)row * (uint32_t)(p.chunk_cols * 2) + (uint32_t)g16 * 32u;
-                            a1 = a0 + 16u;
-                        }
-                        if (p.bias_per_row) {
-                            const float bb = (bias != nullptr && pix_ok) ? __ldg(bias + pix) : 0.0f;
-#pragma unroll
-                            for (int j = 0; j < 16; ++j) v[j] = __fmaf_rn(__uint_as_float(r[j]), p.alpha, bb);
-                        } else {
-#pragma unroll
-                            for (int j4 = 0; j4 < 4; ++j4) {
-                                const float4 b4 = *reinterpret_cast<const float4*>(&cst[eg][0][g16 * 16 + 4 * j4]);
-                                v[4 * j4 + 0] = __fmaf_rn(__uint_as_float(r[4 * j4 + 0]), p.alpha, b4.x);
-                                v[4 * j4 + 1] = __fmaf_rn(__uint_as_float(r[4 * j4 + 1]), p.alpha, b4.y);
-                                v[4 * j4 + 2] = __fmaf_rn(__uint_as_float(r[4 * j4 + 2]), p.alpha, b4.z);
-                                v[4 * j4 + 3] = __fmaf_rn(__uint_as_float(r[4 * j4 + 3]), p.alpha, b4.w);
-                            }
-                        }
-                        if (has_res) {
-                            uint32_t rw[8];
-                            asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(rw[0]), "=r"(rw[1]), "=r"(rw[2]), "=r"(rw[3]) : "r"(sbuf + a0) : "memory");
-                            asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(rw[4]), "=r"(rw[5]), "=r"(rw[6]), "=r"(rw[7]) : "r"(sbuf + a1) : "memory");
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) {
-                                v[2 * j] += unpack_lo(rw[j], p.is_bf16);
-                                v[2 * j + 1] += unpack_hi(rw[j], p.is_bf16);
-                            }
-                        }
-                        if (p.dual) {   // the unnormalised result goes out as well (next block's shortcut / residual source)
-                            uint32_t o1[8];
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) o1[j] = pack2(v[2 * j], v[2 * j + 1], p.is_bf16);
-                            asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(sbuf + a0), "r"(o1[0]), "r"(o1[1]), "r"(o1[2]), "r"(o1[3]) : "memory");
-                            asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(sbuf + a1), "r"(o1[4]), "r"(o1[5]), "r"(o1[6]), "r"(o1[7]) : "memory");
-                        }
-                        if (post_scale != nullptr) {
-                            // the GroupNorm (+ SiLU) that follows this convolution, statistics frozen (fast mode):
-                            // y = act(v * scale[c] + shift[c]) on the fp32 accumulator, before the one rounding to fp16
-#pragma unroll
-                            for (int j4 = 0; j4 < 4; ++j4) {
-                                const float4 sc = *reinterpret_cast<const float4*>(&cst[eg][1][g16 * 16 + 4 * j4]);
-                                const float4 sh = *reinterpret_cast<const float4*>(&cst[eg][2][g16 * 16 + 4 * j4]);
-                                v[4 * j4 + 0] = __fmaf_rn(v[4 * j4 + 0], sc.x, sh.x);
-                                v[4 * j4 + 1] = __fmaf_rn(v[4 * j4 + 1], sc.y, sh.y);
-                                v[4 * j4 + 2] = __fmaf_rn(v[4 * j4 + 2], sc.z, sh.z);
-                                v[4 * j4 + 3] = __fmaf_rn(v[4 * j4 + 3], sc.w, sh.w);
-                            }
-                            if (p.post_act) {
-#pragma unroll
-                                for (int j = 0; j < 16; ++j) v[j] = __fdividef(v[j], 1.0f + __expf(-v[j]));
-                            }
-                        }
-                        uint32_t o[8];
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) o[j] = pack2(v[2 * j], v[2 * j + 1], p.is_bf16);
-                        const uint32_t sdst = p.dual ? sbuf2 : sbuf;
-                        asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(sdst + a0), "r"(o[0]), "r"(o[1]), "r"(o[2]), "r"(o[3]) : "memory");
-                        asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(sdst + a1), "r"(o[4]), "r"(o[5]), "r"(o[6]), "r"(o[7]) : "memory");
-                    }
-                    if (u == last_u) {   // this group's TMEM reads of the accumulator stage are done: hand it back
-                        tc_fence_before();
-                        if (p.pair) mbar_arrive_cluster(smem_u32(&acc_empty[as]) & kPeerBitMask);   // on the leader's barrier
-                        else mbar_arrive(&acc_empty[as]);
-                    }
-                    fence_proxy_async();
-                    named_bar_sync(bar_id, 128);
-                    if (et == 0) {
-                        if (c.img < p.NI) {
-                            if (p.up2) tma_store_5d(&map_d, col0, sx, sy, c.img & 1, c.img >> 1, sbuf);
-                            else tma_store_4d(&map_d, col0, sx, sy, c.img, sbuf);
-                            if (p.dual) {
-                                if (p.up2) tma_store_5d(&map_d2, col0, sx, sy, c.img & 1, c.img >> 1, sbuf2);
-                                else tma_store_4d(&map_d2, col0, sx, sy, c.img, sbuf2);
-                            }
-                        }
-                        bulk_commit();
-                    }
-                }
-                }
-            }
-            if (++as == p.acc_stages) { as = 0; aphase ^= 1u; }
-        }
-        if (et == 0) bulk_wait_all();
+        return;
     }
-    tc_fence_before();
-    if (p.cluster > 1) cluster_sync_all(); else __syncthreads();     // no CTA leaves while a peer may still write into it
-    if (warp == 2) {
-        tc_fence_after();
-        if constexpr (PAIR) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
-        else asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
+
+    // ===================== consumers: wgmma into registers, then the epilogue =====================
+    const int wg = warp >> 2;                 // rows [64 wg, 64 wg + 64) of the tile
+    const bool signal = (threadIdx.x & 127) == 0;
+    float acc[BN / 2];
+    int stage = 0; uint32_t phase = 0;
+    for (int g = blockIdx.x; g < p.num_tiles; g += gridDim.x) {
+        const TileCoord c = decode_tile(p, g);
+        int prev = -1;
+        for (int ks = 0; ks < ksteps; ++ks) {
+            mbar_wait(&full_bar[stage], phase);
+            const uint32_t sa = smem0 + (uint32_t)stage * stage_bytes;
+            const uint64_t da = wgmma_desc_sw128(sa + (uint32_t)(wg * 64 * 128));
+            const uint64_t db = wgmma_desc_sw128(sa + kConvStageA);
+            wgmma_fence_acc(acc);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < kConvBK / 16; ++k) {    // +32 bytes along K inside the swizzle row = +2 in the address field
+                Wgmma<BN, BF16>::mma(acc, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (ks | k) != 0 ? 1u : 0u);
+            }
+            wgmma_commit();
+            wgmma_wait<1>();                          // the previous k-step's MMAs have read their stage: hand it back
+            wgmma_fence_acc(acc);
+            if (prev >= 0 && signal) mbar_arrive(&empty_bar[prev]);
+            prev = stage;
+            if (++stage == p.stages) { stage = 0; phase ^= 1u; }
+        }
+        wgmma_wait<0>();
+        wgmma_fence_acc(acc);
+        if (signal) mbar_arrive(&empty_bar[prev]);
+
+        // accumulator rows of this thread: r0 and r0 + 8; columns 8 j + 2 (lane % 4) + {0, 1}
+        const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+        const int cq = 2 * (lane & 3);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int row = r0 + 8 * h;
+            const int ly = row / p.BW, lx = row - ly * p.BW;
+            const int ox = c.px * p.BW + lx, oy = c.py * p.BH + ly;
+            if (ox >= p.OW || oy >= p.OH || c.img >= p.NI) continue;
+            const long long pix = ((long long)c.img * p.OH + oy) * p.OW + ox;
+            // output pixel: the parity view of the 2x-upsampled image when up2 (one image, N = 1), else the tile pixel
+            const long long opix = p.up2 ? (long long)(2 * oy + (c.img >> 1)) * (2 * p.OW) + 2 * ox + (c.img & 1) : pix;
+            const float bb = (bias != nullptr && p.bias_per_row) ? __ldg(bias + pix) : 0.0f;
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+                const int co = c.nb * BN + 8 * j + cq;
+                if (co >= p.Cout) continue;
+                const bool two = co + 1 < p.Cout;
+                float b0 = bb, b1 = bb;
+                if (bias != nullptr && !p.bias_per_row) { b0 = __ldg(bias + co); b1 = two ? __ldg(bias + co + 1) : 0.0f; }
+                float v0 = __fmaf_rn(acc[4 * j + 2 * h], p.alpha, b0);
+                float v1 = __fmaf_rn(acc[4 * j + 2 * h + 1], p.alpha, b1);
+                if (residual != nullptr) {
+                    const uint16_t* rp = residual + pix * p.res_pitch + co;
+                    const uint32_t rw = two ? __ldg(reinterpret_cast<const unsigned int*>(rp)) : (uint32_t)__ldg(reinterpret_cast<const unsigned short*>(rp));
+                    v0 += unpack_lo(rw, p.is_bf16);
+                    v1 += unpack_hi(rw, p.is_bf16);
+                }
+                if (y2 != nullptr) store_pair(y, opix * p.y_pitch, co, p.Cout, v0, v1, p.is_bf16);   // the unnormalised result
+                if (post_scale != nullptr) {
+                    // the GroupNorm (+ SiLU) that follows this convolution, statistics frozen (fast mode):
+                    // y = act(v * scale[c] + shift[c]) on the fp32 accumulator, before the one rounding to fp16
+                    v0 = __fmaf_rn(v0, __ldg(post_scale + co), __ldg(post_shift + co));
+                    if (two) v1 = __fmaf_rn(v1, __ldg(post_scale + co + 1), __ldg(post_shift + co + 1));
+                    if (p.post_act) {
+                        v0 = __fdividef(v0, 1.0f + __expf(-v0));
+                        v1 = __fdividef(v1, 1.0f + __expf(-v1));
+                    }
+                }
+                if (y2 != nullptr) store_pair(y2, opix * p.y2_pitch, co, p.Cout, v0, v1, p.is_bf16);
+                else store_pair(y, opix * p.y_pitch, co, p.Cout, v0, v1, p.is_bf16);
+            }
+        }
     }
 }
 
@@ -587,6 +277,11 @@ int encode_map(CUtensorMap* out, const void* base, int is_bf16, int rank, const 
     return TD_OK;
 }
 
+template <int BN> bool conv_smem_optin(int bytes) {
+    return cudaFuncSetAttribute(conv_gemm_kernel<BN, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) == cudaSuccess &&
+           cudaFuncSetAttribute(conv_gemm_kernel<BN, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) == cudaSuccess;
+}
+
 struct ConvDev { int sms; int smem_optin; bool ok; };
 ConvDev conv_dev() {
     static std::mutex mu;
@@ -601,11 +296,11 @@ ConvDev conv_dev() {
                cudaDeviceGetAttribute(&d.smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) == cudaSuccess;
         if (d.ok) {   // the opt-in limit covers static + dynamic shared memory: leave room for the kernel's static part
             cudaFuncAttributes fa;
-            if (cudaFuncGetAttributes(&fa, conv_gemm_kernel<false>) != cudaSuccess) { cudaGetLastError(); d.ok = false; }
+            if (cudaFuncGetAttributes(&fa, conv_gemm_kernel<256, false>) != cudaSuccess) { cudaGetLastError(); d.ok = false; }
             else {
                 d.smem_optin -= (int)fa.sharedSizeBytes;
-                if (cudaFuncSetAttribute(conv_gemm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, d.smem_optin) != cudaSuccess ||
-                    cudaFuncSetAttribute(conv_gemm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, d.smem_optin) != cudaSuccess) {
+                if (!conv_smem_optin<16>(d.smem_optin) || !conv_smem_optin<32>(d.smem_optin) || !conv_smem_optin<64>(d.smem_optin) ||
+                    !conv_smem_optin<128>(d.smem_optin) || !conv_smem_optin<256>(d.smem_optin)) {
                     cudaGetLastError();
                     d.ok = false;
                 }
@@ -659,71 +354,33 @@ int conv_run(const td_conv_desc* d, const void* x, const void* w, const float* b
     p.Cout = d->Cout;
     int bn = 256;
     if (d->Cout < 256) { bn = 16; while (bn < d->Cout) bn *= 2; }
-    p.BN = bn;
     p.n_blocks = (d->Cout + bn - 1) / bn;
-    // pixel sub-tile (128 pixels = UMMA M): wide for a GEMM (H == 1), 16 x 8 for images; MT sub-tiles per CTA tile
-    if (gOH == 1) { p.BWs = 128; p.BHs = 1; p.sub_dx = 128; p.sub_dy = 0; }
-    else if (gOW >= 16) { p.BWs = 16; p.BHs = 8; p.sub_dx = 0; p.sub_dy = 8; }
-    else { p.BWs = 8; p.BHs = 16; p.sub_dx = 0; p.sub_dy = 16; }
-    {
-        const char* fm = getenv("TD_CONV_MT");
-        const int want_mt = fm != nullptr ? atoi(fm) : 2;
-        const long long sub_tiles = (long long)gN * ((gOW + p.BWs - 1) / p.BWs) * ((gOH + p.BHs - 1) / p.BHs) * p.n_blocks;
-        // two sub-tiles per CTA when the grid stays full (>= 4 sub-tiles per SM) and the box fits (<= 256 per dimension)
-        // ... and while two accumulator stages still fit in TMEM (BN <= 128): with one stage the epilogue no longer overlaps
-        // the next tile's MMAs (measured: 256 -> 256 at 472^2 drops from 1309 to 1110 TFLOP/s, 128 -> 128 at 944^2 rises
-        // from 859 to 1035); TD_CONV_MT=3 forces two sub-tiles for any BN (measurement only)
-        const bool fits2 = 2 * 2 * bn <= 512 || want_mt >= 3;
-        p.MT = (want_mt >= 2 && fits2 && sub_tiles >= 4LL * dev.sms && bn >= 32 && (p.BWs + p.sub_dx) * d->stride <= 256 && (p.BHs + p.sub_dy) * d->stride <= 256) ? 2 : 1;
-    }
-    // CTA pair (tcgen05.mma.cta_group::2): the two CTAs of a cluster take halves of ONE patch (MT sub-tiles each) and half
-    // of the weight tile each (TD_CONV_PAIR=0 disables)
-    {
-        const char* fp = getenv("TD_CONV_PAIR");
-        const int want_pair = fp != nullptr ? atoi(fp) : 1;
-        const long long sub_tiles = (long long)gN * ((gOW + p.BWs - 1) / p.BWs) * ((gOH + p.BHs - 1) / p.BHs) * p.n_blocks;
-        p.pair = (want_pair >= 1 && bn >= 128 && dev.sms % 2 == 0 && sub_tiles >= 4LL * p.MT * dev.sms) ? 1 : 0;
-    }
-    const int patch_subs = p.MT * (p.pair ? 2 : 1);             // sub-tiles per patch
-    p.BW = p.BWs + (patch_subs - 1) * p.sub_dx;
-    p.BH = p.BHs + (patch_subs - 1) * p.sub_dy;
-    p.acc_stages = std::min(2, 512 / (p.MT * bn));
+    // pixel tile (128 pixels): wide for a GEMM (H == 1), 16 x 8 for images, 8 x 16 for narrow ones
+    if (gOH == 1) { p.BW = 128; p.BH = 1; }
+    else if (gOW >= 16) { p.BW = 16; p.BH = 8; }
+    else { p.BW = 8; p.BH = 16; }
     p.tiles_x = (gOW + p.BW - 1) / p.BW;
     p.tiles_y = (gOH + p.BH - 1) / p.BH;
     const long long mt = (long long)gN * p.tiles_x * p.tiles_y;
     if (mt * p.n_blocks > 0x3fffffffLL) { td_set_error("td_conv2d_nhwc: too many tiles"); return TD_ERR_UNSUPPORTED; }
-    p.m_tiles = (int)mt;
-    // CTA clusters: the weight tile of a k-step is fetched once per cluster (each CTA loads BN / cluster rows and
-    // multicasts them) -- the kernel is bound by L2 -> SM bytes otherwise (48 KB per 128x256x64 MMA step per CTA)
-    int cl = 1;
-    const char* force = getenv("TD_CONV_CLUSTER");
-    const int want = force != nullptr ? atoi(force) : 1;   // measured: no gain on B200 (the bound is bytes INTO the SM, which multicast does not cut)
-    if (want >= 2 && bn >= 64 && dev.sms % 2 == 0 && mt >= 2 * (long long)dev.sms) cl = 2;
-    if (want >= 4 && bn >= 128 && dev.sms % 4 == 0 && mt >= 4 * (long long)dev.sms) cl = 4;
-    if (p.pair) cl = 2;
-    p.cluster = cl;
-    p.m_groups = p.pair ? (int)mt : (int)((mt + cl - 1) / cl);
-    p.num_tiles = p.m_groups * p.n_blocks;
-    p.chunk_cols = std::min(64, bn);
+    p.num_tiles = (int)(mt * p.n_blocks);
     p.is_bf16 = d->dtype == TD_BF16;
     p.bias_per_row = d->bias_per_row;
     p.post_act = d->post_act;
     p.alpha = d->alpha;
+    p.y_pitch = d->y_pitch;
+    p.y2_pitch = d->y2 != nullptr ? d->y2_pitch : 0;
     p.res_pitch = residual != nullptr ? d->res_pitch : 0;
-    p.dual = d->y2 != nullptr ? 1 : 0;
-    const int n_store_bufs = p.dual ? 4 : 2;
-    const int stage_bytes = p.MT * kConvStageA + (p.pair ? bn / 2 : bn) * 128;
-    const int avail = dev.smem_optin - 1024 - n_store_bufs * kConvStoreBuf;
-    p.stages = std::min(kConvMaxStages, avail / stage_bytes);
+    const int stage_bytes = kConvStageA + bn * 128;
+    p.stages = std::min(kConvMaxStages, (dev.smem_optin - 1024) / stage_bytes);
     if (p.stages < 2) { td_set_error("td_conv2d_nhwc: not enough shared memory"); return TD_ERR_UNSUPPORTED; }
-    const size_t smem = (size_t)p.stages * stage_bytes + n_store_bufs * kConvStoreBuf + 1024;
+    const size_t smem = (size_t)p.stages * stage_bytes + 1024;
 
-    alignas(64) CUtensorMap ma, mb, md, md2;
+    alignas(64) CUtensorMap ma, mb;
     {
         const uint64_t dims[4] = {(uint64_t)d->Cin, (uint64_t)d->W, (uint64_t)d->H, (uint64_t)d->N};
         const uint64_t str[3] = {(uint64_t)d->x_pitch * 2, (uint64_t)d->W * d->x_pitch * 2, (uint64_t)d->H * d->W * d->x_pitch * 2};
-        // one box = the MT sub-tiles of one CTA (a pair's patch holds two of them)
-        const uint32_t box[4] = {64, (uint32_t)((p.BWs + (p.MT - 1) * p.sub_dx) * d->stride), (uint32_t)((p.BHs + (p.MT - 1) * p.sub_dy) * d->stride), 1};
+        const uint32_t box[4] = {64, (uint32_t)(p.BW * d->stride), (uint32_t)(p.BH * d->stride), 1};
         const uint32_t es[4] = {1, (uint32_t)d->stride, (uint32_t)d->stride, 1};
         const int rc = encode_map(&ma, x, p.is_bf16, 4, dims, str, box, es, true, "activations");
         if (rc != TD_OK) return rc;
@@ -731,60 +388,27 @@ int conv_run(const td_conv_desc* d, const void* x, const void* w, const float* b
     {
         const uint64_t dims[3] = {(uint64_t)d->Cin, (uint64_t)d->Cout, (uint64_t)(up2 ? 16 : d->kh * d->kw)};
         const uint64_t str[2] = {(uint64_t)d->w_pitch * 2, (uint64_t)d->Cout * d->w_pitch * 2};
-        const uint32_t box[3] = {64, (uint32_t)(bn / p.cluster), 1};      // cluster multicast slices and the pair's halves alike
+        const uint32_t box[3] = {64, (uint32_t)bn, 1};
         const uint32_t es[3] = {1, 1, 1};
         const int rc = encode_map(&mb, w, p.is_bf16, 3, dims, str, box, es, true, "weights");
         if (rc != TD_OK) return rc;
     }
-    for (int which = 0; which < (p.dual ? 2 : 1); ++which) {
-        CUtensorMap* mo = which == 0 ? &md : &md2;
-        void* yo = which == 0 ? y : (up2 && d->y2 != nullptr ? (void*)((uint16_t*)d->y2 + y2_off) : d->y2);
-        const uint64_t pitch = (uint64_t)(which == 0 ? d->y_pitch : d->y2_pitch);
-        if (up2) {
-            // y[2 i + py, 2 j + px, c] as {c, j, i, px, py}: the tile of one parity lands on every second pixel of every second row
-            const uint64_t row = (uint64_t)d->OW * pitch * 2;
-            const uint64_t dims[5] = {(uint64_t)d->Cout, (uint64_t)d->W, (uint64_t)d->H, 2, 2};
-            const uint64_t str[4] = {pitch * 4, row * 2, pitch * 2, row};
-            const uint32_t box[5] = {(uint32_t)p.chunk_cols, (uint32_t)p.BWs, (uint32_t)p.BHs, 1, 1};
-            const uint32_t es[5] = {1, 1, 1, 1, 1};
-            const int rc = encode_map(mo, yo, p.is_bf16, 5, dims, str, box, es, p.chunk_cols == 64, "output (parity view)");
-            if (rc != TD_OK) return rc;
-        } else {
-            const uint64_t dims[4] = {(uint64_t)d->Cout, (uint64_t)d->OW, (uint64_t)d->OH, (uint64_t)d->N};
-            const uint64_t str[3] = {pitch * 2, (uint64_t)d->OW * pitch * 2, (uint64_t)d->OH * d->OW * pitch * 2};
-            const uint32_t box[4] = {(uint32_t)p.chunk_cols, (uint32_t)p.BWs, (uint32_t)p.BHs, 1};
-            const uint32_t es[4] = {1, 1, 1, 1};
-            const int rc = encode_map(mo, yo, p.is_bf16, 4, dims, str, box, es, p.chunk_cols == 64, "output");
-            if (rc != TD_OK) return rc;
-        }
+    uint16_t* yo = static_cast<uint16_t*>(y);
+    uint16_t* y2o = d->y2 != nullptr ? static_cast<uint16_t*>(d->y2) + (up2 ? y2_off : 0) : nullptr;
+    const int grid = std::min(p.num_tiles, dev.sms);
+    const uint16_t* res = static_cast<const uint16_t*>(residual);
+    cudaStream_t st = (cudaStream_t)stream;
+#define TD_CONV_LAUNCH(BN)                                                                                                          \
+    (p.is_bf16 ? conv_gemm_kernel<BN, true><<<grid, kConvThreads, smem, st>>>(ma, mb, p, bias, res, d->post_scale, d->post_shift, yo, y2o) \
+               : conv_gemm_kernel<BN, false><<<grid, kConvThreads, smem, st>>>(ma, mb, p, bias, res, d->post_scale, d->post_shift, yo, y2o))
+    switch (bn) {
+        case 16: TD_CONV_LAUNCH(16); break;
+        case 32: TD_CONV_LAUNCH(32); break;
+        case 64: TD_CONV_LAUNCH(64); break;
+        case 128: TD_CONV_LAUNCH(128); break;
+        default: TD_CONV_LAUNCH(256); break;
     }
-    if (!p.dual) md2 = md;
-    alignas(64) CUtensorMap mr = md;
-    if (residual != nullptr) {   // the residual tile is fetched with the output's own box (zero fill outside the tensor)
-        const uint64_t dims[4] = {(uint64_t)d->Cout, (uint64_t)d->OW, (uint64_t)d->OH, (uint64_t)d->N};
-        const uint64_t str[3] = {(uint64_t)d->res_pitch * 2, (uint64_t)d->OW * d->res_pitch * 2, (uint64_t)d->OH * d->OW * d->res_pitch * 2};
-        const uint32_t box[4] = {(uint32_t)p.chunk_cols, (uint32_t)p.BWs, (uint32_t)p.BHs, 1};
-        const uint32_t es[4] = {1, 1, 1, 1};
-        const int rc = encode_map(&mr, residual, p.is_bf16, 4, dims, str, box, es, p.chunk_cols == 64, "residual");
-        if (rc != TD_OK) return rc;
-    }
-    const int grid = std::max(cl, std::min(p.num_tiles * cl, dev.sms) / cl * cl);
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)grid);
-    cfg.blockDim = dim3(kConvThreads);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = (cudaStream_t)stream;
-    cudaLaunchAttribute attr = {};
-    attr.id = cudaLaunchAttributeClusterDimension;
-    attr.val.clusterDim.x = (unsigned)cl;
-    attr.val.clusterDim.y = 1;
-    attr.val.clusterDim.z = 1;
-    cfg.attrs = &attr;
-    cfg.numAttrs = cl > 1 ? 1 : 0;
-    const cudaError_t le = p.pair
-        ? cudaLaunchKernelEx(&cfg, conv_gemm_kernel<true>, ma, mb, md, md2, mr, p, bias, (const uint16_t*)residual, d->post_scale, d->post_shift)
-        : cudaLaunchKernelEx(&cfg, conv_gemm_kernel<false>, ma, mb, md, md2, mr, p, bias, (const uint16_t*)residual, d->post_scale, d->post_shift);
-    if (le != cudaSuccess) { td_set_error("td_conv2d_nhwc: launch failed: %s", cudaGetErrorString(le)); cudaGetLastError(); return TD_ERR_CUDA; }
+#undef TD_CONV_LAUNCH
     const cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { td_set_error("td_conv2d_nhwc: launch failed: %s", cudaGetErrorString(e)); return TD_ERR_CUDA; }
     return TD_OK;

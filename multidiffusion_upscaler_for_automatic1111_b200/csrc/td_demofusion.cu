@@ -1,4 +1,4 @@
-// DemoFusion extras on sm_100a (tile_methods/demofusion.py of the reference):
+// DemoFusion extras on sm_90a (tile_methods/demofusion.py of the reference):
 //
 //   td_dilated_gather      <- x[:, :, by::s, bx::s] views + torch.cat               demofusion.py:283-308
 //   td_demofusion_combine  <- strided `x_global[...] += view`, `/2` (mixture), `/weights`,

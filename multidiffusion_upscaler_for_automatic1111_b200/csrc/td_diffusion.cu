@@ -1,9 +1,9 @@
-// Per-sampler-step hot path of tiled diffusion on sm_100a:
+// Per-sampler-step hot path of tiled diffusion on sm_90a:
 //   scatter  (crop-with-overlap of the latent into the tile batch)      multidiffusion.py:155
 //   blend    (ordered overlap accumulate + normalise, gather form)      multidiffusion.py:166-167,208
 //            (gaussian-weighted, pre-normalised accumulate)             mixtureofdiffusers.py:122-126
 //
-// Design (B200-first, see DESIGN.md):
+// Design (H100-first, see DESIGN.md):
 //   * ONE launch per step for all T tiles (the reference: T/TB cats + T..3T slice-adds).
 //   * Gather form: each thread owns one 16-byte vector of the output canvas and
 //     visits the tiles covering it in ascending tile index, rounding through the
@@ -744,9 +744,9 @@ blend_mod_async_kernel(const __grid_constant__ BlendParams p, const float* __res
 // Persistent, software-pipelined form of the cp.async blend (TD_FLAG_PIPELINE, opt-in): a CTA walks
 // patches pi = blockIdx.x, += gridDim.x with two stage sets -- the copies of patch n+1
 // are in flight while patch n is consumed, normalised and stored, so DRAM stays busy
-// instead of all CTAs of a wave issuing, waiting and computing in lock step.  Measured on B200
-// (cfg2): 13.9 us vs 10.0 us for one-patch-per-CTA -- 15 resident warps per SM and three
-// barriers per patch lose more than the overlap wins -- so it is not the default.
+// instead of all CTAs of a wave issuing, waiting and computing in lock step.  Fewer resident
+// warps per SM and three barriers per patch can cost more than the overlap wins, so it is an
+// opt-in, not the default.
 // ---------------------------------------------------------------------------
 template <typename T, bool WRITE_BUF, bool FASTDIV>
 __global__ void __launch_bounds__(kAsThreads)
@@ -1391,7 +1391,7 @@ void fill_patch_table(const int32_t* org, int n, int extent, int size, int patch
 int sm_count() {
     static int n = [] {
         int dev = 0, v = 0;
-        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 148;
+        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;
         return v;
     }();
     return n;
@@ -1652,7 +1652,7 @@ extern "C" int td_blend_multidiffusion(const td_grid* g, const void* const* batc
                 default: rc = try_launch_blend_tma<float>(g, bp, tile_dtype, weights, x_out, x_buffer, s); break;
             }
         } else if (!(flags & TD_FLAG_NO_TMA)) {
-            const bool pipe = (flags & TD_FLAG_PIPELINE) != 0;   // measured slower on B200 (DESIGN.md); opt-in
+            const bool pipe = (flags & TD_FLAG_PIPELINE) != 0;   // opt-in (see the comment above the kernel)
             switch (tile_dtype) {
                 case TD_F16: rc = try_launch_blend_async<__half>(g, bp, weights, rcp_weights, x_out, x_buffer, pipe, s); break;
                 case TD_BF16: rc = try_launch_blend_async<__nv_bfloat16>(g, bp, weights, rcp_weights, x_out, x_buffer, pipe, s); break;

@@ -43,7 +43,7 @@ int nhwc_sms() {
     if (sms == 0) {
         int dev = 0, n = 0;
         if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess) sms = n;
-        else sms = 148;
+        else sms = 132;
     }
     return sms;
 }

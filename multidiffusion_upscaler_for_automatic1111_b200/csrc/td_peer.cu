@@ -1,5 +1,5 @@
 // Multi-GPU plumbing for the tile-sharded sampler step (one process per GPU):
-//   * exchange buffers that every rank maps from its peers through CUDA IPC (NVLink 5 / NVSwitch P2P),
+//   * exchange buffers that every rank maps from its peers through CUDA IPC (NVLink / NVSwitch P2P),
 //   * a step-counter signal written straight into the peers' flag arrays,
 // so that the blend kernel can wait for its peers and read their tile outputs over NVLink in the
 // SAME kernel that blends them (td_blend_multidiffusion_peer in td_diffusion.cu): no NCCL call, no

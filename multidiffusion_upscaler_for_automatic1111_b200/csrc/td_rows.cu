@@ -1,4 +1,4 @@
-// Row-block form of the per-step hot path (TD_FLAG_ROWS, opt-in -- see the measurements at the end of this comment):
+// Row-block form of the per-step hot path (TD_FLAG_ROWS, opt-in -- see the end of this comment):
 //   scatter                       multidiffusion.py:155, mixtureofdiffusers.py:88,104
 //   blend + normalise (MD)        multidiffusion.py:166-167, :208
 //   blend (Mixture of Diffusers)  mixtureofdiffusers.py:122-126
@@ -20,17 +20,15 @@
 //     canvas), packed add rounded through the canvas dtype; chunks outside the tile are register zeros (x + (+0) is
 //     exact for MultiDiffusion; the Mixture-of-Diffusers form masks per element because its accumulator can be -0);
 //     threads wait for a unit on the CTA barrier (one thread blocks on the mbarrier): no spinning issue slots;
-//   * normalise in registers, one 256-bit store per thread (fp32 output, as the reference).
+//   * normalise in registers, 32 bytes stored per thread (fp32 output, as the reference).
 // Scatter is the mirror image: one bulk copy brings a unit's canvas rows in, threads re-align and write 128-bit
 // vectors into the tile batch.
 //
-// MEASURED on B200 (round 2, BASELINE cfg2, back-to-back launches in a CUDA graph): bit-identical to the default
-// kernels on every fixture, but SLOWER -- blend 20.3 us vs 8.8 us, scatter 7.1 us vs 4.9 us, zero-visit floor 7.3 us
-// vs 3.5 us.  A 200 KB one-CTA-per-SM kernel cannot become resident while its predecessor drains (no programmatic-
-// dependent-launch overlap), pays the full launch -> barrier init -> copy latency -> consume -> store chain once per
-// launch, and the ~100 small (1.3 KB, 16-byte-aligned) bulk copies per SM complete at ~1 TB/s chip-wide (ncu:
-// the consumers sit on the unit mbarrier; L2-hot and HBM-cold runs take the same time).  Kept as an opt-in for
-// geometries with few, large tiles and as the worked example of why the default is many small co-resident CTAs.
+// Bit-identical to the default kernels on every fixture, but a 200 KB one-CTA-per-SM kernel cannot become resident
+// while its predecessor drains (no programmatic-dependent-launch overlap), pays the full launch -> barrier init -> copy
+// latency -> consume -> store chain once per launch, and many small (1.3 KB, 16-byte-aligned) bulk copies per SM are a
+// poor fit for the copy engine.  Kept as an opt-in for geometries with few, large tiles; the default is many small
+// co-resident CTAs.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -83,13 +81,14 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uin
 }
 __device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 
+// 32 bytes per thread as two 128-bit accesses (sm_90 has no 256-bit load / store)
 __device__ __forceinline__ void stg256(float* p, const float (&f)[8]) {
-    asm volatile("st.global.v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "f"(f[0]), "f"(f[1]), "f"(f[2]), "f"(f[3]),
-                 "f"(f[4]), "f"(f[5]), "f"(f[6]), "f"(f[7]) : "memory");
+    asm volatile("st.global.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p), "f"(f[0]), "f"(f[1]), "f"(f[2]), "f"(f[3]) : "memory");
+    asm volatile("st.global.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p + 4), "f"(f[4]), "f"(f[5]), "f"(f[6]), "f"(f[7]) : "memory");
 }
 __device__ __forceinline__ void ldg256(const float* p, float (&f)[8]) {
-    asm volatile("ld.global.nc.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];" : "=f"(f[0]), "=f"(f[1]), "=f"(f[2]), "=f"(f[3]),
-                 "=f"(f[4]), "=f"(f[5]), "=f"(f[6]), "=f"(f[7]) : "l"(p));
+    asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(f[0]), "=f"(f[1]), "=f"(f[2]), "=f"(f[3]) : "l"(p));
+    asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(f[4]), "=f"(f[5]), "=f"(f[6]), "=f"(f[7]) : "l"(p + 4));
 }
 
 template <typename T> __device__ __forceinline__ uint32_t rows_packed_add(uint32_t a, uint32_t b);

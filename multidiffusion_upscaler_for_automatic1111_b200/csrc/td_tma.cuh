@@ -1,10 +1,10 @@
-// TMA (cp.async.bulk.tensor) + mbarrier plumbing for sm_100a, raw PTX.
+// TMA (cp.async.bulk.tensor) + mbarrier plumbing for sm_90a, raw PTX.
 //
 // Why TMA on this path: a CTA needs ~15 clipped sub-boxes of different tiles, and the
 // per-warp chain "load -> wait -> add" of a register-staged kernel serialises DRAM
 // latency.  A tiled tensor map takes signed box coordinates, clips against the tensor
 // extent with zero fill, and keeps every box of the CTA in flight at once with no
-// staging registers.  MEASURED CONSTRAINT (B200, CUDA 12.9): the innermost start
+// staging registers.  CONSTRAINT (CUDA 12.9): the innermost start
 // coordinate must be 16-byte aligned (a misaligned c0 raises "illegal instruction"),
 // so boxes are fetched as the aligned superset [floor(u0/VEC)*VEC, +BX+VEC) and the
 // 2-byte-granular shift is applied when the threads read shared memory.

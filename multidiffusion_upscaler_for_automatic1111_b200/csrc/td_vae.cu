@@ -1,4 +1,4 @@
-// Tiled-VAE hot path on sm_100a (scripts/tilevae.py of the reference):
+// Tiled-VAE hot path on sm_90a (scripts/tilevae.py of the reference):
 //
 //   td_gn_stats        <- get_var_mean            tilevae.py:207-215   one read of the activation
 //   td_gn_apply        <- custom_group_norm       tilevae.py:218-245   } one read + one write

@@ -1,7 +1,7 @@
 """Tensor-level wrappers over the C-ABI kernels (device pointers + current stream).
 
 PyTorch is plumbing here: it owns the memory and the stream; every byte of the
-hot path moves through the hand-written sm_100a kernels in csrc/.
+hot path moves through the hand-written sm_90a kernels in csrc/.
 """
 from __future__ import annotations
 

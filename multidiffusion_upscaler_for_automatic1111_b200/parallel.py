@@ -261,8 +261,8 @@ class StripShard:
 # measurement switches (defaults = the shipped path): TD_STRIP_LATE_WAIT=0 -> every blend CTA waits for the halos (no own-band
 # test, no reordered schedule)
 _LATE_WAIT = os.environ.get("TD_STRIP_LATE_WAIT", "1") != "0"
-# TD_STRIP_OVERLAP_PUSH=1 -> the tile-halo push rides a side stream (measured on 2 x B200: no gain over the caller's stream --
-# the step is bound by the NVLink round trip of the push itself, 9 us, which the receiving blend has to wait for either way)
+# TD_STRIP_OVERLAP_PUSH=1 -> the tile-halo push rides a side stream (the step is bound by the NVLink round trip of the push
+# itself, which the receiving blend has to wait for either way, so the caller's stream is the default)
 _OVERLAP_PUSH = os.environ.get("TD_STRIP_OVERLAP_PUSH", "0") == "1"
 
 

@@ -1,10 +1,10 @@
 """Base tile-method delegate with the reference's surface
-(tile_methods/abstractdiffusion.py), B200-native underneath.
+(tile_methods/abstractdiffusion.py), H100-native underneath.
 
 What differs from the reference by design:
   * `init_grid_bbox` also builds a `td_grid` plan (C-ABI) and a persistent
     tile-batch buffer: the whole step's scatter is ONE kernel launch and the
-    UNet receives views of that buffer (180 GB of HBM: no need to re-cat).
+    UNet receives views of that buffer (the tile batch is small next to 80 GB of HBM: no need to re-cat).
   * `reset_buffer` only (re)allocates: the fused gather-form blend writes every
     canvas pixel, so the per-step `zero_()` pass of the reference is not needed.
   * Region prompt control (SURVEY.md section 8(f)-1) is built on the same kernels: the grid tiles go through the
@@ -101,7 +101,7 @@ class AbstractDiffusion:
         self.stablesr_tensor_batch = None
         self.stablesr_tensor_custom: list = []
 
-        # B200 engine state
+        # device engine state
         self._grid = None                     # td_grid plan
         self._tiles: Optional[Tensor] = None  # persistent [T*N, C, th, tw] scatter target
         self._icond_tiles: Optional[Tensor] = None
@@ -814,7 +814,7 @@ class AbstractDiffusion:
     # ----------------------------------------------------------- engine glue
     def _check_input(self, x_in: Tensor) -> Tensor:
         if not x_in.is_cuda:
-            raise RuntimeError(f"{self.method}: latent is on {x_in.device}; the B200 path has no CPU fallback")
+            raise RuntimeError(f"{self.method}: latent is on {x_in.device}; the H100 path has no CPU fallback")
         if self.enable_grid_bbox and self._grid is None:
             raise RuntimeError(f"{self.method}: init_grid_bbox() has not been called")
         if self.weights.device != x_in.device:

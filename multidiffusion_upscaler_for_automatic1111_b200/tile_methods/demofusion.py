@@ -1,5 +1,5 @@
 """DemoFusion (arXiv 2311.16973) tile method with the reference's surface
-(tile_methods/demofusion.py), on the sm_100a kernels:
+(tile_methods/demofusion.py), on the sm_90a kernels:
 
     local windows   td_scatter_tiles + td_blend_multidiffusion (count-normalised)     demofusion.py:254-264
     gaussian blur   td_depthwise_conv2d                                                demofusion.py:173-178
@@ -46,7 +46,7 @@ class DemoFusion(AbstractDiffusion):
         if not self._jitter:
             return super()._check_input(x_in)
         if not x_in.is_cuda:
-            raise RuntimeError(f"{self.method}: latent is on {x_in.device}; the B200 path has no CPU fallback")
+            raise RuntimeError(f"{self.method}: latent is on {x_in.device}; the H100 path has no CPU fallback")
         if self._origins_dev is None:
             raise RuntimeError(f"{self.method}: get_views() has not been called")
         return x_in.contiguous()

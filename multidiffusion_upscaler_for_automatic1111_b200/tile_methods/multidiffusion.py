@@ -1,5 +1,5 @@
 """MultiDiffusion (arXiv 2302.08113) tile method with the reference's surface
-(tile_methods/multidiffusion.py), executed by two sm_100a kernels per sampler step:
+(tile_methods/multidiffusion.py), executed by two sm_90a kernels per sampler step:
 
     td_scatter_tiles          <- `torch.cat([x_in[bbox.slicer] ...])` for every batch   (:155)
     td_blend_multidiffusion   <- `x_buffer[slicer] += tile` x T  +  `torch.where(...)`   (:166-167, :208)

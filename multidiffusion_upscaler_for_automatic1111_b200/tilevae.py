@@ -1,8 +1,8 @@
 """Tiled VAE with the reference's surface (scripts/tilevae.py: `VAEHook`, `GroupNormParam`,
-`get_var_mean`, `custom_group_norm`, `crop_valid_region`, `build_task_queue`), B200-native
+`get_var_mean`, `custom_group_norm`, `crop_valid_region`, `build_task_queue`), H100-native
 underneath.
 
-What is different from the reference by design (180 GB of HBM, hand-written sm_100a kernels):
+What is different from the reference by design (80 GB of HBM, hand-written sm_90a kernels):
   * tiles, residuals and parked activations stay in HBM -- the reference stages every tile
     through host RAM (`.cpu()` at tilevae.py:534,610,641) and re-uploads it each round;
   * GroupNorm statistics: one streaming read (`td_gn_stats`, fp32 Chan/Welford merge with
@@ -15,7 +15,7 @@ What is different from the reference by design (180 GB of HBM, hand-written sm_1
   * no per-tile NaN test (each one is a full read + host sync, tilevae.py:625): the result
     is checked once at the end and the estimator keeps its NaN fallback.
   * fp16 / bf16 networks run channels-last with every convolution and the attention GEMMs on the tensor cores
-    (tcgen05, csrc/td_conv.cu) through `vae_engine.TensorCoreBackend`; fp32 networks keep the host application's
+    (wgmma, csrc/td_conv.cu) through `vae_engine.TensorCoreBackend`; fp32 networks keep the host application's
     modules for the dense ops (`vae_engine.ModuleBackend`).
 The network is compiled once into an op program (`vae_engine.compile_program`); GroupNorm sites are barriers between
 tiles unless fast mode froze their statistics.
@@ -258,7 +258,7 @@ class VAEHook:
         self.to_gpu = to_gpu
         self.pad = 11 if is_decoder else 32
         self.verbose = False
-        self.backend_name = None      # which backend ran the last call ("tcgen05" / "modules")
+        self.backend_name = None      # which backend ran the last call ("wgmma" / "modules")
         self._program = None
         self._shard_group = None
         self._shard_world = 1
@@ -318,7 +318,7 @@ class VAEHook:
         param = next(self.net.parameters())
         device, dtype = param.device, param.dtype
         if device.type != "cuda":
-            raise RuntimeError(f"VAEHook: network is on {device}; the B200 tiled-VAE path has no CPU fallback")
+            raise RuntimeError(f"VAEHook: network is on {device}; the H100 tiled-VAE path has no CPU fallback")
         net, tile_size, is_decoder = self.net, self.tile_size, self.is_decoder
         z = z.detach().to(device=device, dtype=dtype).contiguous()
         N, height, width = z.shape[0], z.shape[2], z.shape[3]

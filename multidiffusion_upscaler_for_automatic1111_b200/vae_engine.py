@@ -11,7 +11,7 @@ stop every tile at each GroupNorm, merge the tiles' statistics, continue -- is k
     statistics are merged (pixel-weighted average of variances and means, the reference's rule) and the round resumes.
   * two backends execute the same program:
       - `TensorCoreBackend` (fp16 / bf16 networks): activations channels-last in HBM, every convolution and the four
-        attention GEMMs on tcgen05 (csrc/td_conv.cu), GroupNorm statistics / apply+SiLU / upsample / softmax on the
+        attention GEMMs on wgmma (csrc/td_conv.cu), GroupNorm statistics / apply+SiLU / upsample / softmax on the
         channels-last streaming kernels (csrc/td_nhwc.cu);
       - `ModuleBackend` (fp32 networks or layouts the kernels do not cover): the host application's modules for the
         dense ops, NCHW GroupNorm kernels (csrc/td_vae.cu).
@@ -195,8 +195,8 @@ DUAL_OUTPUT = os.environ.get("TD_VAE_DUAL_OUTPUT", "1") != "0"         # 0: sepa
 
 
 class TensorCoreBackend:
-    """Channels-last activations; convolutions and attention GEMMs on tcgen05, the rest on streaming kernels."""
-    name = "tcgen05"
+    """Channels-last activations; convolutions and attention GEMMs on wgmma, the rest on streaming kernels."""
+    name = "wgmma"
 
     def __init__(self, program: Program, device, dtype):
         self.program, self.device, self.dtype = program, device, dtype
@@ -301,7 +301,7 @@ class TensorCoreBackend:
 
     def attention(self, a, op: Attention, skip, post=None, dual=False):
         """softmax(q k^T / sqrt(C)) v + proj_out (tile_utils/attn.py:49-72) as four tensor-core GEMMs and one row
-        softmax; the [tokens, tokens] score matrix lives in HBM (388 MB fp16 for a 118 x 118 tile: nothing on 180 GB)."""
+        softmax; the [tokens, tokens] score matrix lives in HBM (388 MB fp16 for a 118 x 118 tile: small next to 80 GB)."""
         m = op.module
         _, H, W, C = a.shape
         T = H * W

@@ -147,7 +147,7 @@ def gen_region(ref):
                 out[key + "_dtype"] = np.array(str(o.dtype))
             out[f"{name}_{method}_weights"] = d.weights[0, 0].numpy()
             out[f"{name}_rects"] = np.array([(b.x, b.y, b.w, b.h) for b in d.custom_bboxes], np.int32)
-    np.savez_compressed(os.path.join(GOLDEN_DIR, "region_small.npz"), **out)
+    _save_split("region_small", out)
 
 
 def gen_demofusion_jitter(ref):
@@ -233,6 +233,21 @@ def vae_case_inputs(is_decoder: bool, H: int, W: int):
     return net, z
 
 
+def _save_split(name: str, arrays: dict, part_bytes: int = 1_100_000):
+    """name.npz, name.1.npz, ...: arrays packed in order, about `part_bytes` raw bytes per file (each stays under 1 MB
+    compressed); tests/helpers.load_golden merges them back."""
+    parts, cur, size = [], {}, 0
+    for k, a in arrays.items():
+        if cur and size + a.nbytes > part_bytes:
+            parts.append(cur)
+            cur, size = {}, 0
+        cur[k] = a
+        size += a.nbytes
+    parts.append(cur)
+    for i, part in enumerate(parts):
+        np.savez_compressed(os.path.join(GOLDEN_DIR, f"{name}.npz" if i == 0 else f"{name}.{i}.npz"), **part)
+
+
 def _bits(t: torch.Tensor) -> np.ndarray:
     t = t.contiguous()
     if t.dtype == torch.float32:
@@ -282,6 +297,47 @@ def run_reference_step(ref, method: str, x: torch.Tensor, W, H, tw, th, ov, bs):
     return d, out
 
 
+# one hooked step on an odd canvas (bboxes and output of the reference) and the reference's tile cat
+REF_STEP_CASE = (2, 4, 88, 56, 32, 24, 10, 3)       # N, C, W, H, tw, th, ov, bs
+REF_SCATTER_CASE = (2, 4, 80, 64, 24, 16, 6)         # N, C, W, H, tw, th, ov
+
+
+def gen_reference_steps(ref):
+    """11. tests/test_oracle_vs_reference.py: the reference's step and scatter outputs for the oracle to match --------"""
+    N, C, W, H, tw, th, ov, bs = REF_STEP_CASE
+    out = {}
+    for method in ("md", "mod"):
+        for dn, dt in DTYPES.items():
+            x = synth.latent(11, (N, C, H, W), dt)
+            d, o = run_reference_step(ref, method, x, W, H, tw, th, ov, bs)
+            out[f"{method}_{dn}_bboxes"] = np.array([(b.x, b.y, b.w, b.h) for bb in d.batched_bboxes for b in bb], np.int32)
+            out[f"{method}_{dn}"] = _bits(o)
+            out[f"{method}_{dn}_dtype"] = np.array(str(o.dtype))
+    N, C, W, H, tw, th, ov = REF_SCATTER_CASE
+    x = synth.latent(5, (N, C, H, W), torch.float16)
+    bbs, _ = ref.utils.split_bboxes(W, H, tw, th, ov, 1.0)
+    out["scatter_bboxes"] = np.array([(b.x, b.y, b.w, b.h) for b in bbs], np.int32)
+    out["scatter"] = _bits(torch.cat([x[b.slicer] for b in bbs], dim=0))
+    np.savez_compressed(os.path.join(GOLDEN_DIR, "reference_steps.npz"), **out)
+
+
+HOST_RECORD_MODULES = ("test_region_cond", "test_noise_inverse", "test_side_inputs", "test_demofusion")
+
+
+def gen_host_records(ref):
+    """12. host-logic comparisons (region conditioning, noise inversion, ControlNet / StableSR caches, DemoFusion
+    forward_one_step): each test module's `reference_records(ref)` drives the reference through the same scenario as
+    its test drives our delegate; the digests (sha256 of dtype, shape, bytes) go to host_records.npz -----------------"""
+    import importlib
+    tests_dir = os.path.dirname(GOLDEN_DIR)
+    if tests_dir not in sys.path:
+        sys.path.insert(0, tests_dir)
+    out = {}
+    for name in HOST_RECORD_MODULES:
+        out.update(importlib.import_module(name).reference_records(ref))
+    np.savez_compressed(os.path.join(GOLDEN_DIR, "host_records.npz"), **{k: np.array(v) for k, v in out.items()})
+
+
 def main():
     if not ref_shim.available():
         sys.exit("reference tree not present; goldens can only be generated in the build container")
@@ -293,6 +349,12 @@ def main():
         return
     if "jitter" in sys.argv[1:]:      # regenerate only demofusion_jitter.npz
         gen_demofusion_jitter(ref)
+        return
+    if "steps" in sys.argv[1:]:       # regenerate only reference_steps.npz
+        gen_reference_steps(ref)
+        return
+    if "host" in sys.argv[1:]:        # regenerate only host_records.npz
+        gen_host_records(ref)
         return
 
     # 1. split_bboxes sweep (utils.py:160-177) ------------------------------------
@@ -350,7 +412,7 @@ def main():
                 _, o = run_reference_step(ref, method, x, W, H, tw, th, ov, bs)
                 out[f"{name}_{dn}_{method}"] = _bits(o)
                 out[f"{name}_{dn}_{method}_dtype"] = np.array(str(o.dtype))
-    np.savez_compressed(os.path.join(GOLDEN_DIR, "blend_small.npz"), **out)
+    _save_split("blend_small", out)
 
     # 5. full-size configs, hash only ---------------------------------------------
     out = {"cases": np.array([c[1:] for c in HASH_CASES], np.int32), "names": np.array([c[0] for c in HASH_CASES])}
@@ -408,6 +470,8 @@ def main():
 
     gen_region(ref)
     gen_demofusion_jitter(ref)
+    gen_reference_steps(ref)
+    gen_host_records(ref)
 
     for f in sorted(os.listdir(GOLDEN_DIR)):
         print(f, os.path.getsize(os.path.join(GOLDEN_DIR, f)))

@@ -8,9 +8,10 @@ tile_utils/attn.py:8-10).  None of those exist here.  This shim injects empty
 `/root/reference` on `sys.path`, and returns the reference's own modules so that
 `oracle/make_golden.py` and the CPU tests can call the reference's real code.
 
-It only works where `/root/reference` exists (the build container).  Nothing on
-the GPU box may import it: `available()` is the guard.  No reference source is
-copied; this file contains only stubs.
+`load()` only works where the reference tree exists; `available()` is the guard.
+`host_stubs()` installs the same stub host without it, so the tests can drive our
+delegates against records of the reference's behaviour (tests/golden/host_records.npz).
+No reference source is copied; this file contains only stubs.
 """
 from __future__ import annotations
 
@@ -98,15 +99,13 @@ _installed = False
 
 
 def install(device: str = "cpu"):
-    """Inject the stub host.  Idempotent."""
+    """Inject the stub host (no reference tree needed).  Idempotent."""
     global _installed
     import torch
 
     if _installed:
         sys.modules["modules.devices"].device = torch.device(device)
         return
-    if not available():
-        raise RuntimeError(f"reference tree not found at {REFERENCE_ROOT}")
 
     class KDiffusionSampler:  # isinstance() target, abstractdiffusion.py:77-79
         pass
@@ -178,14 +177,24 @@ def install(device: str = "cpu"):
     _mod("ldm.modules.diffusionmodules")
     _mod("ldm.modules.diffusionmodules.model", AttnBlock=_Dummy, MemoryEfficientAttnBlock=_Dummy)
 
-    if REFERENCE_ROOT not in sys.path:
-        sys.path.insert(0, REFERENCE_ROOT)
     _installed = True
+
+
+def host_stubs(device: str = "cpu"):
+    """The stub host's objects our delegates reach through `host` (shared state, devices, sampler classes)."""
+    install(device)
+    return types.SimpleNamespace(shared=sys.modules["modules.shared"], devices=sys.modules["modules.devices"],
+                                 KDiffusionSampler=sys.modules["modules.sd_samplers_kdiffusion"].KDiffusionSampler,
+                                 CompVisSampler=sys.modules["modules.sd_samplers_timesteps"].CompVisSampler)
 
 
 def load(device: str = "cpu"):
     """Return a namespace of the reference's own (unmodified) modules."""
+    if not available():
+        raise RuntimeError(f"reference tree not found at {REFERENCE_ROOT}")
     install(device)
+    if REFERENCE_ROOT not in sys.path:
+        sys.path.insert(0, REFERENCE_ROOT)
     import importlib
 
     ns = types.SimpleNamespace()
@@ -213,9 +222,9 @@ def make_p(width: int, height: int, sampler_name: str = "Euler a"):
 def make_kdiff_sampler(inner_forward):
     """Fake k-diffusion sampler: `.model_wrap_cfg.inner_model.forward` is what
     MultiDiffusion.hook patches (multidiffusion.py:22-23)."""
-    ref = load()
+    stubs = host_stubs()
 
-    class _Sampler(ref.KDiffusionSampler):
+    class _Sampler(stubs.KDiffusionSampler):
         pass
 
     s = _Sampler()

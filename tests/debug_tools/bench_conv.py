@@ -1,4 +1,4 @@
-"""Hand-run timing of the tcgen05 convolution at BASELINE cfg4's decoder shapes (GPU box): TFLOP/s of td_conv2d_nhwc
+"""Hand-run timing of the wgmma convolution at BASELINE cfg4's decoder shapes (GPU box): TFLOP/s of td_conv2d_nhwc
 next to cuDNN (F.conv2d, channels_last fp16) on the same tensors.  Usage: python tests/debug_tools/bench_conv.py"""
 import json
 import os

@@ -1,4 +1,4 @@
-"""Hand-run launcher for ncu captures of the tcgen05 convolution (GPU box).
+"""Hand-run launcher for ncu captures of the wgmma convolution (GPU box).
 Usage: python tests/debug_tools/run_conv.py H W Cin Cout k [reps] [mode]
 mode: plain (bias only) | gn (frozen GroupNorm + SiLU epilogue) | res (residual) | gnres | dual (residual, two outputs) | up (folded upsample)"""
 import os

@@ -1,10 +1,49 @@
 """Shared helpers for the parity tests (bit views, oracle plans)."""
+import glob
 import hashlib
+import os
 
 import numpy as np
 import torch
 
 DTYPES = {"f16": torch.float16, "bf16": torch.bfloat16, "f32": torch.float32}
+
+
+def load_golden(golden_dir: str, name: str) -> dict:
+    """The arrays of fixture `name`: `name.npz` plus its parts `name.<k>.npz` (large fixtures are split so that no
+    file exceeds 1 MB)."""
+    out = {}
+    for f in [os.path.join(golden_dir, name + ".npz")] + sorted(glob.glob(os.path.join(golden_dir, name + ".*.npz"))):
+        with np.load(f) as z:
+            out.update({k: z[k] for k in z.files})
+    return out
+
+
+def digest(obj) -> str:
+    """SHA-256 of a tensor (dtype, shape and bytes) or of a nest of tuples / lists of tensors, strings and numbers: two
+    results with the same digest are bit-identical (what torch.equal plus a dtype and shape check asserts)."""
+    h = hashlib.sha256()
+
+    def feed(o):
+        if isinstance(o, torch.Tensor):
+            t = o.detach().cpu().contiguous()
+            h.update(f"T{t.dtype}{tuple(t.shape)}|".encode())
+            h.update(t.reshape(-1).view(torch.uint8).numpy().tobytes())
+        elif isinstance(o, (list, tuple)):
+            h.update(f"L{len(o)}[".encode())
+            for v in o:
+                feed(v)
+            h.update(b"]")
+        else:
+            h.update(f"S{type(o).__name__}:{o!r}|".encode())
+    feed(obj)
+    return h.hexdigest()
+
+
+def host_record(golden_dir: str, key: str) -> str:
+    """The recorded digest of the reference's side of a host-logic comparison (oracle/make_golden.py, `host_records`)."""
+    with np.load(os.path.join(golden_dir, "host_records.npz")) as z:
+        return str(z[key])
 
 
 def bits(t: torch.Tensor) -> np.ndarray:
@@ -37,23 +76,25 @@ def assert_bit_equal(a: torch.Tensor, b: torch.Tensor, what: str = "", allow_sig
 
 def region_composite_reference(x_buffer, weights, regions, out=None):
     """The reference's tensor expressions (multidiffusion.py:187-216, mixtureofdiffusers.py:145-175) on CPU tensors:
-    what td_region_composite fuses on the device."""
+    what td_region_composite fuses on the device.  Weights and region tensors are taken to x_buffer's device."""
     N, C, H, W = x_buffer.shape
+    dev = x_buffer.device
     buf = x_buffer.clone()
     fb = fm = fc = None
     for (x, y, w, h, mode, r_out, aux) in regions:
+        r_out, aux = r_out.to(dev), None if aux is None else aux.to(dev)
         sl = (slice(None), slice(None), slice(y, y + h), slice(x, x + w))
         if mode == 0:
             buf[sl] += r_out if aux is None else r_out * aux
         else:
             if fb is None:
-                fb, fm, fc = torch.zeros_like(buf), torch.zeros((1, 1, H, W)), torch.zeros((1, 1, H, W))
+                fb, fm, fc = torch.zeros_like(buf), torch.zeros((1, 1, H, W), device=dev), torch.zeros((1, 1, H, W), device=dev)
             fb[sl] += r_out
             fm[sl] += aux
             fc[sl] += 1
     res = buf
     if weights is not None:
-        wv = weights.view(1, 1, H, W)
+        wv = weights.to(dev).view(1, 1, H, W)
         res = torch.where(wv > 1, buf / wv, buf)
     if fb is not None:
         fb = torch.where(fc > 1, fb / fc, fb)

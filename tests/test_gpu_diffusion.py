@@ -1,4 +1,4 @@
-"""Parity tests proper: the sm_100a kernels, called through the C-ABI, against the oracle
+"""Parity tests proper: the sm_90a kernels, called through the C-ABI, against the oracle
 and the reference-generated fixtures.  Bit-exact (integer/index work AND the fp blend:
 the gather-form kernel reproduces the reference's rounding sequence)."""
 import os
@@ -8,7 +8,7 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import DTYPES, assert_bit_equal, bits, sha
+from helpers import load_golden, DTYPES, assert_bit_equal, bits, sha
 from oracle import blend, synth, tiling
 
 pytestmark = pytest.mark.gpu
@@ -105,7 +105,7 @@ def _oracle_step(method, x, plan, tile_dtype=None):
 @pytest.mark.parametrize("dn", list(DTYPES))
 @pytest.mark.parametrize("flags", ALL_PATHS)
 def test_blend_small_matches_reference_fixtures(eng, golden_dir, method, dn, flags):
-    g = np.load(os.path.join(golden_dir, "blend_small.npz"))
+    g = load_golden(golden_dir, "blend_small")
     for name, (N, C, W, H, tw, th, ov, bs) in zip(g["names"], g["cases"]):
         x = synth.latent(synth.case_seed(str(name), dn), (int(N), int(C), int(H), int(W)), DTYPES[dn])
         out, _, _ = _run_cuda_step(eng, method, x, int(W), int(H), int(tw), int(th), int(ov), int(bs), flags=flags)
@@ -128,7 +128,7 @@ def test_fast_exact_divide_is_ieee_on_its_domain(dn):
 @pytest.mark.parametrize("dn", ["f16", "bf16"])
 @pytest.mark.parametrize("flags", [0, ROWS, PIPE, TMA, NO_TMA])
 def test_blend_with_reciprocal_weights_matches_reference(eng, golden_dir, dn, flags):
-    g = np.load(os.path.join(golden_dir, "blend_small.npz"))
+    g = load_golden(golden_dir, "blend_small")
     for name, (N, C, W, H, tw, th, ov, bs) in zip(g["names"], g["cases"]):
         x = synth.latent(synth.case_seed(str(name), dn), (int(N), int(C), int(H), int(W)), DTYPES[dn])
         out, _, _ = _run_cuda_step(eng, "md", x, int(W), int(H), int(tw), int(th), int(ov), int(bs), flags=flags, use_rcp=True)

@@ -1,7 +1,7 @@
 """GPU tests of everything written after the round-1 GPU budget was spent: region prompt control, ControlNet tile caches,
 DemoFusion random jitter (the list-driven kernels of csrc/td_jitter.cu).  Their host logic is pinned on CPU against the
 reference (tests/test_region*.py, test_side_inputs.py, test_demofusion.py); the device runs below have not executed on
-hardware when they were written; all of them passed on B200 (round-1 driver run, round-2 first run) and are plain tests now.
+hardware when they were written; they are plain tests now.
 
 The file sorts last on purpose: should a never-run kernel fault, the CUDA context of the pytest process is gone, and
 nothing that is already verified may run after it.
@@ -13,7 +13,7 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import DTYPES, assert_bit_equal
+from helpers import load_golden, DTYPES, assert_bit_equal
 from oracle import demofusion as odf
 from oracle import synth
 from oracle.make_golden import DEMO_CFG, REGION_CASES, REGION_DTYPES
@@ -24,7 +24,7 @@ from test_side_inputs import H, W, _hints, _p
 
 @pytest.fixture(scope="module")
 def gold(golden_dir):
-    return np.load(os.path.join(golden_dir, "region_small.npz"))
+    return load_golden(golden_dir, "region_small")
 
 
 # ------------------------------------------------------------------------------- region prompt control (verified kernels + torch)
@@ -36,7 +36,7 @@ def test_delegate_region_step_on_gpu(gold, case, method, dn):
     name, bg, rows = case
     d, out = _run_delegate(method, _x(name, dn), bg, rows, "cuda")
     assert out.is_cuda
-    assert_bit_equal(out, _want(gold, f"{name}_{method}_{dn}"), f"{method} delegate, sm_100a kernels")
+    assert_bit_equal(out, _want(gold, f"{name}_{method}_{dn}"), f"{method} delegate, sm_90a kernels")
 
 
 # ------------------------------------------------------------------------------- ControlNet tile caches (scatter on the x8 plan)
@@ -81,7 +81,7 @@ def test_strip_blend_matches_reference_fixtures_on_gpu(golden_dir, dn, use_rcp, 
     from test_gpu_diffusion import _run_cuda_step
     if use_rcp and dn == "f32":
         pytest.skip("the fast exact divide is a 16-bit path")
-    g = np.load(os.path.join(golden_dir, "blend_small.npz"))
+    g = load_golden(golden_dir, "blend_small")
     for name, (N, C, W, H, tw, th, ov, bs) in zip(g["names"], g["cases"]):
         x = synth.latent(synth.case_seed(str(name), dn), (int(N), int(C), int(H), int(W)), DTYPES[dn])
         out, xb, plan = _run_cuda_step(engine, "md", x, int(W), int(H), int(tw), int(th), int(ov), int(bs), flags=STRIP, use_rcp=use_rcp)
@@ -101,7 +101,7 @@ def test_strip_mixture_matches_reference_fixtures_on_gpu(golden_dir, dn):
     from multidiffusion_upscaler_for_automatic1111_b200 import engine
     from helpers import bits, sha
     from test_gpu_diffusion import _run_cuda_step
-    g = np.load(os.path.join(golden_dir, "blend_small.npz"))
+    g = load_golden(golden_dir, "blend_small")
     for name, (N, C, W, H, tw, th, ov, bs) in zip(g["names"], g["cases"]):
         x = synth.latent(synth.case_seed(str(name), dn), (int(N), int(C), int(H), int(W)), DTYPES[dn])
         out, _, _ = _run_cuda_step(engine, "mod", x, int(W), int(H), int(tw), int(th), int(ov), int(bs), flags=STRIP)

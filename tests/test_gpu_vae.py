@@ -162,7 +162,7 @@ def _sd_width_net(is_dec, seed):
 
 @pytest.mark.parametrize("is_dec,fast,H,W,tile", [(True, True, 40, 52, 16), (True, False, 40, 52, 16), (False, True, 200, 264, 64), (False, False, 136, 200, 64)])
 def test_vaehook_tensor_core_backend_matches_fp32_reference(tv, is_dec, fast, H, W, tile):
-    """fp16 network on the tcgen05 / channels-last backend vs the fp32 restatement of the reference's tiled algorithm
+    """fp16 network on the wgmma / channels-last backend vs the fp32 restatement of the reference's tiled algorithm
     (oracle, run on the GPU in fp32: same tiles, same statistics merge).  fp16 activations through ~60 layers:
     mean error <= 2e-3 * scale, max <= 3e-2 * scale."""
     from oracle import synth
@@ -175,7 +175,7 @@ def test_vaehook_tensor_core_backend_matches_fp32_reference(tv, is_dec, fast, H,
     hook = tv.VAEHook(net16, tile, is_dec, fast_decoder=fast, fast_encoder=fast, color_fix=False)
     with torch.no_grad():
         got = hook(z.cuda().half())
-    assert hook.backend_name == "tcgen05"
+    assert hook.backend_name == "wgmma"
     assert got.dtype == torch.float16 and got.shape == want.shape
     diff = (got.cpu().float() - want).abs()
     scale = want.abs().max().item()
@@ -183,7 +183,7 @@ def test_vaehook_tensor_core_backend_matches_fp32_reference(tv, is_dec, fast, H,
 
 
 def test_tensor_core_backend_matches_module_backend_on_the_same_fp16_network(tv):
-    """Same fp16 weights, same tiles: tcgen05 / channels-last backend vs cuDNN modules + NCHW kernels."""
+    """Same fp16 weights, same tiles: wgmma / channels-last backend vs cuDNN modules + NCHW kernels."""
     from multidiffusion_upscaler_for_automatic1111_b200 import vae_engine as ve
     from oracle import synth
     net16 = _sd_width_net(True, 3).cuda().half()

@@ -29,7 +29,7 @@ def emul():
     srcs = [os.path.join(ROOT, "tests", "emul", "jitter_host_emul.cu"), os.path.join(PKG, "csrc", "td_host.cpp")]
     deps = srcs + [os.path.join(PKG, "csrc", "td_jitter.cu")]
     if not os.path.exists(so) or any(os.path.getmtime(d) > os.path.getmtime(so) for d in deps):
-        cmd = [nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-O2", "-std=c++17", "--shared", "-Xcompiler", "-fPIC,-ffp-contract=off",
+        cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O2", "-std=c++17", "--shared", "-Xcompiler", "-fPIC,-ffp-contract=off",
                "--expt-relaxed-constexpr", "-I", os.path.join(ROOT, "include"), "-I", os.path.join(PKG, "csrc"), "-o", so, *srcs]
         res = subprocess.run(cmd, capture_output=True, text=True)
         assert res.returncode == 0, res.stderr[-3000:]

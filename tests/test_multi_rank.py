@@ -91,11 +91,11 @@ def _gloo_delegate_worker(rank, world, port, result_dir):
     def blend_multidiffusion(g, outs, N, C, tile_bs, weights, acc_dtype, x_buffer=None, flags=0, out=None, rcp_weights=None):
         buf = torch.zeros((N, C, g.H, g.W), dtype=acc_dtype)
         blend.accumulate_md(buf, torch.cat(list(outs), dim=0), bbs(g), N)
-        return blend.normalise_md(buf, weights)
+        return blend.normalise_md(buf, weights.to(buf.device))
 
     def blend_mixture(g, outs, N, C, tile_bs, tile_weights, rescale, x_buffer, flags=0):
         x_buffer.zero_()
-        blend.accumulate_mod(x_buffer, torch.cat(list(outs), dim=0), bbs(g), N, tile_weights, rescale)
+        blend.accumulate_mod(x_buffer, torch.cat(list(outs), dim=0), bbs(g), N, tile_weights.to(x_buffer.device), rescale.to(x_buffer.device))
         return x_buffer
     engine.scatter_tiles, engine.blend_multidiffusion, engine.blend_mixture = scatter_tiles, blend_multidiffusion, blend_mixture
     abstractdiffusion.AbstractDiffusion._check_input = lambda self, x: x.contiguous()
@@ -360,7 +360,7 @@ def _gpu_worker(rank, world, port, result_dir):
 @pytest.mark.gpu
 def test_two_gpu_sharded_multidiffusion_bit_identical(tmp_path):
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     mp.spawn(_gpu_worker, args=(2, _free_port(), str(tmp_path)), nprocs=2, join=True)
     assert (tmp_path / "ok0").exists() and (tmp_path / "ok1").exists()
 
@@ -406,7 +406,7 @@ def _gpu_mod_worker(rank, world, port, result_dir):
 @pytest.mark.gpu
 def test_two_gpu_sharded_mixture_bit_identical(tmp_path):
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     mp.spawn(_gpu_mod_worker, args=(2, _free_port(), str(tmp_path)), nprocs=2, join=True)
     assert (tmp_path / "ok0").exists() and (tmp_path / "ok1").exists()
 
@@ -453,6 +453,6 @@ def _gpu_demofusion_worker(rank, world, port, result_dir):
 @pytest.mark.gpu
 def test_two_gpu_sharded_demofusion_matches_oracle(tmp_path):
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     mp.spawn(_gpu_demofusion_worker, args=(2, _free_port(), str(tmp_path)), nprocs=2, join=True)
     assert (tmp_path / "ok0").exists() and (tmp_path / "ok1").exists()

@@ -1,8 +1,9 @@
 """Tiled noise inversion (SURVEY.md section 8(f)-3): `init_noise_inverse` replaces the sampler's `sample_img2img`; the
 Euler inversion loop runs the tiled denoiser (`get_noise`), the result is mixed with fresh noise under the retouch mask.
 
-The UNMODIFIED reference (oracle/ref_shim.py) runs next to our delegate on CPU, with the device kernels swapped for the
-oracle's scatter / blend (pinned by tests/test_gpu_diffusion.py); outputs must be identical.
+Our delegate runs on CPU under the stub host (oracle/ref_shim.py), with the device kernels swapped for the oracle's
+scatter / blend (pinned by tests/test_gpu_diffusion.py); its outputs must be identical to the UNMODIFIED reference's in
+the same job, recorded by `reference_records` (oracle/make_golden.py -> tests/golden/host_records.npz).
 """
 import types
 
@@ -10,9 +11,8 @@ import numpy as np
 import pytest
 import torch
 
+from helpers import digest, host_record
 from oracle import blend, ref_shim
-
-pytestmark = pytest.mark.skipif(not ref_shim.available(), reason="reference tree not present")
 
 W, H = 64, 48
 ROWS = [(True, 0.1, 0.2, 0.5, 0.4, "a cat", "", "Background", 0.2, -1),
@@ -40,7 +40,7 @@ def _image():
     return Image.fromarray(a)
 
 
-def _job(ref, cls, settings, draw_background, with_regions):
+def _job(stubs, cls, settings, cache_cls, draw_background, with_regions):
     """(delegate, sampler, p, cache) ready for sampler.sample_img2img(...)."""
     sd_model = types.SimpleNamespace(sd_model_hash="abc", get_learned_conditioning=lambda prompts: torch.full((len(prompts), 77, 8), 0.25))
     g = torch.Generator().manual_seed(5)
@@ -49,7 +49,7 @@ def _job(ref, cls, settings, draw_background, with_regions):
                               init_latent=torch.randn(1, 4, H, W, generator=g), image_conditioning=torch.zeros(1, 5, 1, 1),
                               init_images=[_image()], show_tile_progress=False)
 
-    class _Sampler(ref.KDiffusionSampler):
+    class _Sampler(stubs.KDiffusionSampler):
         pass
     sampler = _Sampler()
     sampler.model_wrap = _DNW()
@@ -64,7 +64,7 @@ def _job(ref, cls, settings, draw_background, with_regions):
 
     def set_cache(x0, xt, prompts):
         cache["sets"] += 1
-        cache["v"] = ref.utils.NoiseInverseCache("abc", x0, xt, 4, 1.5, prompts)
+        cache["v"] = cache_cls("abc", x0, xt, 4, 1.5, prompts)
 
     d = cls(p, sampler)
     d.init_grid_bbox(16, 16, 8, 4)
@@ -92,7 +92,7 @@ def _oracle_engine(monkeypatch):
         blend.accumulate_md(buf, torch.cat(list(outs), dim=0), bbs(g), N)
         if x_buffer is not None:
             x_buffer.copy_(buf)
-        return blend.normalise_md(buf, weights)
+        return blend.normalise_md(buf, weights.to(buf.device))
 
     from helpers import region_composite_reference
     monkeypatch.setattr(engine, "region_composite", region_composite_reference)
@@ -101,35 +101,52 @@ def _oracle_engine(monkeypatch):
     monkeypatch.setattr(abstractdiffusion.AbstractDiffusion, "_check_input", lambda self, x: x.contiguous())
 
 
-@pytest.mark.parametrize("mode", ["grid", "grid+regions", "regions_only"])
-def test_noise_inversion_like_the_reference(monkeypatch, mode):
-    from multidiffusion_upscaler_for_automatic1111_b200 import MultiDiffusion, host
-    ref = ref_shim.load()
+MODES = ["grid", "grid+regions", "regions_only"]
+
+
+def _record(mode, ref=None):
+    """Digest of (inverted latent, combined noise, combined noise from the cache, steps) of one job: our delegate, or
+    the reference's (`ref` given)."""
+    from multidiffusion_upscaler_for_automatic1111_b200 import host
+    stubs = ref_shim.host_stubs()
     host._a1111_cache.clear()
-    _oracle_engine(monkeypatch)
-    ref.shared.sd_model.apply_model = lambda x, t, cond=None: x * 0.5 + t.view(-1, 1, 1, 1) * 1e-3 + cond["c_crossattn"][0].mean() * 0.1
-    if hasattr(ref.shared.sd_model, "apply_model_original_md"):
-        del ref.shared.sd_model.apply_model_original_md
+    stubs.shared.sd_model.apply_model = lambda x, t, cond=None: x * 0.5 + t.view(-1, 1, 1, 1) * 1e-3 + cond["c_crossattn"][0].mean() * 0.1
+    if hasattr(stubs.shared.sd_model, "apply_model_original_md"):
+        del stubs.shared.sd_model.apply_model_original_md
     with_regions, bg = mode != "grid", mode != "regions_only"
+    if ref is None:
+        from multidiffusion_upscaler_for_automatic1111_b200 import MultiDiffusion as cls
+        from multidiffusion_upscaler_for_automatic1111_b200.tile_utils.utils import NoiseInverseCache as cache_cls
+        settings = {i: r for i, r in enumerate(ROWS)}
+    else:
+        cls, cache_cls = ref.multidiffusion.MultiDiffusion, ref.utils.NoiseInverseCache
+        settings = {i: ref.utils.BBoxSettings(*r) for i, r in enumerate(ROWS)}
 
     # region prompts at a noise-inversion step go through the (stand-in) prompt parser: [tokens] -> unsqueeze -> apply_model
     noise = torch.randn(1, 4, H, W, generator=torch.Generator().manual_seed(9))
     x = torch.zeros(1, 4, H, W)
-    results = []
-    for cls, settings in ((ref.multidiffusion.MultiDiffusion, {i: ref.utils.BBoxSettings(*r) for i, r in enumerate(ROWS)}),
-                          (MultiDiffusion, {i: r for i, r in enumerate(ROWS)})):
-        ref.shared.state.sampling_step = 0
-        d, sampler, p, cache = _job(ref, cls, settings, bg, with_regions)
-        assert sampler.sample_img2img.__func__ is not None          # replaced by a bound method of the sampler
-        first = sampler.sample_img2img(p, x, noise, None, None)
-        assert cache["sets"] == 1
-        second = sampler.sample_img2img(p, x, noise, None, None)     # cache hit: no second inversion
-        assert cache["sets"] == 1
-        results.append((first, second, cache["v"].xt))
-    (rf, rs, rxt), (of, os_, oxt) = results
-    assert of[0] == rf[0] == "sampled" and of[3] == rf[3]
-    assert torch.equal(oxt, rxt), "inverted latent"
-    assert torch.equal(of[2], rf[2]), "combined noise"
-    assert torch.equal(os_[2], rs[2]), "combined noise from the cache"
-    assert torch.isfinite(of[2]).all() and not torch.equal(of[2], noise)
+    stubs.shared.state.sampling_step = 0
+    d, sampler, p, cache = _job(stubs, cls, settings, cache_cls, bg, with_regions)
+    assert sampler.sample_img2img.__func__ is not None          # replaced by a bound method of the sampler
+    first = sampler.sample_img2img(p, x, noise, None, None)
+    assert cache["sets"] == 1
+    second = sampler.sample_img2img(p, x, noise, None, None)     # cache hit: no second inversion
+    assert cache["sets"] == 1
+    assert first[0] == "sampled"
+    assert torch.isfinite(first[2]).all() and not torch.equal(first[2], noise)
     host._a1111_cache.clear()
+    return " ".join(digest(t) for t in (cache["v"].xt, first[2], second[2], first[3]))
+
+
+def reference_records(ref):
+    """The reference's side of every comparison below (run by oracle/make_golden.py)."""
+    return {f"noise_inverse_{mode}": _record(mode, ref) for mode in MODES}
+
+
+@pytest.mark.parametrize("mode", MODES)
+def test_noise_inversion_like_the_reference(monkeypatch, golden_dir, mode):
+    _oracle_engine(monkeypatch)
+    got = _record(mode).split()
+    want = host_record(golden_dir, f"noise_inverse_{mode}").split()
+    for what, g, w in zip(("inverted latent", "combined noise", "combined noise from the cache", "steps"), got, want):
+        assert g == w, what

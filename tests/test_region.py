@@ -13,7 +13,7 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import region_composite_reference, DTYPES, assert_bit_equal
+from helpers import load_golden, region_composite_reference, DTYPES, assert_bit_equal
 from oracle import blend, region, synth, tiling
 from oracle.make_golden import REGION_CASES, REGION_DTYPES, REGION_GRID
 
@@ -22,7 +22,7 @@ G = REGION_GRID
 
 @pytest.fixture(scope="module")
 def gold(golden_dir):
-    return np.load(os.path.join(golden_dir, "region_small.npz"))
+    return load_golden(golden_dir, "region_small")
 
 
 def _want(gold, key):
@@ -132,11 +132,11 @@ def _oracle_engine(monkeypatch):
         blend.accumulate_md(buf, torch.cat(list(outs), dim=0), bbs(g), N)
         if x_buffer is not None:
             x_buffer.copy_(buf)
-        return blend.normalise_md(buf, weights)
+        return blend.normalise_md(buf, weights.to(buf.device))
 
     def blend_mixture(g, outs, N, C, tile_bs, tile_weights, rescale, x_buffer, flags=0):
         x_buffer.zero_()
-        blend.accumulate_mod(x_buffer, torch.cat(list(outs), dim=0), bbs(g), N, tile_weights, rescale)
+        blend.accumulate_mod(x_buffer, torch.cat(list(outs), dim=0), bbs(g), N, tile_weights.to(x_buffer.device), rescale.to(x_buffer.device))
         return x_buffer
 
     monkeypatch.setattr(engine, "region_composite", region_composite_reference)

@@ -1,15 +1,17 @@
 """ControlNet / StableSR tile caches (SURVEY.md section 8(f)-2): the per-batch hint tiles our delegate caches and
 hands to the extension objects must equal the reference's, for k-diffusion and DDIM samplers, grid and custom bboxes.
 
-CPU: the UNMODIFIED reference (oracle/ref_shim.py) next to our delegate, with the scatter kernel swapped for the
-oracle's scatter (the kernel itself is pinned by tests/test_gpu_diffusion.py).  GPU: the same caches through
-td_scatter_tiles on the x8-scaled tile plan, against plain slicing.
+CPU: our delegate under the stub host (oracle/ref_shim.py), with the scatter kernel swapped for the oracle's scatter
+(the kernel itself is pinned by tests/test_gpu_diffusion.py), against the UNMODIFIED reference's caches in the same
+sequence of calls, recorded by `reference_records` (oracle/make_golden.py -> tests/golden/host_records.npz).  GPU: the
+same caches through td_scatter_tiles on the x8-scaled tile plan, against plain slicing.
 """
 import types
 
 import pytest
 import torch
 
+from helpers import digest, host_record
 from oracle import blend, ref_shim
 
 W, H = 64, 48
@@ -50,99 +52,111 @@ def _delegate(cls, sampler, settings, with_regions):
     return d
 
 
-@pytest.mark.skipif(not ref_shim.available(), reason="reference tree not present")
+def _settings(ref):
+    if ref is None:
+        from multidiffusion_upscaler_for_automatic1111_b200 import MultiDiffusion
+        return MultiDiffusion, {i: r for i, r in enumerate(ROWS)}
+    return ref.multidiffusion.MultiDiffusion, {i: ref.utils.BBoxSettings(*r) for i, r in enumerate(ROWS)}
+
+
+CONTROLNET_CASES = [(kdiff, with_regions, tensor_cpu) for tensor_cpu in (False, True) for with_regions in (False, True) for kdiff in (True, False)]
+
+
+def _controlnet_trace(kdiff, with_regions, tensor_cpu, ref=None):
+    """Digests of every hint tensor our delegate (or the reference's, `ref` given) caches and hands to the ControlNet
+    script, in call order."""
+    from multidiffusion_upscaler_for_automatic1111_b200 import host
+    stubs = ref_shim.host_stubs()
+    host._a1111_cache.clear()
+    if kdiff:
+        sampler = ref_shim.make_kdiff_sampler(lambda x, s, cond=None: x)
+    else:
+        class _S(stubs.CompVisSampler):
+            pass
+        sampler = _S()
+        sampler.model_wrap_cfg = types.SimpleNamespace(inner_model=types.SimpleNamespace(forward=None), image_cfg_scale=None, step=0)
+    cls, settings = _settings(ref)
+    d = _delegate(cls, sampler, settings, with_regions)
+    assert d.is_kdiff == kdiff
+    cs = _controlnet_script()
+    d.init_controlnet(cs, tensor_cpu)
+    d.init_done()
+    if getattr(d, "pbar", None) is not None:
+        d.pbar.disable = True
+    trace = [d.num_batches, [len(bb) for bb in d.batched_bboxes]]
+    assert len(d.control_tensor_batch) == 2
+    trace.append(("batch", [list(pr) for pr in d.control_tensor_batch]))
+    if with_regions:
+        trace.append(("custom", [list(pr) for pr in d.control_tensor_custom]))
+    for batch_id in (0, d.num_batches - 1):
+        n_tiles = len(d.batched_bboxes[batch_id])
+        for is_denoise in (False, True):
+            d.switch_controlnet_tensors(batch_id, 2, n_tiles, is_denoise=is_denoise)
+            trace.append(("switch", batch_id, is_denoise, [q.hint_cond for q in cs.latest_network.control_params]))
+    if with_regions:
+        d.set_custom_controlnet_tensors(1, 3)
+        trace.append(("set_custom", [q.hint_cond for q in cs.latest_network.control_params]))
+    d.reset_controlnet_tensors()
+    assert all(q.hint_cond.shape == (1, 3, H * 8, W * 8) for q in cs.latest_network.control_params)
+    trace.append(("reset", [q.hint_cond for q in cs.latest_network.control_params]))
+    host._a1111_cache.clear()
+    return [digest(t) for t in trace]
+
+
+def _stablesr_trace(ref=None):
+    from multidiffusion_upscaler_for_automatic1111_b200 import host
+    ref_shim.host_stubs()
+    host._a1111_cache.clear()
+    latent = torch.arange(2 * 4 * H * W, dtype=torch.float32).view(2, 4, H, W)
+    cls, settings = _settings(ref)
+    d = _delegate(cls, ref_shim.make_kdiff_sampler(lambda x, s, cond=None: x), settings, True)
+    model = types.SimpleNamespace(set_image_hooks={}, latent_image=None)
+    d.init_stablesr(types.SimpleNamespace(stablesr_model=model))
+    d.init_done()
+    if getattr(d, "pbar", None) is not None:
+        d.pbar.disable = True
+    model.set_image_hooks["TiledDiffusion"](latent)
+    assert d.enable_stablesr
+    trace = [d.num_batches, len(d.stablesr_tensor_batch)]
+    for b in range(d.num_batches):
+        d.switch_stablesr_tensors(b)
+        trace.append(model.latent_image)
+    d.set_custom_stablesr_tensors(1)
+    trace.append(model.latent_image)
+    d.reset_stablesr_tensors()
+    assert model.latent_image is latent
+    host._a1111_cache.clear()
+    return [digest(t) for t in trace]
+
+
+def _cn_key(kdiff, with_regions, tensor_cpu):
+    return f"controlnet_{'kdiff' if kdiff else 'ddim'}_{'regions' if with_regions else 'grid'}_{'cpu' if tensor_cpu else 'dev'}"
+
+
+def reference_records(ref):
+    """The reference's side of every comparison below (run by oracle/make_golden.py)."""
+    out = {_cn_key(*c): " ".join(_controlnet_trace(*c, ref=ref)) for c in CONTROLNET_CASES}
+    out["stablesr"] = " ".join(_stablesr_trace(ref))
+    return out
+
+
+def _same_trace(got, want):
+    assert len(got) == len(want)
+    for i, (g, w) in enumerate(zip(got, want)):
+        assert g == w, f"trace entry {i} differs from the reference's"
+
+
 @pytest.mark.parametrize("kdiff", [True, False], ids=["kdiff", "ddim"])
 @pytest.mark.parametrize("with_regions", [False, True], ids=["grid", "grid+regions"])
 @pytest.mark.parametrize("tensor_cpu", [False, True], ids=["dev", "cpu_cache"])
-def test_controlnet_tile_caches_like_the_reference(monkeypatch, kdiff, with_regions, tensor_cpu):
-    from multidiffusion_upscaler_for_automatic1111_b200 import MultiDiffusion, host
-    ref = ref_shim.load()
-    host._a1111_cache.clear()
+def test_controlnet_tile_caches_like_the_reference(monkeypatch, golden_dir, kdiff, with_regions, tensor_cpu):
     _oracle_scatter(monkeypatch)
-
-    def sampler():
-        if kdiff:
-            return ref_shim.make_kdiff_sampler(lambda x, s, cond=None: x)
-
-        class _S(ref.CompVisSampler):
-            pass
-        s = _S()
-        s.model_wrap_cfg = types.SimpleNamespace(inner_model=types.SimpleNamespace(forward=None), image_cfg_scale=None, step=0)
-        return s
-
-    d_ref = _delegate(ref.multidiffusion.MultiDiffusion, sampler(), {i: ref.utils.BBoxSettings(*r) for i, r in enumerate(ROWS)}, with_regions)
-    d_our = _delegate(MultiDiffusion, sampler(), {i: r for i, r in enumerate(ROWS)}, with_regions)
-    assert d_our.is_kdiff == kdiff == d_ref.is_kdiff
-    scripts = []
-    for d in (d_ref, d_our):
-        cs = _controlnet_script()
-        scripts.append(cs)
-        d.init_controlnet(cs, tensor_cpu)
-        d.init_done()
-        if getattr(d, "pbar", None) is not None:
-            d.pbar.disable = True
-    cs_ref, cs_our = scripts
-
-    assert len(d_our.control_tensor_batch) == len(d_ref.control_tensor_batch) == 2
-    for pr, po in zip(d_ref.control_tensor_batch, d_our.control_tensor_batch):
-        assert len(pr) == len(po) == d_ref.num_batches
-        for tr, to in zip(pr, po):
-            assert tr.shape == to.shape and torch.equal(tr, to)
-    if with_regions:
-        for pr, po in zip(d_ref.control_tensor_custom, d_our.control_tensor_custom):
-            for tr, to in zip(pr, po):
-                assert torch.equal(tr, to)
-
-    for batch_id in (0, d_ref.num_batches - 1):
-        n_tiles = len(d_ref.batched_bboxes[batch_id])
-        for is_denoise in (False, True):
-            for d in (d_ref, d_our):
-                d.switch_controlnet_tensors(batch_id, 2, n_tiles, is_denoise=is_denoise)
-            for a, b in zip(cs_ref.latest_network.control_params, cs_our.latest_network.control_params):
-                assert a.hint_cond.shape == b.hint_cond.shape and torch.equal(a.hint_cond, b.hint_cond)
-    if with_regions:
-        for d in (d_ref, d_our):
-            d.set_custom_controlnet_tensors(1, 3)
-        for a, b in zip(cs_ref.latest_network.control_params, cs_our.latest_network.control_params):
-            assert torch.equal(a.hint_cond, b.hint_cond)
-    for d in (d_ref, d_our):
-        d.reset_controlnet_tensors()
-    for a, b in zip(cs_ref.latest_network.control_params, cs_our.latest_network.control_params):
-        assert a.hint_cond.shape == (1, 3, H * 8, W * 8) and torch.equal(a.hint_cond, b.hint_cond)
-    host._a1111_cache.clear()
+    _same_trace(_controlnet_trace(kdiff, with_regions, tensor_cpu), host_record(golden_dir, _cn_key(kdiff, with_regions, tensor_cpu)).split())
 
 
-@pytest.mark.skipif(not ref_shim.available(), reason="reference tree not present")
-def test_stablesr_tile_caches_like_the_reference(monkeypatch):
-    from multidiffusion_upscaler_for_automatic1111_b200 import MultiDiffusion, host
-    ref = ref_shim.load()
-    host._a1111_cache.clear()
+def test_stablesr_tile_caches_like_the_reference(monkeypatch, golden_dir):
     _oracle_scatter(monkeypatch)
-    latent = torch.arange(2 * 4 * H * W, dtype=torch.float32).view(2, 4, H, W)
-    models = []
-    for cls, settings in ((ref.multidiffusion.MultiDiffusion, {i: ref.utils.BBoxSettings(*r) for i, r in enumerate(ROWS)}),
-                          (MultiDiffusion, {i: r for i, r in enumerate(ROWS)})):
-        d = _delegate(cls, ref_shim.make_kdiff_sampler(lambda x, s, cond=None: x), settings, True)
-        model = types.SimpleNamespace(set_image_hooks={}, latent_image=None)
-        d.init_stablesr(types.SimpleNamespace(stablesr_model=model))
-        d.init_done()
-        if getattr(d, "pbar", None) is not None:
-            d.pbar.disable = True
-        model.set_image_hooks["TiledDiffusion"](latent)
-        models.append((d, model))
-    (d_ref, m_ref), (d_our, m_our) = models
-    assert d_our.enable_stablesr and len(d_our.stablesr_tensor_batch) == len(d_ref.stablesr_tensor_batch)
-    for b in range(d_ref.num_batches):
-        for d in (d_ref, d_our):
-            d.switch_stablesr_tensors(b)
-        assert m_ref.latent_image.shape == m_our.latent_image.shape and torch.equal(m_ref.latent_image, m_our.latent_image)
-    for d in (d_ref, d_our):
-        d.set_custom_stablesr_tensors(1)
-    assert torch.equal(m_ref.latent_image, m_our.latent_image)
-    for d in (d_ref, d_our):
-        d.reset_stablesr_tensors()
-    assert m_our.latent_image is latent and m_ref.latent_image is latent
-    host._a1111_cache.clear()
+    _same_trace(_stablesr_trace(), host_record(golden_dir, "stablesr").split())
 
 
 def test_scaled_grid_is_the_tile_plan_times_opt_f():
