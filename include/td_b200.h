@@ -39,16 +39,18 @@ typedef enum td_dtype { TD_F16 = 0, TD_BF16 = 1, TD_F32 = 2 } td_dtype;
 
 /* blend flags */
 #define TD_FLAG_FORCE_GENERIC 1u /* use the scalar any-alignment kernel (test / fallback path) */
-#define TD_FLAG_NO_TMA 2u        /* use the register-staged vector kernels (no smem staging)      */
+#define TD_FLAG_NO_TMA 2u        /* use the register-staged vector kernels (no smem staging): scatter_vec_kernel
+                                    instead of the row-block scatter, the register-staged blends */
 #define TD_FLAG_TMA 4u           /* blend: use the TMA-staged kernel instead of the cp.async one   */
 #define TD_FLAG_PIPELINE 8u      /* blend: persistent software-pipelined cp.async form (measured slower) */
 #define TD_FLAG_PEER_ASYNC 16u   /* peer blend: stage peer tiles with cp.async instead of direct 128-bit loads */
 #define TD_FLAG_NO_PDL 32u       /* launch without the programmatic-dependent-launch attribute (A/B measurement) */
-#define TD_FLAG_ONE_PLANE 64u    /* cp.async blend: one (n, c) plane per CTA instead of two (A/B measurement) */
+#define TD_FLAG_ONE_PLANE 64u    /* cp.async blend: one (n, c) plane per CTA (the default of a TD_AS_PPC=1 build) */
 #define TD_FLAG_STRIP 128u       /* MultiDiffusion blend: strip CTAs (8 rows x full width), opt-in, see csrc/td_strip.cu */
 #define TD_FLAG_DBG_NO_TILES 0x100u /* measurement aid: skip all tile visits (launch + epilogue floor) */
-#define TD_FLAG_ROWS 0x400u      /* row-block form (csrc/td_rows.cu: one persistent CTA per SM, bulk-copy staging), opt-in: bit-identical,
-                                    the default kernels stay many small co-resident CTAs (DESIGN.md section 4) */
+#define TD_FLAG_ROWS 0x400u      /* row-block form (csrc/td_rows.cu: one persistent CTA per SM, bulk-copy staging), bit-identical:
+                                    the scatter's default; opt-in for the blends, whose defaults stay many small co-resident
+                                    CTAs (DESIGN.md section 4) */
 
 #define TD_MAX_GRID_DIM 256   /* max tile rows / cols of a grid plan            */
 #define TD_MAX_BATCH_PTRS 128 /* max UNet output batch tensors per blend launch */

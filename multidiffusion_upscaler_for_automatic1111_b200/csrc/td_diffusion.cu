@@ -16,6 +16,9 @@
 //   * Grid geometry (<= 256 row + 256 col origins) and the UNet's per-batch output
 //     pointers travel in the kernel parameter block: no device tables, no H2D.
 //   * All memory-bound: no tensor cores here on purpose.
+//   * Defaults on H100 (DESIGN.md 4.4): the scatter is the row-block form of td_rows.cu
+//     (scatter_vec_kernel where it does not apply, or with TD_FLAG_NO_TMA), both launched
+//     with PDL; the MultiDiffusion blend is blend_md_async_kernel with one plane per CTA.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -80,11 +83,23 @@ __device__ __forceinline__ void load_origins(const GeomParams& g, short* s_ys, s
 // floor(n / d) for n, d < 2^16 with magic = ceil(2^32 / d); d == 1 is passed as magic 0.
 __device__ __forceinline__ unsigned fastdiv(unsigned n, unsigned magic) { return magic ? __umulhi(n, magic) : n; }
 
+// Programmatic dependent launch (sm_90+): a kernel launched with the stream-serialisation attribute may become
+// resident while its predecessor in the stream drains.  pdl_wait() blocks until the predecessor has completed and
+// its memory is visible -- it precedes every global read or write below, so stream order is kept; what overlaps
+// is the launch itself, the parameter fetch and the index arithmetic.  Both are no-ops for an ordinary launch.
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+
 // ---------------------------------------------------------------------------
-// Scatter, vector path.  One block = `rows_per_block` rows of one (tile, n, c)
+// Scatter, vector path (the default).  One block = `rows_per_block` rows of one (tile, n, c)
 // plane; tile origin and the funnel shift are block-uniform.  Each thread moves
 // 16-byte vectors: two aligned 128-bit loads of the (misaligned) canvas row,
 // one aligned 128-bit store into the tile batch; 4 vectors in flight per thread.
+// Launched with PDL.  A TMA-staged form (aligned-superset boxes through shared memory,
+// re-aligned by the threads) measured slower (DESIGN.md 4.4).  A pure bulk copy -- a
+// tensor-map box loaded at the tile's exact origin, stored back with cp.async.bulk -- does
+// not apply at cfg2: its origins (0, 46, 92, ...) are not 16-byte aligned, and a box whose
+// innermost start is not 16-byte aligned faults with an illegal instruction (td_tma.cuh).
 // ---------------------------------------------------------------------------
 template <typename T>
 __global__ void __launch_bounds__(128)
@@ -105,6 +120,8 @@ scatter_vec_kernel(const __grid_constant__ GeomParams g, const T* __restrict__ x
     const int s = xs & (VEC - 1), k0 = xs >> L2V;         // block-uniform shift
     const T* src = x + ((long long)plane * g.H + ys + v0) * g.W;
     T* dst = tiles + ((long long)tp * g.th + v0) * g.tw;
+    pdl_launch_dependents();
+    pdl_wait();   // x is read and tiles are written only after the previous kernel in the stream has completed
     for (int base = threadIdx.x; base < nvec; base += 128 * UNROLL) {
         uint4 A[UNROLL], B[UNROLL];
 #pragma unroll
@@ -429,13 +446,6 @@ __device__ __forceinline__ float div_exact_small_int(float a, float w, float rcp
     // w > 0: the quotient carries a's sign (this also keeps -0 / w = -0, which the fma chain turns into +0)
     return __uint_as_float((__float_as_uint(q2) & 0x7fffffffu) | (__float_as_uint(a) & 0x80000000u));
 }
-
-// Programmatic dependent launch (sm_90+): a kernel launched with the stream-serialisation attribute may become
-// resident while its predecessor in the stream drains.  pdl_wait() blocks until the predecessor has completed and
-// its memory is visible -- it precedes every global read or write below, so stream order is kept; what overlaps
-// is the launch itself, the parameter fetch and the index arithmetic.  Both are no-ops for an ordinary launch.
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
 struct __align__(16) VisitEntry {   // per tile visit of a CTA, computed once by one thread
     long long origin;               // byte address of tile element (v0, k0*VEC) of this plane (may lie before the tile)
@@ -1031,92 +1041,6 @@ blend_md_tma_kernel(const __grid_constant__ TmaBlendParams<NB> p, const float* _
     if constexpr (WRITE_BUF) stg128(out_buf + o, acc);
 }
 
-// ---------------------------------------------------------------------------
-// Scatter, TMA path: a CTA moves one whole (tile, n, c) plane.  One thread issues up to
-// kScBoxes box loads (aligned superset of `rb` tile rows each, one mbarrier per box) from
-// the canvas, all in flight at once; the threads then walk the boxes in order: re-align
-// (two LDS.128 + funnel shift specialised on the block-uniform shift) and write the tile
-// batch with aligned 128-bit stores, so the first stores overlap the later loads.
-// ---------------------------------------------------------------------------
-constexpr int kScBoxes = 8;
-constexpr int kScThreads = 256;
-
-struct TmaScatterParams {
-    GeomParams g;
-    CUtensorMap src;   // canvas  [N*C][H][W], box [1][rb][tw + VEC]
-};
-
-template <typename T, int S>
-__device__ __forceinline__ void scatter_rows(const unsigned char* box, T* dst, int nvec, int twv, unsigned twv_magic, int pitch) {
-    for (int i = threadIdx.x; i < nvec; i += kScThreads) {
-        const unsigned vi = fastdiv((unsigned)i, twv_magic);
-        const int uv = i - (int)vi * twv;
-        const unsigned char* src = box + (size_t)vi * pitch + (size_t)uv * 16;
-        const uint4 A = lds128(src);
-        uint4 e = A;
-        if constexpr (S != 0) e = Vec<T>::window(A, lds128(src + 16), S);
-        stg128(dst + (long long)i * Vec<T>::kElems, e);
-    }
-}
-
-template <typename T>
-__global__ void __launch_bounds__(kScThreads)
-scatter_tma_kernel(const __grid_constant__ TmaScatterParams p, T* __restrict__ tiles, int tile_begin, int rb, int nboxes, int box_bytes) {
-    constexpr int VEC = Vec<T>::kElems;
-    constexpr int L2V = Vec<T>::kLog2;
-    extern __shared__ __align__(128) unsigned char td_smem[];
-    __shared__ uint64_t bars[kScBoxes];
-    const GeomParams& g = p.g;
-    const unsigned tp = blockIdx.x;
-    const unsigned tl = fastdiv(tp, g.nc_magic);
-    const int plane = (int)(tp - tl * (unsigned)(g.N * g.C));
-    const int t = tile_begin + (int)tl;
-    const int r = t / g.cols, c = t - r * g.cols;
-    const int xs = (int)g.xs[c], ys = (int)g.ys[r];
-    const int pitch = (g.tw + VEC) * (int)sizeof(T);
-    pdl_launch_dependents();
-    if (threadIdx.x == 0) {
-        for (int b = 0; b < nboxes; ++b) mbar_init(&bars[b], 1);
-        fence_proxy_async();
-    }
-    pdl_wait();   // x is read (TMA) and tiles are written only after the previous kernel in the stream has completed
-    if (threadIdx.x == 0) {
-        for (int b = 0; b < nboxes; ++b) {
-            mbar_arrive_expect_tx(&bars[b], (uint32_t)(pitch * rb));
-            tma_load_3d(td_smem + (size_t)b * box_bytes, &p.src, (xs >> L2V) * VEC, ys + b * rb, plane, &bars[b]);
-        }
-    }
-    __syncthreads();
-    const int s = xs & (VEC - 1);
-    const int twv = g.tw >> L2V;
-    T* dst = tiles + (long long)tp * g.th * g.tw;
-    for (int b = 0; b < nboxes; ++b) {
-        const int nvec = min(rb, g.th - b * rb) * twv;
-        const unsigned char* box = td_smem + (size_t)b * box_bytes;
-        T* d = dst + (long long)b * rb * g.tw;
-        mbar_wait(&bars[b], 0);
-        if constexpr (VEC == 8) {
-            switch (s) {
-                case 0: scatter_rows<T, 0>(box, d, nvec, twv, g.twv_magic, pitch); break;
-                case 1: scatter_rows<T, 1>(box, d, nvec, twv, g.twv_magic, pitch); break;
-                case 2: scatter_rows<T, 2>(box, d, nvec, twv, g.twv_magic, pitch); break;
-                case 3: scatter_rows<T, 3>(box, d, nvec, twv, g.twv_magic, pitch); break;
-                case 4: scatter_rows<T, 4>(box, d, nvec, twv, g.twv_magic, pitch); break;
-                case 5: scatter_rows<T, 5>(box, d, nvec, twv, g.twv_magic, pitch); break;
-                case 6: scatter_rows<T, 6>(box, d, nvec, twv, g.twv_magic, pitch); break;
-                default: scatter_rows<T, 7>(box, d, nvec, twv, g.twv_magic, pitch); break;
-            }
-        } else {
-            switch (s) {
-                case 0: scatter_rows<T, 0>(box, d, nvec, twv, g.twv_magic, pitch); break;
-                case 1: scatter_rows<T, 1>(box, d, nvec, twv, g.twv_magic, pitch); break;
-                case 2: scatter_rows<T, 2>(box, d, nvec, twv, g.twv_magic, pitch); break;
-                default: scatter_rows<T, 3>(box, d, nvec, twv, g.twv_magic, pitch); break;
-            }
-        }
-    }
-}
-
 // Blend, generic path: one element per thread, any width / alignment, tile
 // dtype and canvas dtype independent.
 template <typename TIn, typename TAcc, int MODE>
@@ -1236,7 +1160,7 @@ int launch_scatter(GeomParams gp, const void* x, void* tiles, int tile_begin, in
         const int rows_per_block = std::max(1, std::min(gp.th, (128 * 4 + twv - 1) / twv));  // ~4 vectors per thread
         if ((long long)rows_per_block * twv >= 65536) { td_set_error("tile row too wide for the vector scatter"); return TD_ERR_UNSUPPORTED; }
         dim3 grid((unsigned)(n_tiles * gp.N * gp.C), (unsigned)((gp.th + rows_per_block - 1) / rows_per_block));
-        scatter_vec_kernel<T><<<grid, 128, 0, st>>>(gp, (const T*)x, (T*)tiles, tile_begin, rows_per_block);
+        launch_pdl(scatter_vec_kernel<T>, grid, dim3(128), 0, st, gp, (const T*)x, (T*)tiles, tile_begin, rows_per_block);
     } else {
         scatter_generic_kernel<T><<<blocks_for(elems, 256), 256, 0, st>>>(gp, (const T*)x, (T*)tiles, tile_begin, elems);
     }
@@ -1342,39 +1266,6 @@ int try_launch_blend_tma(const td_grid* g, const BlendParams& bp, int tile_dtype
               : launch_blend_tma_nb<T, false, TD_MAX_BATCH_PTRS>(g, bp, tile_dtype, weights, out_f32, out_buf, nv_cap, st);
 }
 
-template <typename T>
-int try_launch_scatter_tma(GeomParams gp, const void* x, void* tiles, int dtype, int tile_begin, int n_tiles, cudaStream_t st) {
-    constexpr int VEC = Vec<T>::kElems;
-    const int es = (int)sizeof(T);
-    if (gp.tw + VEC > 256 || n_tiles <= 0) return 1;
-    const long long planes_out = (long long)n_tiles * gp.N * gp.C;
-    if (planes_out > 0x7fffffffLL) return 1;
-    const int pitch = (gp.tw + VEC) * es;
-    // whole plane per CTA in <= kScBoxes boxes of rb rows (<= 256 rows per box, ~8 KB each when possible)
-    int rb = std::max(1, std::min(256, 8192 / pitch));
-    rb = std::max(rb, (gp.th + kScBoxes - 1) / kScBoxes);
-    if (rb > 256) return 1;
-    const int nboxes = (gp.th + rb - 1) / rb;
-    const int box_bytes = (rb * pitch + 127) / 128 * 128;
-    const int smem = nboxes * box_bytes;
-    if (smem > 200 * 1024) return 1;
-    const int twv = gp.tw / VEC;
-    if ((long long)rb * twv >= 65536) return 1;
-    gp.twv_magic = magic_u16((unsigned)twv);
-    static TmaScatterParams tp;
-    static std::mutex mu;
-    std::lock_guard<std::mutex> lk(mu);
-    tp.g = gp;
-    int rc = td_encode_tensor_map_3d(&tp.src, x, dtype, (uint64_t)gp.N * gp.C, (uint64_t)gp.H, (uint64_t)gp.W, (uint32_t)rb,
-                                     (uint32_t)(gp.tw + VEC));
-    if (rc != TD_OK) return rc;
-    static SmemOptIn configured;
-    rc = ensure_dyn_smem(scatter_tma_kernel<T>, smem, &configured);
-    if (rc != TD_OK) return rc;
-    launch_pdl(scatter_tma_kernel<T>, dim3((unsigned)planes_out), dim3(kScThreads), (size_t)smem, st, tp, (T*)tiles, tile_begin, rb, nboxes, box_bytes);
-    return check_launch("td_scatter_tiles (tma)");
-}
-
 // tiles touching each patch along one axis: first index and count (both fit a byte: <= 256 tiles per axis)
 void fill_patch_table(const int32_t* org, int n, int extent, int size, int patch, unsigned char* lo_out, unsigned char* n_out) {
     int idx = 0;
@@ -1416,7 +1307,7 @@ int launch_blend_async_ppc(const BlendParams& bp, const float* weights, const fl
 
 // planes per CTA (tl_ppc_max is set per C-ABI call: TD_FLAG_ONE_PLANE forces 1)
 #ifndef TD_AS_PPC
-#define TD_AS_PPC 2   // tuning knob (-DTD_AS_PPC=): 1 / 2 / 4
+#define TD_AS_PPC 1   // tuning knob (-DTD_AS_PPC=): 1 / 2 / 4; cfg2 blend 12.5 us at 1 vs 13.35 us at 2 (H100 80GB HBM3, 700 W)
 #endif
 thread_local int tl_ppc_max = TD_AS_PPC;
 
@@ -1607,14 +1498,9 @@ extern "C" int td_scatter_tiles(const td_grid* g, const void* x, void* tiles, in
     tl_pdl = !(flags & TD_FLAG_NO_PDL);
     const bool vec_ok = !(flags & TD_FLAG_FORCE_GENERIC) && gp.W % vec == 0 && gp.tw % vec == 0 && aligned16(x) && aligned16(tiles);
     cudaStream_t s = (cudaStream_t)stream;
-    if (vec_ok && (flags & TD_FLAG_ROWS)) {   // opt-in: row-block form (td_rows.cu); falls through when not applicable
+    if (vec_ok && !(flags & TD_FLAG_NO_TMA)) {   // default: row-block form (td_rows.cu); falls through when not applicable
         const int rc = td_rows_try_launch_scatter(g, x, tiles, N, C, dtype, tile_begin, tile_end, (flags & TD_FLAG_NO_PDL) ? 0 : 1, stream);
         if (rc <= 0) return rc;
-    }
-    if (vec_ok && !(flags & TD_FLAG_NO_TMA)) {
-        const int rc = es == 2 ? try_launch_scatter_tma<__half>(gp, x, tiles, dtype, tile_begin, tile_end - tile_begin, s)
-                               : try_launch_scatter_tma<float>(gp, x, tiles, dtype, tile_begin, tile_end - tile_begin, s);
-        if (rc <= 0) return rc;   // launched (0) or hard error (<0); 1 = not applicable -> vector kernel
     }
     // fp16 and bf16 are both moved as opaque 16-bit words
     if (es == 2) return launch_scatter<__half>(gp, x, tiles, tile_begin, tile_end - tile_begin, vec_ok, s);
