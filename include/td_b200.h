@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define TD_ABI_VERSION 6
+#define TD_ABI_VERSION 7
 
 typedef enum td_status {
     TD_OK = 0,
@@ -383,6 +383,15 @@ int td_conv2d_nhwc(const td_conv_desc* d, const void* x, const void* w, const fl
  * H x W input, OH = 2H, OW = 2W, kh = kw = 3, stride 1, pad 1; w16: folded taps [16 = (py*2+px)*4 + ty*2 + tx][Cout][w_pitch]
  * (fold in fp32, round once: vae_ops.fold_upsample_weight); no residual; the post_scale / post_shift stage applies. */
 int td_upconv2x_nhwc(const td_conv_desc* d, const void* x, const void* w16, const float* bias, void* y, void* stream);
+
+/* The mid-block's single-head attention core (tile_utils/attn.py:49-72: q·kᵀ scaled by alpha, softmax over the keys,
+ * times v) fused into one kernel with an online softmax (csrc/td_attn.cu):
+ *   o[t, :] = softmax_s(alpha * sum_c q[t, c] k[s, c]) v[s, :]      t, s < T
+ * q / k / v / o: token-major [T, pitch >= C] fp16 or bf16 (pitches in elements, multiples of 8; 16-byte aligned);
+ * fp32 accumulation; C % 64 == 0 and C <= 512 (else TD_ERR_UNSUPPORTED); any T >= 1.  Nothing of size T x T is
+ * written: the call needs no memory beyond its four operands.  One rounding of o to the storage dtype. */
+int td_attention(const void* q, const void* k, const void* v, void* o, int T, int C, int64_t q_pitch, int64_t k_pitch,
+                 int64_t v_pitch, int64_t o_pitch, float alpha, int dtype, void* stream);
 
 /* Channels-last (NHWC) streaming kernels around the tensor-core convolutions (csrc/td_nhwc.cu).  fp16 / bf16.
  *

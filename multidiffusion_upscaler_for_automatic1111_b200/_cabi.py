@@ -32,7 +32,7 @@ TD_MAX_GRID_DIM = 256
 TD_MAX_BATCH_PTRS = 128
 TD_MAX_PEERS = 16
 TD_IPC_HANDLE_BYTES = 64
-ABI_VERSION = 6
+ABI_VERSION = 7
 
 DTYPE_CODE = {torch.float16: TD_F16, torch.bfloat16: TD_BF16, torch.float32: TD_F32}
 
@@ -140,6 +140,8 @@ _SIGNATURES = {
     "td_depthwise_conv2d": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, POINTER(c_float), c_int, c_int, c_void_p]),
     "td_conv2d_nhwc": (c_int, [POINTER(TdConvDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "td_upconv2x_nhwc": (c_int, [POINTER(TdConvDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "td_attention": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int64, c_int64, c_int64, c_int64, c_float, c_int,
+                             c_void_p]),
     "td_nchw_to_nhwc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int64, c_int64, c_int64, c_int, c_int, c_void_p]),
     "td_nhwc_to_nchw_region": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int64, c_int, c_int64, c_int64, c_int64, c_int64,
                                        c_int, c_void_p]),

@@ -257,26 +257,6 @@ EncodeTiledFn conv_encode_fn() {
     return fn;
 }
 
-int encode_map(CUtensorMap* out, const void* base, int is_bf16, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-               const uint32_t* box, const uint32_t* estr, bool swizzle128, const char* what) {
-    EncodeTiledFn fn = conv_encode_fn();
-    if (fn == nullptr) { td_set_error("cuTensorMapEncodeTiled is not available from this driver"); return TD_ERR_CUDA; }
-    cuuint64_t d[5]; cuuint64_t s[4]; cuuint32_t b[5]; cuuint32_t e[5];
-    for (int i = 0; i < rank; ++i) { d[i] = dims[i]; b[i] = box[i]; e[i] = estr[i]; }
-    for (int i = 0; i + 1 < rank; ++i) s[i] = strides_bytes[i];
-    const CUresult r = fn(out, is_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank,
-                          const_cast<void*>(base), d, s, b, e, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                          swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-        td_set_error("cuTensorMapEncodeTiled failed (%d) for %s: dims [%llu,%llu,%llu,%llu] box [%u,%u,%u,%u]", (int)r, what,
-                     (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)(rank > 2 ? dims[2] : 0),
-                     (unsigned long long)(rank > 3 ? dims[3] : 0), box[0], box[1], rank > 2 ? box[2] : 0, rank > 3 ? box[3] : 0);
-        return TD_ERR_CUDA;
-    }
-    return TD_OK;
-}
-
 template <int BN> bool conv_smem_optin(int bytes) {
     return cudaFuncSetAttribute(conv_gemm_kernel<BN, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) == cudaSuccess &&
            cudaFuncSetAttribute(conv_gemm_kernel<BN, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) == cudaSuccess;
@@ -313,6 +293,26 @@ ConvDev conv_dev() {
 }
 
 }  // namespace
+
+int td_encode_map(CUtensorMap* out, const void* base, int is_bf16, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
+                  const uint32_t* box, const uint32_t* estr, bool swizzle128, const char* what) {
+    EncodeTiledFn fn = conv_encode_fn();
+    if (fn == nullptr) { td_set_error("cuTensorMapEncodeTiled is not available from this driver"); return TD_ERR_CUDA; }
+    cuuint64_t d[5]; cuuint64_t s[4]; cuuint32_t b[5]; cuuint32_t e[5];
+    for (int i = 0; i < rank; ++i) { d[i] = dims[i]; b[i] = box[i]; e[i] = estr[i]; }
+    for (int i = 0; i + 1 < rank; ++i) s[i] = strides_bytes[i];
+    const CUresult r = fn(out, is_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank,
+                          const_cast<void*>(base), d, s, b, e, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                          swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+        td_set_error("cuTensorMapEncodeTiled failed (%d) for %s: dims [%llu,%llu,%llu,%llu] box [%u,%u,%u,%u]", (int)r, what,
+                     (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)(rank > 2 ? dims[2] : 0),
+                     (unsigned long long)(rank > 3 ? dims[3] : 0), box[0], box[1], rank > 2 ? box[2] : 0, rank > 3 ? box[3] : 0);
+        return TD_ERR_CUDA;
+    }
+    return TD_OK;
+}
 
 namespace {
 // up2 = 1: `d` describes nearest-2x upsample + 3x3 / pad 1 (OH = 2 H, OW = 2 W) of ONE image; `w` holds the 16 folded taps.
@@ -382,7 +382,7 @@ int conv_run(const td_conv_desc* d, const void* x, const void* w, const float* b
         const uint64_t str[3] = {(uint64_t)d->x_pitch * 2, (uint64_t)d->W * d->x_pitch * 2, (uint64_t)d->H * d->W * d->x_pitch * 2};
         const uint32_t box[4] = {64, (uint32_t)(p.BW * d->stride), (uint32_t)(p.BH * d->stride), 1};
         const uint32_t es[4] = {1, (uint32_t)d->stride, (uint32_t)d->stride, 1};
-        const int rc = encode_map(&ma, x, p.is_bf16, 4, dims, str, box, es, true, "activations");
+        const int rc = td_encode_map(&ma, x, p.is_bf16, 4, dims, str, box, es, true, "activations");
         if (rc != TD_OK) return rc;
     }
     {
@@ -390,7 +390,7 @@ int conv_run(const td_conv_desc* d, const void* x, const void* w, const float* b
         const uint64_t str[2] = {(uint64_t)d->w_pitch * 2, (uint64_t)d->Cout * d->w_pitch * 2};
         const uint32_t box[3] = {64, (uint32_t)bn, 1};
         const uint32_t es[3] = {1, 1, 1};
-        const int rc = encode_map(&mb, w, p.is_bf16, 3, dims, str, box, es, true, "weights");
+        const int rc = td_encode_map(&mb, w, p.is_bf16, 3, dims, str, box, es, true, "weights");
         if (rc != TD_OK) return rc;
     }
     uint16_t* yo = static_cast<uint16_t*>(y);

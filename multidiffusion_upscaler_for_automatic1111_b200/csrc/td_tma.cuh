@@ -74,3 +74,7 @@ __device__ __forceinline__ uint4 lds128(const void* p) {
 // Returns 0 on success; fills `out`.  Encoded through the driver entry point (no link-time libcuda).
 int td_encode_tensor_map_3d(CUtensorMap* out, const void* base, int dtype, uint64_t planes, uint64_t rows, uint64_t cols,
                             uint32_t box_rows, uint32_t box_cols);
+// fp16 / bf16 tensor of rank 2..5 (dims innermost first, strides in bytes of dims 1..rank-1), not cached; swizzle128: the
+// box lands as 128-byte rows in the 128-byte swizzle of the wgmma operands (td_conv.cu).
+int td_encode_map(CUtensorMap* out, const void* base, int is_bf16, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
+                  const uint32_t* box, const uint32_t* estr, bool swizzle128, const char* what);

@@ -192,6 +192,11 @@ class ModuleBackend:
 
 FOLD_UPSAMPLE = os.environ.get("TD_VAE_FOLD_UPSAMPLE", "1") != "0"     # 0: materialise the upsampled tensor (measurement only)
 DUAL_OUTPUT = os.environ.get("TD_VAE_DUAL_OUTPUT", "1") != "0"         # 0: separate GroupNorm pass at block boundaries (measurement only)
+# Attention tiles with more tokens than this run the fused kernel (vae_ops.attention): their fp16 [T, T] score matrix
+# would pass 2^31 elements (4 GiB), and the reference's H100 default tiles (decoder 256, encoder 3072) need 11-27 GiB of
+# it.  Smaller tiles keep the four-GEMM path and its exact output.  The bound depends only on the tile, so a tile takes
+# the same path, with the same bits, on any card.
+SCORE_MATRIX_MAX_TOKENS = 46340
 
 
 class TensorCoreBackend:
@@ -300,8 +305,9 @@ class TensorCoreBackend:
         return ops.gn_apply_nhwc(a, mean, var, gamma, beta, op.act, NUM_GROUPS, GN_EPS)
 
     def attention(self, a, op: Attention, skip, post=None, dual=False):
-        """softmax(q k^T / sqrt(C)) v + proj_out (tile_utils/attn.py:49-72) as four tensor-core GEMMs and one row
-        softmax; the [tokens, tokens] score matrix lives in HBM (388 MB fp16 for a 118 x 118 tile: small next to 80 GB)."""
+        """softmax(q k^T / sqrt(C)) v + proj_out (tile_utils/attn.py:49-72).  Up to SCORE_MATRIX_MAX_TOKENS tokens:
+        four tensor-core GEMMs and one row softmax, the [tokens, tokens] score matrix in HBM (388 MB fp16 for a 118 x 118
+        tile); larger tiles: the fused online-softmax kernel, no score matrix."""
         m = op.module
         _, H, W, C = a.shape
         T = H * W
@@ -311,6 +317,10 @@ class TensorCoreBackend:
         wv, bv, *_ = self._conv_w(m.v)
         q = ops.gemm_nt(x2, wq[0], bias=bq)
         k = ops.gemm_nt(x2, wk[0], bias=bk)
+        wp, bp, *_ = self._conv_w(m.proj_out)
+        if T > SCORE_MATRIX_MAX_TOKENS:
+            o = ops.attention(q, k, ops.gemm_nt(x2, wv[0], bias=bv), float(int(C) ** -0.5))
+            return ops.conv2d_nhwc(o.view(1, H, W, C), wp, bp, ksize=1, residual=skip, post=post, dual=dual)
         Tp = ops.round_up(T, 8)
         vt = torch.empty((C, Tp), dtype=self.dtype, device=self.device)
         if Tp != T:
@@ -321,7 +331,6 @@ class TensorCoreBackend:
         ops.gemm_nt(q, k, alpha=float(int(C) ** -0.5), out=s[:, :T])
         ops.softmax_rows(s, T, out=s)
         o = ops.gemm_nt(s, vt)         # K = Tp (a multiple of 8; the last partial 64-chunk is zero-filled by the TMA unit)
-        wp, bp, *_ = self._conv_w(m.proj_out)
         return ops.conv2d_nhwc(o.view(1, H, W, C), wp, bp, ksize=1, residual=skip, post=post, dual=dual)
 
     def tanh(self, a):

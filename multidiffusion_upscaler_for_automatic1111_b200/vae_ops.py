@@ -150,6 +150,25 @@ def gemm_nt(a: torch.Tensor, b: torch.Tensor, bias: Optional[torch.Tensor] = Non
     return out
 
 
+def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, alpha: float, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """O[T, C] = softmax(alpha * Q K^T) V in one fused kernel (csrc/td_attn.cu): online softmax, nothing of size T x T is
+    allocated.  q / k / v / out: [T, C] views with unit inner stride, row pitches multiples of 8 elements; C % 64 == 0,
+    C <= 512."""
+    _cuda(q, "q"); _cuda(k, "k"); _cuda(v, "v")
+    T, C = q.shape
+    assert k.shape == (T, C) and v.shape == (T, C), f"q {tuple(q.shape)}, k {tuple(k.shape)}, v {tuple(v.shape)} differ"
+    assert k.dtype == q.dtype and v.dtype == q.dtype and k.device == q.device and v.device == q.device
+    if out is None:
+        out = torch.empty((T, C), dtype=q.dtype, device=q.device)
+    assert out.shape == (T, C) and out.dtype == q.dtype
+    for name, t in (("q", q), ("k", k), ("v", v), ("out", out)):
+        assert t.stride(1) == 1 and t.stride(0) % 8 == 0, f"{name}: unit inner stride and a row pitch that is a multiple of 8 (got {t.stride()})"
+    with torch.cuda.device(q.device):
+        check(lib.td_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), T, C, q.stride(0), k.stride(0), v.stride(0),
+                               out.stride(0), float(alpha), dtype_code(q.dtype), current_stream_ptr(q.device)))
+    return out
+
+
 def nchw_to_nhwc(x: torch.Tensor, cpad: int) -> torch.Tensor:
     """[N, C, h, w] view (unit inner stride) -> contiguous [N, h, w, cpad], channels zero-padded."""
     _cuda(x, "x")
