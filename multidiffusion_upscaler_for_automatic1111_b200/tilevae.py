@@ -3,8 +3,10 @@
 underneath.
 
 What is different from the reference by design (80 GB of HBM, hand-written sm_90a kernels):
-  * tiles, residuals and parked activations stay in HBM -- the reference stages every tile
-    through host RAM (`.cpu()` at tilevae.py:534,610,641) and re-uploads it each round;
+  * tiles, residuals and parked activations stay in HBM while they fit -- the reference stages every tile
+    through host RAM (`.cpu()` at tilevae.py:534,610,641) and re-uploads it each round; when the tiles held at a
+    slow-mode GroupNorm barrier exceed the budget (`VAEHook.max_resident_bytes`, default: the free device memory),
+    the ones needed last wait in pinned host memory, copied on dedicated streams (`_Parking`);
   * GroupNorm statistics: one streaming read (`td_gn_stats`, fp32 Chan/Welford merge with
     warp shuffles) instead of `var_mean` on a reshaped copy;
   * GroupNorm apply + affine + SiLU: ONE fused pass (`td_gn_apply`) instead of
@@ -24,6 +26,8 @@ from __future__ import annotations
 
 import ctypes
 import math
+import time
+import weakref
 from typing import Callable, List, Optional
 
 import numpy as np
@@ -246,6 +250,146 @@ class GroupNormParam:
         return packed[k:2 * k] / packed[-1], packed[:k] / packed[-1]
 
 
+# --------------------------------------------------------------------------- parking
+def _dense_bytes(t: torch.Tensor) -> torch.Tensor:
+    """A uint8 view of the memory of a dense tensor in any dimension order (the module backend's convolutions may
+    return channels-last tensors): a parked tensor comes back with its own strides, so later ops see the same layout."""
+    p = t.permute(sorted(range(t.dim()), key=lambda d: -t.stride(d)))
+    assert p.is_contiguous(), f"cannot park a tensor with strides {t.stride()}"
+    return p.reshape(-1).view(torch.uint8)
+
+
+class _Parking:
+    """Pinned host homes for the tiles a residency plan parks, and the two copy streams that move them (the H100 has a
+    copy engine per direction).  Copies overlap with the kernels of the tiles being computed.
+
+      * park: after the tile's statistics kernel, its `act` / `skip` go to its pinned buffer on the device-to-host
+        stream; the device blocks are handed back with record_stream, so the caching allocator reuses them only once
+        the copy has read them.  A shortcut whose host copy is still current (the block input of an identity shortcut,
+        parked at norm1, is the shortcut at norm2) is not copied again.  Buffer layout: shortcut at 0, activation after
+        it; an aliased pair is one region.
+      * resume: the tile's upload (issued before, while the previous tile computed) is waited on by the compute stream,
+        the deferred barrier norm is applied, and the upload of the next parked tile in the visiting order is issued.
+    Buffers are pageable host memory registered with cudaHostRegister (exact sizes), released by `close`."""
+
+    def __init__(self, device, sizes, stats: dict):
+        self.device, self.sizes, self.stats = device, sizes, stats
+        self.d2h = torch.cuda.Stream(device)
+        self.h2d = torch.cuda.Stream(device)
+        self.buf = {}          # tile -> registered uint8 host tensor
+        self.slot = {}         # tile -> {"act": (offset, shape, strides, dtype), "skip": ..., "written": Event}
+        self.home = set()      # tiles whose state is on the host
+        self.uploads = {}      # tile -> (act, skip, Event): device tensors being filled on the upload stream
+        self.pending = {}      # tile -> (norm op, mean, var) to apply on resume
+        self.current = {}      # tile -> weakref of the device shortcut whose host copy is current
+        self.last_written = None
+
+    def parked(self, i) -> bool:
+        return i in self.home
+
+    def _buffer(self, i):
+        if i not in self.buf:
+            t0 = time.perf_counter()
+            t = torch.empty(self.sizes[i], dtype=torch.uint8)
+            err = int(torch.cuda.cudart().cudaHostRegister(t.data_ptr(), t.numel(), 0))
+            if err != 0:
+                raise RuntimeError(f"[Tiled VAE]: pinning {t.numel()} bytes of host memory failed (cudaError {err})")
+            self.buf[i] = t
+            self.stats["host_bytes"] += t.numel()
+            self.stats["pin_s"] += time.perf_counter() - t0
+        return self.buf[i]
+
+    def park(self, i, st, site: int) -> None:
+        buf = self._buffer(i)
+        if self.last_written is not None:
+            # one write-back in flight: the caching allocator frees a parked block on the host's side once its copy is
+            # done, so without this wait a run ahead of the copy engine would keep every parked tile allocated
+            self.last_written.synchronize()
+        ready = torch.cuda.Event()
+        ready.record(torch.cuda.current_stream(self.device))
+        self.d2h.wait_event(ready)
+        ref = self.current.pop(i, None)
+        slot, copied, off = {}, [], 0
+        with torch.cuda.stream(self.d2h):
+            if st.skip is not None:
+                if ref is None or ref() is not st.skip:
+                    copied.append((0, st.skip))
+                slot["skip"] = (0, st.skip.shape, st.skip.stride(), st.skip.dtype)
+                off = st.skip.numel() * st.skip.element_size()
+            if st.skip is not None and st.act is st.skip:
+                slot["act"] = slot["skip"]
+            else:
+                copied.append((off, st.act))
+                slot["act"] = (off, st.act.shape, st.act.stride(), st.act.dtype)
+            for o, t in copied:
+                n = t.numel() * t.element_size()
+                buf[o:o + n].copy_(_dense_bytes(t), non_blocking=True)
+                t.record_stream(self.d2h)
+                self.stats["d2h_bytes"] += n
+            slot["written"] = torch.cuda.Event()
+            slot["written"].record(self.d2h)
+        self.slot[i] = slot
+        self.last_written = slot["written"]
+        st.act = st.skip = None
+        self.home.add(i)
+        per_site = self.stats["tiles_parked"]
+        per_site[site] = per_site.get(site, 0) + 1
+
+    def defer(self, i, norm, mean, var) -> None:
+        self.pending[i] = (norm, mean, var)
+
+    def _upload(self, i) -> None:
+        if i in self.uploads or i not in self.home:
+            return
+        slot, buf = self.slot[i], self.buf[i]
+        alloc = lambda d: torch.empty_strided(d[1], d[2], dtype=d[3], device=self.device)     # the parked tensor's strides
+        skip = alloc(slot["skip"]) if "skip" in slot else None
+        aliased = "skip" in slot and slot["act"] is slot["skip"]
+        act = skip if aliased else alloc(slot["act"])
+        # the blocks come from the compute stream's pool: kernels queued before may still read their previous tenant
+        free = torch.cuda.Event()
+        free.record(torch.cuda.current_stream(self.device))
+        self.h2d.wait_event(free)
+        self.h2d.wait_event(slot["written"])
+        with torch.cuda.stream(self.h2d):
+            for t, desc in ((skip, slot.get("skip")), (None if aliased else act, slot["act"])):
+                if t is None:
+                    continue
+                n = t.numel() * t.element_size()
+                _dense_bytes(t).copy_(buf[desc[0]:desc[0] + n], non_blocking=True)
+                self.stats["h2d_bytes"] += n
+            done = torch.cuda.Event()
+            done.record(self.h2d)
+        self.uploads[i] = (act, skip, done)
+
+    def resume(self, ex, i, st, ahead) -> None:
+        """Before tile i computes: its state back on the device, and the next parked tile of `ahead` on its way."""
+        self._upload(i)
+        nxt = next((j for j in ahead if j in self.home), None)
+        if nxt is not None:
+            self._upload(nxt)
+        if i not in self.home:
+            return
+        act, skip, done = self.uploads.pop(i)
+        torch.cuda.current_stream(self.device).wait_event(done)
+        self.home.discard(i)
+        st.act, st.skip = act, skip
+        if skip is not None:
+            self.current[i] = weakref.ref(skip)
+        if i in self.pending:
+            ex.apply_barrier(st, *self.pending.pop(i))
+
+    def close(self) -> None:
+        """Drain both copy streams (also after an interrupt), then release the pinned buffers."""
+        self.d2h.synchronize()
+        self.h2d.synchronize()
+        self.uploads.clear()
+        self.pending.clear()
+        for t in self.buf.values():
+            torch.cuda.cudart().cudaHostUnregister(t.data_ptr())
+        self.buf.clear()
+
+
 # --------------------------------------------------------------------------- the hook
 class VAEHook:
 
@@ -259,6 +403,10 @@ class VAEHook:
         self.pad = 11 if is_decoder else 32
         self.verbose = False
         self.backend_name = None      # which backend ran the last call ("wgmma" / "modules")
+        # Slow-mode tiles kept in GPU memory at a GroupNorm barrier may hold at most this many bytes; the others wait in
+        # pinned host memory.  None: the free device memory at the start of the call, less the working reserve.
+        self.max_resident_bytes: Optional[int] = None
+        self.last_park_stats: Optional[dict] = None    # what the last call parked (see _run_tiles)
         self._program = None
         self._shard_group = None
         self._shard_world = 1
@@ -338,6 +486,10 @@ class VAEHook:
         out_c = [op for op in program.ops if isinstance(op, ve.Conv)][-1].module.out_channels
         oh, ow = (height * 8, width * 8) if is_decoder else (height // 8, width // 8)
         result = torch.zeros((N, out_c, oh, ow), dtype=dtype, device=device)   # zeros: a partial (interrupted) result reads 0 elsewhere
+        # budget / reserve: bytes (None when no barrier); host_bytes: pinned host memory (its peak: buffers live until the
+        # call ends); d2h / h2d_bytes: bytes copied each way; pin_s: seconds spent pinning; tiles_parked: {site: tiles}
+        self.last_park_stats = {"budget": None, "reserve": None, "host_bytes": 0, "d2h_bytes": 0, "h2d_bytes": 0, "pin_s": 0.0,
+                                "tiles_parked": {}}
         finished = 0
         images = [slice(n, n + 1) for n in range(N)] if per_image else [slice(0, N)]
         for img in images:
@@ -358,54 +510,109 @@ class VAEHook:
         return result
 
     def _run_tiles(self, ex, backend, z, result, in_bboxes, out_bboxes) -> int:
-        """All tiles of one image (or image batch) through the program: rounds separated by the barrier sites."""
+        """All tiles of one image (or image batch) through the program: rounds separated by the barrier sites.  An input
+        tile is loaded on its first visit.  When the tiles held at a barrier do not all fit in GPU memory, the ones the
+        residency plan picks wait in pinned host memory until their next visit (`_Parking`); when they fit, nothing is
+        copied."""
         from . import vae_engine as ve
-        states = []
-        for b in in_bboxes:
-            st = ve.TileState(backend.load(z[:, :, b[2]:b[3], b[0]:b[1]]))
-            states.append(st)
+        num_tiles = len(in_bboxes)
+        states = [ve.TileState(None) for _ in range(num_tiles)]
         sharded = self._shard_world > 1
         rounds = ex.barrier_sites()
-        num_tiles = len(states)
+        barriers = [op for op in ex.program.ops if isinstance(op, ve.Norm) and ex.frozen[op.site] is None]
+        plan = self._park_plan(ex, backend, z, in_bboxes, barriers)
+        pk = _Parking(z.device, plan[1], self.last_park_stats) if plan is not None else None
         done = 0
         forward = True
-        for rnd in range(rounds + 1):
-            if host.interrupted():
-                break
-            collect = GroupNormParam(self._shard_group, sharded)
-            site = None
-            order = range(num_tiles) if forward else range(num_tiles - 1, -1, -1)     # the reference's zig-zag (:599)
-            for i in order:
+        try:
+            for rnd in range(rounds + 1):
                 if host.interrupted():
                     break
-                st = states[i]
-                if st is None:
-                    continue
-                stop = ex.run(st)
-                if stop is None:
-                    backend.paste(st.act, result, in_bboxes[i], out_bboxes[i], self.is_decoder)
-                    states[i] = None
-                    done += 1
-                else:
-                    site = stop
-                    var, mean = backend.stats(st.act)
-                    collect.add(var, mean, backend.pixels(st.act))
-            forward = not forward
-            if rnd == rounds or host.interrupted():
-                break
-            if site is None and sharded:      # a rank without tiles still joins the round's all-reduce
-                site = [op for op in ex.program.ops if isinstance(op, ve.Norm) and ex.frozen[op.site] is None][rnd]
-            if site is None:
-                break
-            stat_len = NUM_GROUPS * (z.shape[0] if not isinstance(backend, ve.TensorCoreBackend) else 1)
-            merged = collect.summary(stat_len, z.device)
-            if merged is None:
-                break
-            mean, var = merged
-            for st in states:
-                if st is not None:
-                    ex.apply_barrier(st, site, mean, var)
+                collect = GroupNormParam(self._shard_group, sharded)
+                site = None
+                order = list(range(num_tiles)) if forward else list(range(num_tiles - 1, -1, -1))   # the reference's zig-zag (:599)
+                park_now = set(plan[0][rnd]) if pk is not None and rnd < rounds else ()
+                for k, i in enumerate(order):
+                    if host.interrupted():
+                        break
+                    st = states[i]
+                    if st is None:
+                        continue
+                    if pk is not None:
+                        pk.resume(ex, i, st, [j for j in order[k + 1:] if states[j] is not None])
+                    if st.act is None:
+                        b = in_bboxes[i]
+                        st.act = backend.load(z[:, :, b[2]:b[3], b[0]:b[1]])
+                    stop = ex.run(st)
+                    if stop is None:
+                        backend.paste(st.act, result, in_bboxes[i], out_bboxes[i], self.is_decoder)
+                        states[i] = None
+                        done += 1
+                    else:
+                        site = stop
+                        var, mean = backend.stats(st.act)
+                        collect.add(var, mean, backend.pixels(st.act))
+                        if i in park_now:
+                            pk.park(i, st, stop.site)
+                forward = not forward
+                if rnd == rounds or host.interrupted():
+                    break
+                if site is None and sharded:      # a rank without tiles still joins the round's all-reduce
+                    site = barriers[rnd]
+                if site is None:
+                    break
+                stat_len = NUM_GROUPS * (z.shape[0] if not isinstance(backend, ve.TensorCoreBackend) else 1)
+                merged = collect.summary(stat_len, z.device)
+                if merged is None:
+                    break
+                mean, var = merged
+                for i, st in enumerate(states):
+                    if st is None:
+                        continue
+                    if pk is not None and pk.parked(i):
+                        pk.defer(i, site, mean, var)      # normalised when it is back on the device
+                    else:
+                        ex.apply_barrier(st, site, mean, var)
+        finally:
+            if pk is not None:
+                pk.close()
         return done
+
+    def _park_plan(self, ex, backend, z, in_bboxes, barriers):
+        """None when every tile fits at every barrier; else (tiles parked at each barrier, pinned bytes per parked tile).
+
+        Budget for the resident tiles: the free device memory (driver + the caching allocator's unused blocks) less
+        the largest working set of one tile and two tiles' parked bytes (one upload and one write-back in flight);
+        `max_resident_bytes` lowers it."""
+        from . import vae_engine as ve
+        if not barriers or not in_bboxes:
+            return None
+        fps = {}
+        for b in in_bboxes:
+            key = (b[3] - b[2], b[1] - b[0])
+            if key not in fps:
+                fps[key] = ve.tile_footprint(ex.program, backend.name, backend.dtype, key[0], key[1], z.shape[0])
+        tiles = [fps[(b[3] - b[2], b[1] - b[0])] for b in in_bboxes]
+        held = [[fp.held(op.site) for fp in tiles] for op in barriers]            # what a park / upload moves
+        resident = [[fp.resident(op.site) for fp in tiles] for op in barriers]    # what a waiting tile holds
+        reserve = max(fp.working for fp in fps.values()) + 2 * max(max(h) for h in held)
+        dev = z.device
+        free = torch.cuda.mem_get_info(dev)[0] + torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev)
+        budget = max(free - reserve, 0)
+        if self.max_resident_bytes is not None:
+            budget = min(budget, max(int(self.max_resident_bytes), 0))
+        self.last_park_stats.update(budget=budget, reserve=reserve)
+        n = len(in_bboxes)
+        orders = [list(range(n)) if r % 2 == 0 else list(range(n - 1, -1, -1)) for r in range(len(barriers))]
+        parked = ve.plan_residency(orders, resident, budget)
+        if not any(parked):
+            return None
+        sizes = {}       # a tile's buffer: its largest footprint over the barriers where it is parked
+        for r, p in enumerate(parked):
+            for i in p:
+                sizes[i] = max(sizes.get(i, 0), held[r][i])
+        ve.require_host_memory(sum(sizes.values()))
+        return parked, sizes
 
     def _exchange_regions(self, result, in_bboxes, out_bboxes):
         """Tile shard: every rank pasted its own tiles; gather the disjoint output regions (one all-gather of the

@@ -121,6 +121,176 @@ def compile_program(net, is_decoder: bool) -> Program:
     return Program(seq, sites, is_decoder, first_resample)
 
 
+# ----------------------------------------------------------------------------------------------- residency plan
+@dataclass
+class TileFootprint:
+    """What one tile holds in HBM along the program, in the backend's real layouts.  Per GroupNorm site: `act`, the
+    bytes of the activation entering the norm, and `skip`, the bytes of the held shortcut (0 when there is none or
+    when it IS the activation: an identity shortcut is one tensor).  `working`: the largest set of live tensors of
+    the tile between two sites (its own state, the op's outputs and temporaries, the four-GEMM attention's score
+    matrix).  `alias[site]`: the shortcut is the activation (identity shortcut)."""
+    act: List[int]
+    skip: List[int]
+    alias: List[bool]
+    working: int
+
+    def held(self, site: int) -> int:
+        """Bytes at the site: what parking copies."""
+        return self.act[site] + self.skip[site]
+
+    def resident(self, site: int) -> int:
+        """Bytes once the site's norm is applied: the normalised activation no longer aliases an identity shortcut."""
+        return self.act[site] + (self.act[site] if self.alias[site] else self.skip[site])
+
+
+def tile_footprint(program: Program, backend_name: str, dtype, h: int, w: int, batch: int = 1) -> TileFootprint:
+    """Shape walk of `program` for an input tile of h x w pixels.  backend_name "wgmma": channels-last, one image,
+    conv_in's input padded to 64 channels, output channels rounded up to 16; "modules": NCHW, `batch` images,
+    exact channels."""
+    e = torch.empty((), dtype=dtype).element_size()
+    tc = backend_name == TensorCoreBackend.name
+    n = 1 if tc else batch
+
+    def nbytes(c, hh, ww):
+        return n * c * hh * ww * e
+
+    def out_c(m):
+        co = m.out_channels
+        return (co if co % 16 == 0 else ops.round_up(co, 16)) if tc else co
+
+    c = program.ops[0].module.in_channels
+    c = ops.round_up(c, 64) if tc else c
+    H, W = h, w
+    act, skip, alias = nbytes(c, H, W), 0, False
+    act_at: List[int] = []
+    skip_at: List[int] = []
+    alias_at: List[bool] = []
+    working = act
+
+    def live(*extra):
+        nonlocal working
+        working = max(working, act + (0 if alias else skip) + sum(extra))
+
+    for op in program.ops:
+        if isinstance(op, Conv):
+            m, tmp = op.module, 0
+            if op.upsample_first:
+                folded = tc and FOLD_UPSAMPLE and m.kernel_size == (3, 3) and m.out_channels % 16 == 0
+                if not folded:
+                    tmp = nbytes(c, 2 * H, 2 * W)
+                H, W = 2 * H, 2 * W
+            if op.downsample:
+                if not tc:
+                    tmp = nbytes(c, H + 1, W + 1)          # F.pad
+                H, W = (H - 2) // 2 + 1, (W - 2) // 2 + 1
+            c = out_c(m)
+            y = nbytes(c, H, W)
+            live(tmp, y, y if tc else 0)                   # tensor cores: a dual-output epilogue writes two
+            act, alias = y, False
+            if op.add_skip:
+                skip = 0
+        elif isinstance(op, Skip):
+            if op.module is None:
+                skip, alias = act, True
+            else:
+                y = nbytes(out_c(op.module), H, W)
+                live(y)
+                skip, alias = y, False
+        elif isinstance(op, Norm):
+            act_at.append(act)
+            skip_at.append(0 if alias else skip)
+            alias_at.append(alias)
+            live(act)
+            alias = False
+        elif isinstance(op, Attention):
+            T = H * W
+            y = nbytes(c, H, W)
+            if tc:
+                qk = 2 * T * ops.round_up(c, 8) * e
+                if T > SCORE_MATRIX_MAX_TOKENS:
+                    extra = qk + 2 * T * c * e                                  # v, o
+                else:
+                    Tp = ops.round_up(T, 8)
+                    extra = qk + c * Tp * e + T * Tp * e + T * ops.round_up(c, 8) * e   # v^T, scores, o
+                live(extra, y, y)
+            else:
+                live(3 * y, 2 * y, y)                      # q, k, v; the attention output and its NCHW copy
+            act, skip, alias = y, 0, False
+        elif isinstance(op, Tanh):
+            live(act)
+    return TileFootprint(act_at, skip_at, alias_at, working)
+
+
+def plan_residency(orders: List[List[int]], held: List[List[int]], budget: int) -> List[List[int]]:
+    """Which tiles wait in host memory at each barrier.  orders[r]: the tiles in the order round r visits them (round r
+    ends at barrier r); held[r][i]: bytes tile i holds in HBM while it waits at barrier r (`TileFootprint.resident`:
+    its barrier norm is applied before the next round).  -> parked[r], the tiles parked at barrier r.
+
+    Round r+1 visits the tiles in reverse (the zig-zag), so the tiles visited last in round r are needed first: keep
+    the longest suffix of round r's order resident (Belady: what is needed soonest stays).  The suffix is shortened
+    until the resident bytes fit the budget at the barrier AND at every point of the round, where the tiles still
+    waiting at barrier r-1 and the ones already resident at barrier r are held together."""
+    parked: List[List[int]] = []
+    prev: Dict[int, int] = {}              # tile -> bytes, resident at the previous barrier
+    for r, order in enumerate(orders):
+        n = len(order)
+        waiting = [0] * (n + 1)           # waiting[k]: bytes of previous residents visited at position >= k
+        for k in range(n - 1, -1, -1):
+            waiting[k] = waiting[k + 1] + prev.get(order[k], 0)
+        keep = n
+        while keep > 0:
+            first = n - keep
+            kept, ok = 0, True
+            for k in range(n + 1):         # after k visits
+                if k > first:
+                    kept += held[r][order[k - 1]]
+                if kept + waiting[k] > budget:
+                    ok = False
+                    break
+            if ok:
+                break
+            keep -= 1
+        resident = order[n - keep:]
+        parked.append(order[:n - keep])
+        prev = {t: held[r][t] for t in resident}
+    return parked
+
+
+def host_available_bytes(meminfo: str = "/proc/meminfo", cgroup: str = "/sys/fs/cgroup") -> Optional[int]:
+    """MemAvailable of the host, lowered to what the process's cgroup (v2) still allows when it has a memory limit (a
+    container's cap is not in /proc/meminfo); None where neither is reported."""
+    avail = None
+    try:
+        with open(meminfo) as f:
+            for line in f:
+                if line.startswith("MemAvailable:"):
+                    avail = int(line.split()[1]) * 1024
+                    break
+    except OSError:
+        pass
+    try:
+        with open(os.path.join(cgroup, "memory.max")) as f:
+            cap = f.read().strip()
+        with open(os.path.join(cgroup, "memory.current")) as f:
+            used = int(f.read().strip())
+        if cap != "max":
+            left = max(int(cap) - used, 0)
+            avail = left if avail is None else min(avail, left)
+    except (OSError, ValueError):
+        pass
+    return avail
+
+
+def require_host_memory(need: int, available: Optional[int] = None) -> None:
+    """Refuse a parking plan the host cannot pin, before any tile runs (rather than letting the OOM killer decide)."""
+    if available is None:
+        available = host_available_bytes()
+    if available is not None and need > available:
+        raise RuntimeError(f"[Tiled VAE]: parking the tiles that do not fit in GPU memory needs {need / 1e9:.1f} GB of pinned "
+                           f"host memory, but only {available / 1e9:.1f} GB are available; use a smaller image or a "
+                           f"smaller tile size, or free host memory")
+
+
 # ----------------------------------------------------------------------------------------------- backends
 def _f32(t: Optional[torch.Tensor], device) -> Optional[torch.Tensor]:
     return None if t is None else t.detach().to(device=device, dtype=torch.float32).contiguous()
