@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define TD_ABI_VERSION 7
+#define TD_ABI_VERSION 8
 
 typedef enum td_status {
     TD_OK = 0,
@@ -291,6 +291,12 @@ typedef struct td_region {
 } td_region;
 int td_region_composite(const void* x_buffer, const float* weights, const td_region* regions, int n_regions,
                         int N, int C, int H, int W, int dtype, float* out, void* stream);
+/* td_region_composite limited to canvas rows [row_begin, row_end) (0 <= row_begin <= row_end <= H): the same per-pixel
+ * arithmetic, only those rows of `out` are written (x_buffer, weights and out are still whole-canvas pointers).  Regions keep
+ * canvas coordinates; a region may also be given clipped to the window -- y and h narrowed to the rows it covers there,
+ * `out` holding just those rows as [N, C, h, w] and `aux` pointing at the first of them -- and reads the same values. */
+int td_region_composite_rows(const void* x_buffer, const float* weights, const td_region* regions, int n_regions,
+                             int N, int C, int H, int W, int dtype, float* out, int row_begin, int row_end, void* stream);
 
 /* ------------------------------------------------------------------------- *
  *  DemoFusion extras (tile_methods/demofusion.py).

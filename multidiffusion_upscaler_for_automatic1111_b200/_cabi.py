@@ -32,7 +32,7 @@ TD_MAX_GRID_DIM = 256
 TD_MAX_BATCH_PTRS = 128
 TD_MAX_PEERS = 16
 TD_IPC_HANDLE_BYTES = 64
-ABI_VERSION = 7
+ABI_VERSION = 8
 
 DTYPE_CODE = {torch.float16: TD_F16, torch.bfloat16: TD_BF16, torch.float32: TD_F32}
 
@@ -127,6 +127,8 @@ _SIGNATURES = {
     "td_peer_wait": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
     "td_push_regions": (c_int, [POINTER(TdPushRegion), c_int, POINTER(c_void_p), c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     "td_region_composite": (c_int, [c_void_p, c_void_p, POINTER(TdRegion), c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "td_region_composite_rows": (c_int, [c_void_p, c_void_p, POINTER(TdRegion), c_int, c_int, c_int, c_int, c_int, c_int, c_void_p,
+                                         c_int, c_int, c_void_p]),
     "td_dilated_gather": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_int32),
                                   POINTER(c_int32), POINTER(c_int32), c_int, c_int, c_void_p]),
     "td_demofusion_combine": (c_int, [c_void_p, POINTER(c_void_p), c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int,

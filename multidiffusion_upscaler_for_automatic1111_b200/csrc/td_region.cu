@@ -10,6 +10,8 @@
 //   FOREGROUND   fb = round_T(float(fb) + float(r)); fm += mask; fc += 1   (feather buffer in T, mask / count in fp32)
 //   composite    if fc > 1: fbf = float(fb) / fc, fm = fm / fc;  if fc > 0: o = o * (1 - fm) + fbf * fm
 //                (each product and the sum rounded separately: no FMA contraction)
+// td_region_composite_rows runs the same kernel over a window of canvas rows (the row-strip shard composites only the
+// rows a rank owns); td_region_composite is its [0, H) case.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -28,6 +30,7 @@ using namespace td;
 struct RegionParams {
     int n;
     int N, C, H, W;
+    int row_begin, rows;              // canvas rows [row_begin, row_begin + rows) are produced; the rest of `out` is untouched
     int divide;                       // 1: MultiDiffusion normalisation by the weight canvas
     int x[TD_MAX_REGIONS], y[TD_MAX_REGIONS], w[TD_MAX_REGIONS], h[TD_MAX_REGIONS], mode[TD_MAX_REGIONS];
     const void* out[TD_MAX_REGIONS];      // region denoiser output [N, C, h, w] of T
@@ -38,12 +41,13 @@ template <typename T>
 __global__ void __launch_bounds__(256)
 region_composite_kernel(const __grid_constant__ RegionParams p, const T* __restrict__ x_buffer, const float* __restrict__ weights,
                         float* __restrict__ out) {
-    const long long total = (long long)p.N * p.C * p.H * p.W;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-        const int px = (int)(i % p.W);
-        long long t = i / p.W;
-        const int py = (int)(t % p.H);
-        const long long plane = t / p.H;               // n * C + c
+    const long long total = (long long)p.N * p.C * p.rows * p.W;
+    for (long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x; k < total; k += (long long)gridDim.x * blockDim.x) {
+        const int px = (int)(k % p.W);
+        long long t = k / p.W;
+        const int py = p.row_begin + (int)(t % p.rows);
+        const long long plane = t / p.rows;            // n * C + c
+        const long long i = (plane * p.H + py) * p.W + px;
         float acc = Elem<T>::to_f32(x_buffer[i]);
         float fb = 0.0f, fm = 0.0f, fc = 0.0f;
         for (int r = 0; r < p.n; ++r) {
@@ -74,37 +78,55 @@ region_composite_kernel(const __grid_constant__ RegionParams p, const T* __restr
     }
 }
 
-}  // namespace
-
-extern "C" int td_region_composite(const void* x_buffer, const float* weights, const td_region* regions, int n_regions, int N, int C,
-                                   int H, int W, int dtype, float* out, void* stream) {
+// Both entry points: validation, parameter block and launch for canvas rows [row_begin, row_end).
+int region_composite_launch(const char* fn, const void* x_buffer, const float* weights, const td_region* regions, int n_regions, int N,
+                            int C, int H, int W, int dtype, float* out, int row_begin, int row_end, void* stream) {
     if (x_buffer == nullptr || out == nullptr || N <= 0 || C <= 0 || H <= 0 || W <= 0 || n_regions < 0 || (n_regions > 0 && regions == nullptr)) {
-        td_set_error("td_region_composite: bad arguments");
+        td_set_error("%s: bad arguments", fn);
         return TD_ERR_INVALID_ARG;
     }
-    if (n_regions > TD_MAX_REGIONS) { td_set_error("td_region_composite: %d regions exceed TD_MAX_REGIONS=%d", n_regions, TD_MAX_REGIONS); return TD_ERR_UNSUPPORTED; }
+    if (row_begin < 0 || row_begin > row_end || row_end > H) {
+        td_set_error("%s: rows [%d,%d) outside [0,%d)", fn, row_begin, row_end, H);
+        return TD_ERR_INVALID_ARG;
+    }
+    if (n_regions > TD_MAX_REGIONS) { td_set_error("%s: %d regions exceed TD_MAX_REGIONS=%d", fn, n_regions, TD_MAX_REGIONS); return TD_ERR_UNSUPPORTED; }
     RegionParams p;
     p.n = n_regions; p.N = N; p.C = C; p.H = H; p.W = W;
+    p.row_begin = row_begin; p.rows = row_end - row_begin;
     p.divide = weights != nullptr ? 1 : 0;
     for (int r = 0; r < n_regions; ++r) {
         const td_region& g = regions[r];
         if (g.x < 0 || g.y < 0 || g.w <= 0 || g.h <= 0 || g.x + g.w > W || g.y + g.h > H || g.out == nullptr || (g.mode != 0 && g.mode != 1) ||
             (g.mode == 1 && g.aux == nullptr)) {
-            td_set_error("td_region_composite: region %d is invalid", r);
+            td_set_error("%s: region %d is invalid", fn, r);
             return TD_ERR_INVALID_ARG;
         }
         p.x[r] = g.x; p.y[r] = g.y; p.w[r] = g.w; p.h[r] = g.h; p.mode[r] = g.mode; p.out[r] = g.out; p.aux[r] = g.aux;
     }
-    const long long total = (long long)N * C * H * W;
+    if (p.rows == 0) return TD_OK;
+    const long long total = (long long)N * C * p.rows * W;
     const int grid = (int)std::min<long long>((total + 255) / 256, 148LL * 16);
     cudaStream_t st = (cudaStream_t)stream;
     switch (dtype) {
         case TD_F16: region_composite_kernel<__half><<<grid, 256, 0, st>>>(p, (const __half*)x_buffer, weights, out); break;
         case TD_BF16: region_composite_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>(p, (const __nv_bfloat16*)x_buffer, weights, out); break;
         case TD_F32: region_composite_kernel<float><<<grid, 256, 0, st>>>(p, (const float*)x_buffer, weights, out); break;
-        default: td_set_error("td_region_composite: unknown dtype %d", dtype); return TD_ERR_INVALID_ARG;
+        default: td_set_error("%s: unknown dtype %d", fn, dtype); return TD_ERR_INVALID_ARG;
     }
     const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { td_set_error("td_region_composite: launch failed: %s", cudaGetErrorString(e)); return TD_ERR_CUDA; }
+    if (e != cudaSuccess) { td_set_error("%s: launch failed: %s", fn, cudaGetErrorString(e)); return TD_ERR_CUDA; }
     return TD_OK;
+}
+
+}  // namespace
+
+extern "C" int td_region_composite(const void* x_buffer, const float* weights, const td_region* regions, int n_regions, int N, int C,
+                                   int H, int W, int dtype, float* out, void* stream) {
+    return region_composite_launch("td_region_composite", x_buffer, weights, regions, n_regions, N, C, H, W, dtype, out, 0, H, stream);
+}
+
+extern "C" int td_region_composite_rows(const void* x_buffer, const float* weights, const td_region* regions, int n_regions, int N,
+                                        int C, int H, int W, int dtype, float* out, int row_begin, int row_end, void* stream) {
+    return region_composite_launch("td_region_composite_rows", x_buffer, weights, regions, n_regions, N, C, H, W, dtype, out, row_begin,
+                                   row_end, stream);
 }

@@ -235,15 +235,10 @@ def blend_bboxes(batch_outs: Sequence[torch.Tensor], tile_bs: int, origins_dev: 
     return out
 
 
-def region_composite(x_buffer: torch.Tensor, weights: Optional[torch.Tensor], regions: Sequence[tuple], out: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """Everything after the custom regions' denoiser calls in one launch (multidiffusion.py:187-216,
-    mixtureofdiffusers.py:145-175).  regions: [(x, y, w, h, mode, region_out [N,C,h,w], aux fp32 [h,w] or None)] in list
-    order, mode 0 BACKGROUND (aux = optional multiplier) / 1 FOREGROUND (aux = feather mask).  weights: the fp32
-    divide-where->1 canvas (MultiDiffusion) or None.  Returns fp32 [N,C,H,W]."""
+def _region_table(xb: torch.Tensor, regions: Sequence[tuple]):
+    """td_region array of `regions` [(x, y, w, h, mode, region_out [N,C,h,w], aux fp32 [h,w] or None)] + the tensors it points at."""
     from ._cabi import TdRegion
-    _require_cuda(x_buffer, "x_buffer")
-    N, C, H, W = x_buffer.shape
-    xb = x_buffer.contiguous()
+    N, C = xb.shape[0], xb.shape[1]
     arr = (TdRegion * max(1, len(regions)))()
     keep = []
     for i, (rx, ry, rw, rh, mode, r_out, aux) in enumerate(regions):
@@ -257,8 +252,37 @@ def region_composite(x_buffer: torch.Tensor, weights: Optional[torch.Tensor], re
                 aux.to(device=xb.device, dtype=torch.float32).reshape(rh, rw).contiguous()
         keep += [ro, ax]
         arr[i] = TdRegion(int(rx), int(ry), int(rw), int(rh), int(mode), ro.data_ptr(), ax.data_ptr() if ax is not None else None)
+    return arr, keep
+
+
+def region_composite(x_buffer: torch.Tensor, weights: Optional[torch.Tensor], regions: Sequence[tuple], out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Everything after the custom regions' denoiser calls in one launch (multidiffusion.py:187-216,
+    mixtureofdiffusers.py:145-175).  regions: [(x, y, w, h, mode, region_out [N,C,h,w], aux fp32 [h,w] or None)] in list
+    order, mode 0 BACKGROUND (aux = optional multiplier) / 1 FOREGROUND (aux = feather mask).  weights: the fp32
+    divide-where->1 canvas (MultiDiffusion) or None.  Returns fp32 [N,C,H,W]."""
+    _require_cuda(x_buffer, "x_buffer")
+    N, C, H, W = x_buffer.shape
+    xb = x_buffer.contiguous()
+    arr, keep = _region_table(xb, regions)
     res = out if out is not None else torch.empty((N, C, H, W), dtype=torch.float32, device=xb.device)
     with torch.cuda.device(xb.device):
         check(lib.td_region_composite(xb.data_ptr(), weights.data_ptr() if weights is not None else None, arr, len(regions), N, C, H, W,
                                       dtype_code(xb.dtype), res.data_ptr(), current_stream_ptr(xb.device)))
     return res
+
+
+def region_composite_rows(x_buffer: torch.Tensor, weights: Optional[torch.Tensor], regions: Sequence[tuple], row_begin: int, row_end: int,
+                          out: torch.Tensor) -> torch.Tensor:
+    """`region_composite` of the canvas rows [row_begin, row_end) only, written into those rows of `out` (fp32 [N,C,H,W], the
+    other rows are left as they are).  Regions are in canvas coordinates; one that is given clipped to the window (y, h and
+    its output / aux narrowed to the rows it covers there) composites the same values."""
+    _require_cuda(x_buffer, "x_buffer")
+    N, C, H, W = x_buffer.shape
+    if not x_buffer.is_contiguous() or not out.is_contiguous() or out.dtype != torch.float32 or tuple(out.shape) != (N, C, H, W):
+        raise ValueError("region_composite_rows: x_buffer and out must be contiguous whole-canvas tensors, out fp32")
+    arr, keep = _region_table(x_buffer, regions)
+    with torch.cuda.device(x_buffer.device):
+        check(lib.td_region_composite_rows(x_buffer.data_ptr(), weights.data_ptr() if weights is not None else None, arr, len(regions), N, C,
+                                           H, W, dtype_code(x_buffer.dtype), out.data_ptr(), int(row_begin), int(row_end),
+                                           current_stream_ptr(x_buffer.device)))
+    return out

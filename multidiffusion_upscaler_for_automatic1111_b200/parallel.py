@@ -36,7 +36,7 @@ class TileShard:
         self.chunk = -(-num_tiles // world)
         self.begin = min(rank * self.chunk, num_tiles)
         self.end = min(self.begin + self.chunk, num_tiles)
-        self.num_chunks = -(-num_tiles // self.chunk)     # ranks >= num_chunks own no tile
+        self.num_chunks = -(-num_tiles // self.chunk) if self.chunk else 0    # ranks >= num_chunks own no tile
 
     @property
     def num_local(self) -> int:
@@ -57,6 +57,119 @@ def gather_tile_outputs(local_padded: torch.Tensor, group=None) -> torch.Tensor:
         parts = list(out.chunk(world, dim=0))
         dist.all_gather(parts, local_padded.contiguous(), group=group)
     return out
+
+
+class RegionShard:
+    """Region prompt control under the tile shard (pure bookkeeping, no device work): which rank denoises which custom
+    region, and how the region rectangles and outputs are packed for the two all-gathers of a step.
+
+    Region j (list order) is denoised by rank j % world, on every rank the same without any communication.  Every rank
+    then needs every region output for the composite (replicate mode: of the whole canvas; strip mode: of its own rows),
+    so the owners' outputs are packed back to back in list order, padded to the largest rank's pack and all-gathered.
+    In strip mode a rank holds valid latent rows only in its own strip: the rows of region j that lie in strip [B[q],
+    B[q+1]) are packed by rank q and reach the owner of j through one more all-gather before the denoiser calls."""
+
+    def __init__(self, rects: Sequence[Sequence[int]], rank: int, world: int):
+        if not (0 <= rank < world):
+            raise ValueError(f"rank {rank} outside world {world}")
+        self.rects = [tuple(int(v) for v in r) for r in rects]        # (x, y, w, h) in latent pixels
+        self.rank, self.world = rank, world
+        self.owner = [j % world for j in range(len(self.rects))]
+
+    def mine(self, r: Optional[int] = None) -> List[int]:
+        """Regions denoised by rank r, in list order."""
+        r = self.rank if r is None else r
+        return [j for j, o in enumerate(self.owner) if o == r]
+
+    # ---- outputs: owners -> every rank -----------------------------------------------------------------------
+    def _area(self, j: int) -> int:
+        return self.rects[j][2] * self.rects[j][3]
+
+    def output_pack_numel(self, planes: int) -> int:
+        """Elements of one rank's padded output pack (planes = N * C)."""
+        return planes * max(sum(self._area(j) for j in self.mine(r)) for r in range(self.world))
+
+    def pack_outputs(self, outs: Sequence[torch.Tensor], planes: int, like: torch.Tensor) -> torch.Tensor:
+        """This rank's region outputs (in `mine()` order, [N, C, h, w] each) -> one flat padded pack of like's dtype."""
+        mine = self.mine()
+        if len(outs) != len(mine):
+            raise ValueError(f"{len(outs)} region outputs for {len(mine)} regions of rank {self.rank}")
+        pack = torch.zeros(self.output_pack_numel(planes), dtype=like.dtype, device=like.device)
+        off = 0
+        for j, o in zip(mine, outs):
+            n = planes * self._area(j)
+            pack[off:off + n].view(o.shape).copy_(o)
+            off += n
+        return pack
+
+    def unpack_outputs(self, gathered: torch.Tensor, N: int, C: int) -> List[torch.Tensor]:
+        """[world, pack] -> every region's output [N, C, h, w] in list order (views of `gathered`)."""
+        outs: List[Optional[torch.Tensor]] = [None] * len(self.rects)
+        for r in range(self.world):
+            off = 0
+            for j in self.mine(r):
+                _, _, w, h = self.rects[j]
+                n = N * C * w * h
+                outs[j] = gathered[r, off:off + n].view(N, C, h, w)
+                off += n
+        return outs
+
+    # ---- inputs in strip mode: row owners -> region owner ----------------------------------------------------
+    def input_pieces(self, lo: int, hi: int) -> List[tuple]:
+        """[(region j, a, b)]: the canvas rows [a, b) of region j that lie in [lo, hi), in list order."""
+        out = []
+        for j, (_, y, _, h) in enumerate(self.rects):
+            a, b = max(y, lo), min(y + h, hi)
+            if b > a:
+                out.append((j, a, b))
+        return out
+
+    def input_pack_numel(self, B: Sequence[int], planes: int) -> int:
+        return planes * max(sum((b - a) * self.rects[j][2] for j, a, b in self.input_pieces(B[r], B[r + 1])) for r in range(self.world))
+
+    def pack_inputs(self, x: torch.Tensor, B: Sequence[int]) -> torch.Tensor:
+        """The rows of every region rectangle inside this rank's strip [B[rank], B[rank+1]) of x [N, C, H, W] -> one flat
+        padded pack (only those rows of x are read)."""
+        planes = x.shape[0] * x.shape[1]
+        pack = torch.zeros(self.input_pack_numel(B, planes), dtype=x.dtype, device=x.device)
+        off = 0
+        for j, a, b in self.input_pieces(B[self.rank], B[self.rank + 1]):
+            rx, _, w, _ = self.rects[j]
+            n = planes * (b - a) * w
+            pack[off:off + n].view(x.shape[0], x.shape[1], b - a, w).copy_(x[:, :, a:b, rx:rx + w])
+            off += n
+        return pack
+
+    def unpack_inputs(self, gathered: torch.Tensor, B: Sequence[int], N: int, C: int) -> dict:
+        """[world, pack] -> {j: region j's input [N, C, h, w]} for this rank's regions."""
+        mine = set(self.mine())
+        ins = {}
+        for j in mine:
+            _, _, w, h = self.rects[j]
+            ins[j] = torch.empty((N, C, h, w), dtype=gathered.dtype, device=gathered.device)
+        for r in range(self.world):
+            off = 0
+            for j, a, b in self.input_pieces(B[r], B[r + 1]):
+                _, y, w, _ = self.rects[j]
+                n = N * C * (b - a) * w
+                if j in mine:
+                    ins[j][:, :, a - y:b - y] = gathered[r, off:off + n].view(N, C, b - a, w)
+                off += n
+        return ins
+
+
+def gather_region_inputs(rs: RegionShard, x: torch.Tensor, B: Sequence[int], group=None) -> dict:
+    """Strip mode: one all-gather of the strip-packed region rows -> {j: input of region j} for this rank's regions."""
+    N, C = x.shape[0], x.shape[1]
+    gathered = gather_tile_outputs(rs.pack_inputs(x, B).view(1, -1), group)
+    return rs.unpack_inputs(gathered, B, N, C)
+
+
+def exchange_region_outputs(rs: RegionShard, outs: Sequence[torch.Tensor], like: torch.Tensor, group=None) -> List[torch.Tensor]:
+    """One all-gather of the packed region outputs -> every region's output, in list order, on every rank."""
+    N, C = like.shape[0], like.shape[1]
+    gathered = gather_tile_outputs(rs.pack_outputs(outs, N * C, like).view(1, -1), group)
+    return rs.unpack_outputs(gathered, N, C)
 
 
 class _RawCudaBuffer:
@@ -140,15 +253,17 @@ class PeerExchange:
 
 
 def blend_multidiffusion_peer(g, exchange: PeerExchange, parity: int, shard: TileShard, N: int, C: int, weights: torch.Tensor,
-                              dtype: torch.dtype, out: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """Wait for every rank's step counter, then blend reading the peers' chunks over NVLink (one kernel)."""
+                              dtype: torch.dtype, out: Optional[torch.Tensor] = None, x_buffer: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Wait for every rank's step counter, then blend reading the peers' chunks over NVLink (one kernel).  With `x_buffer`
+    the un-normalised accumulator is stored there as well (region prompt control)."""
     dev = exchange.device
     nb = shard.num_chunks
     ptrs = (ctypes.c_void_p * nb)(*exchange.buf_ptrs[parity][:nb])
     x_out = out if out is not None else torch.empty((N, C, g.H, g.W), dtype=torch.float32, device=dev)
     with torch.cuda.device(dev):
         check(lib.td_blend_multidiffusion_peer(ctypes.byref(g), ptrs, nb, shard.chunk, N, C, _cabi.dtype_code(dtype),
-                                               _cabi.dtype_code(dtype), weights.data_ptr(), x_out.data_ptr(), None,
+                                               _cabi.dtype_code(dtype), weights.data_ptr(), x_out.data_ptr(),
+                                               x_buffer.data_ptr() if x_buffer is not None else None,
                                                ctypes.c_void_p(exchange.flag_ptrs[exchange.rank]), exchange.world,
                                                ctypes.c_void_p(exchange.counter_ptr), 0, _cabi.current_stream_ptr(dev)))
     return x_out
@@ -435,8 +550,11 @@ class StripExchange:
                 ptrs.append(self._own.data_ptr())
         return (ctypes.c_void_p * sh.rows)(*ptrs)
 
-    def blend(self, g, weights: torch.Tensor, rcp_weights: Optional[torch.Tensor], flags: int = 0) -> torch.Tensor:
-        """Blend this rank's strip into its IPC-mapped latent buffer (waits in-kernel for the tile halos)."""
+    def blend(self, g, weights: torch.Tensor, rcp_weights: Optional[torch.Tensor], flags: int = 0,
+              x_buffer: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Blend this rank's strip into its IPC-mapped latent buffer (waits in-kernel for the tile halos).  With `x_buffer`
+        ([N, C, H, W] of the latent dtype) the un-normalised accumulator of the strip's rows is stored there as well (the
+        region composite starts from it)."""
         sh = self.shard
         lo, hi = sh.strip()
         first = self._senders[0] if self._senders else 0
@@ -449,8 +567,8 @@ class StripExchange:
         with torch.cuda.device(self.device):
             check(lib.td_blend_multidiffusion_rows(ctypes.byref(g), self._ptr_table, sh.rows, sh.cols, self.N, self.C, _cabi.dtype_code(self.dtype),
                                                    _cabi.dtype_code(self.dtype), weights.data_ptr(),
-                                                   rcp_weights.data_ptr() if rcp_weights is not None else None, self.x_out.data_ptr(), None,
-                                                   lo, hi, f if count else None, count, v if count else None,
+                                                   rcp_weights.data_ptr() if rcp_weights is not None else None, self.x_out.data_ptr(),
+                                                   x_buffer.data_ptr() if x_buffer is not None else None, lo, hi, f if count else None, count, v if count else None,
                                                    sh.band_begin[sh.rank] if _LATE_WAIT else 0, sh.band_end[sh.rank] if _LATE_WAIT else 0, int(flags),
                                                    _cabi.current_stream_ptr(self.device)))
         return self.x_out

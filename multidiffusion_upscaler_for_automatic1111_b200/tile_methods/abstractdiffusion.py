@@ -115,6 +115,7 @@ class AbstractDiffusion:
         self._shard_mode = "replicate"
         self._strip = None
         self._strip_exchange = None
+        self._region_shard = None             # parallel.RegionShard: custom regions under the tile shard
 
     # ----------------------------------------------------------------- helpers
     def _sd_model(self):
@@ -253,20 +254,31 @@ class AbstractDiffusion:
         `sample_one_step` returns is valid on the rank's own rows plus that halo; `gather_latent` assembles the full
         latent (after the last step).  Bit-identical to a single-GPU run.
         mode "replicate": each rank denoises `tiles[begin:end)`, ALL tile outputs are exchanged (fused: peer reads over
-        NVLink inside the blend kernel; else NCCL all-gather) and every rank blends the full latent."""
+        NVLink inside the blend kernel; else NCCL all-gather) and every rank blends the full latent.
+
+        Custom regions (init_custom_bbox) are shared out as well: region j is denoised by rank j % world and its output
+        all-gathered (parallel.RegionShard); in strip mode its input rows are gathered from the strips' owners first.  Every
+        rank composites the regions over the rows it returns.  Without a background layer (draw_background=False, no
+        init_grid_bbox) only the regions are sharded, in replicate mode."""
         import torch.distributed as dist
         from .. import parallel
-        if self._grid is None:
-            raise RuntimeError("init_tile_shard() must follow init_grid_bbox()")
+        if self._grid is None and not self.enable_custom_bbox:
+            raise RuntimeError("init_tile_shard() must follow init_grid_bbox() or init_custom_bbox()")
         if mode is None:
-            mode = "strip" if (fused and self.method == "MultiDiffusion") else "replicate"
+            mode = "strip" if (fused and self.method == "MultiDiffusion" and self._grid is not None) else "replicate"
         if mode not in ("strip", "replicate"):
             raise ValueError(f"unknown shard mode {mode!r}")
+        if mode == "strip" and self._grid is None:
+            raise ValueError("the strip shard partitions the grid tiles: it needs init_grid_bbox()")
         rank, world = dist.get_rank(group), dist.get_world_size(group)
         self._shard_group, self._shard_fused, self._shard_mode = group, fused, mode
+        self._region_shard = None
         bboxes = [b for batch in self.batched_bboxes for b in batch]
         g = self._grid
-        if mode == "strip":
+        if g is None:
+            self._strip = None
+            self._shard = parallel.TileShard(0, rank, world)
+        elif mode == "strip":
             self._strip = parallel.StripShard(list(g.ys[:g.rows]), g.cols, g.tile_h, g.H, rank, world)
             t0, t1 = self._strip.tile_range()
             self._shard = parallel.TileShard(self.num_tiles, rank, world)     # kept for callers that read .begin / .end
@@ -275,7 +287,7 @@ class AbstractDiffusion:
             self._strip = None
             self._shard = parallel.TileShard(self.num_tiles, rank, world)
         local = bboxes[self._shard.begin:self._shard.end]
-        self.local_batched_bboxes = [local[i:i + self.tile_bs] for i in range(0, len(local), self.tile_bs)]
+        self.local_batched_bboxes = [local[i:i + self.tile_bs] for i in range(0, len(local), self.tile_bs)] if local else []
         return self._shard
 
     def gather_latent(self, x: Tensor) -> Tensor:
@@ -285,25 +297,68 @@ class AbstractDiffusion:
             return x
         return self._strip_exchange.gather_latent(x)
 
-    def _strip_step(self, outs, x: Tensor, N: int, C: int) -> Tensor:
-        """Strip-shard tail of MultiDiffusion.sample_one_step: own tile outputs -> halo push -> strip blend -> latent halo."""
+    def _strip_step(self, outs, x: Tensor, N: int, C: int, regions_done=None) -> Tensor:
+        """Strip-shard tail of MultiDiffusion.sample_one_step: own tile outputs -> halo push -> strip blend (-> region composite
+        of the own rows over the blend's accumulator) -> latent halo."""
         from .. import parallel
         g = self._grid
         if self._strip_exchange is None:
             self._strip_exchange = parallel.StripExchange(self._strip, N, C, g.tile_w, g.W, x.dtype, x.device, self._shard_group)
         ex = self._strip_exchange
-        own = ex.own_tiles()
-        off = 0
-        for o in outs:
-            own[off:off + o.shape[0]].copy_(o)
-            off += o.shape[0]
-        ex.push_tile_halos()
-        x_out = ex.blend(g, self.weights, self._rcp_weights if x.dtype != torch.float32 else None, flags=self._blend_flags)
+        lo, hi = self._strip.strip()
+        if self.enable_grid_bbox:
+            own = ex.own_tiles()
+            off = 0
+            for o in outs:
+                own[off:off + o.shape[0]].copy_(o)
+                off += o.shape[0]
+            ex.push_tile_halos()
+            x_out = ex.blend(g, self.weights, self._rcp_weights if x.dtype != torch.float32 else None, flags=self._blend_flags,
+                             x_buffer=self.x_buffer if regions_done is not None else None)
+        else:
+            # draw_background=False: no grid pass, the regions paint over zeros (the tile halos are not exchanged at all)
+            x_out = ex.x_out
+            self.x_buffer[:, :, lo:hi].zero_()
+        if regions_done is not None:
+            self._composite_regions(self.x_buffer, self.weights, regions_done, rows=(lo, hi), out=x_out)
         ex.push_x_halos_and_wait()
         return x_out
 
-    def _exchange_and_blend_md(self, outs, x: Tensor, N: int, C: int) -> Tensor:
-        """Tile-shard tail of MultiDiffusion.sample_one_step."""
+    def _region_pass_sharded(self, x: Tensor, custom_func: Callable, poll_interrupt: bool, interrupted: bool):
+        """`_custom_region_pass` under the tile shard: this rank denoises its regions (parallel.RegionShard: region j on rank
+        j % world), whose inputs come from the local latent (replicate mode) or from the strips' owners (strip mode, one
+        all-gather), and one all-gather of the outputs gives every rank every region output.  An interrupted rank still
+        takes part in both exchanges with placeholder outputs (its inputs) so that the collectives stay in lock-step.
+
+        Returns ([(bbox_id, bbox, x_tile_out)] in list order, interrupted)."""
+        from .. import parallel
+        if self._region_shard is None:
+            self._region_shard = parallel.RegionShard([(b.x, b.y, b.w, b.h) for b in self.custom_bboxes], self._shard.rank,
+                                                      self._shard.world)
+        rs = self._region_shard
+        if self._strip is not None:
+            inputs = parallel.gather_region_inputs(rs, x, self._strip.B, self._shard_group)
+        else:
+            inputs = {j: x[self.custom_bboxes[j].slicer] for j in rs.mine()}
+        use_networks = not getattr(self.p, "disable_extra_networks", False)
+        outs = []
+        for j in rs.mine():
+            bbox = self.custom_bboxes[j]
+            if interrupted or (poll_interrupt and host.interrupted()):
+                interrupted = True
+                outs.append(inputs[j])          # placeholder with the right shape: the exchange must still happen
+                continue
+            if use_networks:
+                host.extra_networks_activate(self.p, bbox.extra_network_data)
+            outs.append(custom_func(inputs[j], j, bbox))
+            if use_networks:
+                host.extra_networks_deactivate(self.p, bbox.extra_network_data)
+            self.update_pbar()
+        all_outs = parallel.exchange_region_outputs(rs, outs, x, self._shard_group)
+        return [(j, b, all_outs[j]) for j, b in enumerate(self.custom_bboxes)], interrupted
+
+    def _exchange_and_blend_md(self, outs, x: Tensor, N: int, C: int, x_buffer: Optional[Tensor] = None) -> Tensor:
+        """Tile-shard tail of MultiDiffusion.sample_one_step (`x_buffer`: also store the un-normalised accumulator there)."""
         from .. import parallel
         sh, g = self._shard, self._grid
         plane = N * C * g.tile_h * g.tile_w
@@ -317,7 +372,7 @@ class AbstractDiffusion:
                 buf = self._exchange.local_buffer(parity, dt)[:sh.num_local * plane].view(sh.num_local * N, C, g.tile_h, g.tile_w)
                 torch.cat([o.to(dt) for o in outs], dim=0, out=buf)
             self._exchange.signal()
-            return parallel.blend_multidiffusion_peer(g, self._exchange, parity, sh, N, C, self.weights, dt)
+            return parallel.blend_multidiffusion_peer(g, self._exchange, parity, sh, N, C, self.weights, dt, x_buffer=x_buffer)
         local = torch.zeros((sh.chunk * N, C, g.tile_h, g.tile_w), dtype=dt, device=x.device)
         if outs:
             torch.cat(outs, dim=0, out=local[:sh.num_local * N])
@@ -326,7 +381,7 @@ class AbstractDiffusion:
         for b in range(sh.num_chunks):
             nt = min(sh.chunk, sh.num_tiles - b * sh.chunk)
             chunks.append(gathered[b * sh.chunk * N: (b * sh.chunk + nt) * N])
-        return engine.blend_multidiffusion(g, chunks, N, C, sh.chunk, self.weights, x.dtype, x_buffer=None, flags=self._blend_flags,
+        return engine.blend_multidiffusion(g, chunks, N, C, sh.chunk, self.weights, x.dtype, x_buffer=x_buffer, flags=self._blend_flags,
                                            rcp_weights=self._rcp_weights)
 
     # ------------------------------------------------- region prompt control
@@ -507,16 +562,20 @@ class AbstractDiffusion:
             self.update_pbar()
         return done
 
-    def _composite_regions(self, x_buffer: Tensor, weights: Optional[Tensor], done, background_aux=None) -> Tensor:
+    def _composite_regions(self, x_buffer: Tensor, weights: Optional[Tensor], done, background_aux=None, rows=None, out=None) -> Tensor:
         """x_buffer (grid accumulator) + the collected region outputs -> the step's result, fp32 (td_region_composite:
-        BACKGROUND adds in list order, normalisation by `weights` when given, FOREGROUND feather average and overlay)."""
+        BACKGROUND adds in list order, normalisation by `weights` when given, FOREGROUND feather average and overlay).
+        rows=(lo, hi): only those canvas rows, written into `out` (td_region_composite_rows, strip shard)."""
         regions = []
-        for bbox_id, bbox, out in done:
+        for bbox_id, bbox, r_out in done:
             if bbox.blend_mode == BlendMode.BACKGROUND:
-                regions.append((bbox.x, bbox.y, bbox.w, bbox.h, 0, out, background_aux(bbox_id) if background_aux is not None else None))
+                regions.append((bbox.x, bbox.y, bbox.w, bbox.h, 0, r_out, background_aux(bbox_id) if background_aux is not None else None))
             elif bbox.blend_mode == BlendMode.FOREGROUND:
-                regions.append((bbox.x, bbox.y, bbox.w, bbox.h, 1, out, bbox.feather_mask))
-        return engine.region_composite(x_buffer, weights.view(x_buffer.shape[2], x_buffer.shape[3]) if weights is not None else None, regions)
+                regions.append((bbox.x, bbox.y, bbox.w, bbox.h, 1, r_out, bbox.feather_mask))
+        w2d = weights.view(x_buffer.shape[2], x_buffer.shape[3]) if weights is not None else None
+        if rows is not None:
+            return engine.region_composite_rows(x_buffer, w2d, regions, rows[0], rows[1], out)
+        return engine.region_composite(x_buffer, w2d, regions)
 
     # -------------------------------------------------- tiled noise inversion
     @noise_inverse

@@ -89,13 +89,14 @@ class MixtureOfDiffusers(AbstractDiffusion):
         x = self._check_input(x_in)
         self.reset_buffer(x)
         regions = self.enable_custom_bbox and len(self.custom_bboxes) > 0
-        if regions and self._shard is not None:
-            raise NotImplementedError("region prompt control is not combined with the multi-GPU tile shard yet")
+        interrupted = False
 
         if self.enable_grid_bbox:
             x_out = self._grid_pass(x_in, x, t_in, c_in, sd_model, N, C)
             if x_out is None:
-                return x_in            # interrupted
+                if self._shard is None or not regions:
+                    return x_in        # interrupted
+                interrupted = True     # sharded: the region exchange still has to happen
         else:
             # draw_background=False: only the custom regions paint (mixtureofdiffusers.py:82 skips the grid loop)
             self.x_buffer.zero_()
@@ -112,7 +113,12 @@ class MixtureOfDiffusers(AbstractDiffusion):
             c_out = self.make_cond_dict(c_in, tcond, icond, self.get_vcond(c_in))
             return sd_model.apply_model(x_tile, t_in, cond=c_out)
 
-        done = self._custom_region_pass(x, custom_func, poll_interrupt=False)
+        if self._shard is not None:
+            done, interrupted = self._region_pass_sharded(x, custom_func, False, interrupted)
+            if interrupted:
+                return x_in
+        else:
+            done = self._custom_region_pass(x, custom_func, poll_interrupt=False)
         # mixtureofdiffusers.py:145-175 in one launch: BACKGROUND adds weighted by the pre-rescaled custom weights, no
         # normalisation, FOREGROUND feather overlay
         out = self._composite_regions(self.x_buffer, None, done, background_aux=lambda bbox_id: self.custom_weights[bbox_id])
@@ -173,10 +179,12 @@ class MixtureOfDiffusers(AbstractDiffusion):
     def _grid_pass_sharded(self, x: Tensor, t_in: Tensor, c_in: CondDict, sd_model, N: int, C: int):
         """Tile shard (init_tile_shard): this rank denoises its contiguous chunk of the tile list, the eps tiles are
         all-gathered, and every rank runs the same ordered gaussian blend over all tiles -- bit-identical to the
-        single-GPU result on every rank."""
+        single-GPU result on every rank.  An interrupted rank stops its denoiser calls but still joins the all-gather
+        (placeholder tiles) so that the collectives stay in lock-step, then returns None."""
         from .. import parallel
         sh, g = self._shard, self._grid
         outs = []
+        interrupted = False
         if sh.num_local > 0:
             self._tiles = engine.scatter_tiles(g, x, out=self._tiles, tile_begin=sh.begin, tile_end=sh.end, flags=self._blend_flags)
             icond_tiles, n_icond = None, 0
@@ -187,12 +195,14 @@ class MixtureOfDiffusers(AbstractDiffusion):
                     n_icond = icond_full.shape[0]
             off = 0
             for batch_id, bboxes in enumerate(self.local_batched_bboxes):
-                if host.interrupted():
-                    return None
                 n_rep = len(bboxes)
                 x_tile = self._tiles[off * N:(off + n_rep) * N]
                 icond_tile = icond_tiles[off * n_icond:(off + n_rep) * n_icond] if icond_tiles is not None else None
                 off += n_rep
+                if interrupted or host.interrupted():
+                    interrupted = True
+                    outs.append(x_tile)
+                    continue
                 outs.append(self._denoise_tile_batch(sd_model, x_tile, n_rep, t_in, c_in, icond_tile, batch_id, N))
                 self.update_pbar()
         dt = outs[0].dtype if outs else x.dtype
@@ -204,8 +214,9 @@ class MixtureOfDiffusers(AbstractDiffusion):
         for b in range(sh.num_chunks):
             nt = min(sh.chunk, sh.num_tiles - b * sh.chunk)
             chunks.append(gathered[b * sh.chunk * N:(b * sh.chunk + nt) * N])
-        return engine.blend_mixture(g, chunks, N, C, sh.chunk, self.tile_weights, self.rescale_factor, self.x_buffer,
-                                    flags=self._blend_flags)
+        x_out = engine.blend_mixture(g, chunks, N, C, sh.chunk, self.tile_weights, self.rescale_factor, self.x_buffer,
+                                     flags=self._blend_flags)
+        return None if interrupted else x_out
 
     def custom_apply_model(self, x_in: Tensor, t_in: Tensor, c_in: CondDict, bbox_id: int, bbox: CustomBBox) -> Tensor:
         """mixtureofdiffusers.py:181-196: a region goes through the un-hijacked `apply_model` with its own prompts."""

@@ -10,7 +10,7 @@ kernel (pointer table, no concatenation copy).
 """
 from __future__ import annotations
 
-from typing import Callable, List, Union
+from typing import Callable, List, Optional, Union
 
 import torch
 from torch import Tensor
@@ -155,9 +155,7 @@ class MultiDiffusion(AbstractDiffusion):
         self._step_token = self.__dict__.get("_step_token", 0) + 1     # memoised per-batch inputs are re-validated once per step
         regions = self.enable_custom_bbox and len(self.custom_bboxes) > 0
         if self._shard is not None:
-            if regions:
-                raise NotImplementedError("region prompt control is not combined with the multi-GPU tile shard yet")
-            return self._sample_one_step_sharded(x_in, x, repeat_func, N, C)
+            return self._sample_one_step_sharded(x_in, x, repeat_func, custom_func if regions else None, N, C)
 
         x_out = None
         if self.enable_grid_bbox:
@@ -193,8 +191,10 @@ class MultiDiffusion(AbstractDiffusion):
         # multidiffusion.py:187-216 in one launch: BACKGROUND adds, divide where weights > 1, FOREGROUND feather overlay
         return self._composite_regions(self.x_buffer, self.weights, done)
 
-    def _sample_one_step_sharded(self, x_in: Tensor, x: Tensor, repeat_func: Callable, N: int, C: int) -> Tensor:
-        """This rank's tiles, then the exchange + deterministic blend (init_tile_shard).
+    def _sample_one_step_sharded(self, x_in: Tensor, x: Tensor, repeat_func: Callable, custom_func: Optional[Callable], N: int,
+                                 C: int) -> Tensor:
+        """This rank's tiles (and custom regions, when `custom_func` is given), then the exchange + deterministic blend
+        (init_tile_shard), then the region composite over the blend's accumulator.
 
         An interrupt (multidiffusion.py:152) stops the denoiser calls of THIS rank but not its part of the exchange:
         the peers' kernels wait for this rank's signal, so the step always publishes (possibly stale) tile outputs,
@@ -202,7 +202,7 @@ class MultiDiffusion(AbstractDiffusion):
         sh = self._shard
         outs = []
         interrupted = False
-        if sh.num_local > 0:
+        if self.enable_grid_bbox and sh.num_local > 0:
             self._tiles = engine.scatter_tiles(self._grid, x, out=self._tiles, tile_begin=sh.begin, tile_end=sh.end,
                                                flags=self._blend_flags)
             off = 0
@@ -215,10 +215,21 @@ class MultiDiffusion(AbstractDiffusion):
                     continue
                 outs.append(repeat_func(x_tile, bboxes))
                 self.update_pbar()
+        done = None
+        if custom_func is not None:
+            # the region exchange (NCCL) comes before the tile exchange: its in-kernel waits then never sit in front of a collective
+            self.reset_buffer(x)
+            done, interrupted = self._region_pass_sharded(x, custom_func, True, interrupted)
         if self._shard_mode == "strip":
-            out = self._strip_step(outs, x, N, C)
-        else:
+            out = self._strip_step(outs, x, N, C, done)
+        elif done is None:
             out = self._exchange_and_blend_md(outs, x, N, C)
+        else:
+            if self.enable_grid_bbox:
+                self._exchange_and_blend_md(outs, x, N, C, x_buffer=self.x_buffer)
+            else:
+                self.x_buffer.zero_()
+            out = self._composite_regions(self.x_buffer, self.weights, done)
         return x_in if interrupted else out
 
     def get_noise(self, x_in: Tensor, sigma_in: Tensor, cond_in: CondDict, step: int) -> Tensor:
