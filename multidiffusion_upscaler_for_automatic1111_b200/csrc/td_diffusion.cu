@@ -1091,7 +1091,12 @@ blend_grid_generic_kernel(const __grid_constant__ BlendParams p, const float* __
 // magic = ceil(2^32 / d) for fastdiv(); 0 encodes d == 1
 unsigned magic_u16(unsigned d) { return d <= 1 ? 0u : (unsigned)(((1ull << 32) + d - 1) / d); }
 
-int fill_geom(const td_grid* g, int N, int C, GeomParams* o) {
+constexpr uint32_t kWrapBits = TD_FLAG_WRAP_X | TD_FLAG_WRAP_Y;
+constexpr uint32_t kOptInForms = TD_FLAG_ROWS | TD_FLAG_STRIP | TD_FLAG_TMA | TD_FLAG_PIPELINE;
+
+// `wrap`: the TD_FLAG_WRAP_* bits of the call.  On an axis whose bit is clear every tile must lie inside the canvas
+// (the kernels of this file index the canvas without bounds checks); on a periodic axis an origin lies in [0, extent).
+int fill_geom(const td_grid* g, int N, int C, GeomParams* o, uint32_t wrap = 0) {
     if (g == nullptr) { td_set_error("null grid"); return TD_ERR_INVALID_ARG; }
     if (N <= 0 || C <= 0) { td_set_error("N and C must be positive (N=%d C=%d)", N, C); return TD_ERR_INVALID_ARG; }
     if (g->rows <= 0 || g->cols <= 0 || g->rows > TD_MAX_GRID_DIM || g->cols > TD_MAX_GRID_DIM ||
@@ -1100,6 +1105,22 @@ int fill_geom(const td_grid* g, int N, int C, GeomParams* o) {
         return TD_ERR_INVALID_ARG;
     }
     if (g->H >= 32768 || g->W >= 32768) { td_set_error("canvas %dx%d too large", g->H, g->W); return TD_ERR_UNSUPPORTED; }
+    if (g->tile_w <= 0 || g->tile_h <= 0 || g->tile_w > g->W || g->tile_h > g->H) {
+        td_set_error("tile %dx%d does not fit the %dx%d canvas", g->tile_w, g->tile_h, g->W, g->H);
+        return TD_ERR_INVALID_ARG;
+    }
+    for (int c = 0; c < g->cols; ++c)
+        if (g->xs[c] < 0 || g->xs[c] >= g->W || (!(wrap & TD_FLAG_WRAP_X) && g->xs[c] + g->tile_w > g->W)) {
+            td_set_error("tile column %d (x=%d, w=%d) leaves the %d-wide canvas%s", c, g->xs[c], g->tile_w, g->W,
+                         (wrap & TD_FLAG_WRAP_X) ? "" : " (a periodic plan needs TD_FLAG_WRAP_X)");
+            return TD_ERR_INVALID_ARG;
+        }
+    for (int r = 0; r < g->rows; ++r)
+        if (g->ys[r] < 0 || g->ys[r] >= g->H || (!(wrap & TD_FLAG_WRAP_Y) && g->ys[r] + g->tile_h > g->H)) {
+            td_set_error("tile row %d (y=%d, h=%d) leaves the %d-high canvas%s", r, g->ys[r], g->tile_h, g->H,
+                         (wrap & TD_FLAG_WRAP_Y) ? "" : " (a periodic plan needs TD_FLAG_WRAP_Y)");
+            return TD_ERR_INVALID_ARG;
+        }
     o->H = g->H; o->W = g->W; o->th = g->tile_h; o->tw = g->tile_w;
     o->rows = g->rows; o->cols = g->cols; o->N = N; o->C = C;
     for (int i = 0; i < g->rows; ++i) o->ys[i] = (short)g->ys[i];
@@ -1433,8 +1454,8 @@ int dispatch_generic(int tile_dtype, int acc_dtype, const BlendParams& bp, const
 }
 
 int fill_blend(const td_grid* g, const void* const* batch_ptrs, int num_batches, int tile_bs, int N, int C, int tile_dtype,
-               int acc_dtype, BlendParams* bp) {
-    int st = fill_geom(g, N, C, &bp->g);
+               int acc_dtype, BlendParams* bp, uint32_t wrap = 0) {
+    int st = fill_geom(g, N, C, &bp->g, wrap);
     if (st != TD_OK) return st;
     if (td_dtype_size(tile_dtype) == 0 || td_dtype_size(acc_dtype) == 0) { td_set_error("unknown dtype"); return TD_ERR_INVALID_ARG; }
     if (batch_ptrs == nullptr || num_batches <= 0 || tile_bs <= 0) { td_set_error("bad batch pointer table"); return TD_ERR_INVALID_ARG; }
@@ -1457,6 +1478,23 @@ int fill_blend(const td_grid* g, const void* const* batch_ptrs, int num_batches,
     bp->bs_magic = magic_u16((unsigned)tile_bs);
     bp->num_batches = num_batches;
     bp->tile_stride = (long long)N * C * g->tile_h * g->tile_w;
+    return TD_OK;
+}
+
+// the wrap bits select td_wrap.cu, which has one form: the opt-in forms of this file do not take them
+int refuse_opt_in(uint32_t flags, const char* what) {
+    if ((flags & kWrapBits) && (flags & kOptInForms)) {
+        td_set_error("%s: TD_FLAG_WRAP_X / TD_FLAG_WRAP_Y do not combine with the ROWS / STRIP / TMA / PIPELINE forms", what);
+        return TD_ERR_UNSUPPORTED;
+    }
+    return TD_OK;
+}
+
+int refuse_wrap(uint32_t flags, const char* what) {
+    if (flags & kWrapBits) {
+        td_set_error("%s: no form for a periodic canvas (TD_FLAG_WRAP_X / TD_FLAG_WRAP_Y)", what);
+        return TD_ERR_UNSUPPORTED;
+    }
     return TD_OK;
 }
 
@@ -1485,8 +1523,9 @@ extern "C" int td_debug_launch_empty(int blocks, int threads, void* stream) {
 extern "C" int td_scatter_tiles(const td_grid* g, const void* x, void* tiles, int N, int C, int dtype, int tile_begin,
                                 int tile_end, uint32_t flags, void* stream) {
     GeomParams gp;
-    int st = fill_geom(g, N, C, &gp);
+    int st = fill_geom(g, N, C, &gp, flags & kWrapBits);
     if (st != TD_OK) return st;
+    if ((st = refuse_opt_in(flags, "td_scatter_tiles")) != TD_OK) return st;
     if (x == nullptr || tiles == nullptr) { td_set_error("td_scatter_tiles: null tensor"); return TD_ERR_INVALID_ARG; }
     if (tile_begin < 0 || tile_end < tile_begin || tile_end > g->num_tiles) {
         td_set_error("td_scatter_tiles: tile range [%d,%d) outside [0,%d)", tile_begin, tile_end, g->num_tiles);
@@ -1494,6 +1533,7 @@ extern "C" int td_scatter_tiles(const td_grid* g, const void* x, void* tiles, in
     }
     const int es = td_dtype_size(dtype);
     if (es == 0) { td_set_error("td_scatter_tiles: unknown dtype %d", dtype); return TD_ERR_INVALID_ARG; }
+    if (flags & kWrapBits) return td_wrap_scatter(g, x, tiles, N, C, dtype, tile_begin, tile_end, flags, stream);
     const int vec = 16 / es;
     tl_pdl = !(flags & TD_FLAG_NO_PDL);
     const bool vec_ok = !(flags & TD_FLAG_FORCE_GENERIC) && gp.W % vec == 0 && gp.tw % vec == 0 && aligned16(x) && aligned16(tiles);
@@ -1513,9 +1553,13 @@ extern "C" int td_blend_multidiffusion(const td_grid* g, const void* const* batc
     BlendParams bp;
     tl_pdl = !(flags & TD_FLAG_NO_PDL);
     tl_ppc_max = (flags & TD_FLAG_ONE_PLANE) ? 1 : TD_AS_PPC;
-    int st = fill_blend(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, &bp);
+    int st = fill_blend(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, &bp, flags & kWrapBits);
     if (st != TD_OK) return st;
     if (weights == nullptr || x_out == nullptr) { td_set_error("td_blend_multidiffusion: null weights / x_out"); return TD_ERR_INVALID_ARG; }
+    if ((st = refuse_opt_in(flags, "td_blend_multidiffusion")) != TD_OK) return st;
+    if (flags & kWrapBits)
+        return td_wrap_blend(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, 0, weights, nullptr, nullptr, x_out, x_buffer,
+                             flags, stream);
     bp.g.dbg_no_tiles = (flags & TD_FLAG_DBG_NO_TILES) ? 1 : 0;
     cudaStream_t s = (cudaStream_t)stream;
     if (!(flags & TD_FLAG_FORCE_GENERIC) && blend_vec_ok(bp, tile_dtype, acc_dtype, {weights, rcp_weights, x_out, x_buffer})) {
@@ -1563,7 +1607,9 @@ extern "C" int td_blend_multidiffusion_rows(const td_grid* g, const void* const*
     BlendParams bp;
     tl_pdl = !(flags & TD_FLAG_NO_PDL);
     tl_ppc_max = (flags & TD_FLAG_ONE_PLANE) ? 1 : TD_AS_PPC;
-    int st = fill_blend(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, &bp);
+    int st = refuse_wrap(flags, "td_blend_multidiffusion_rows");
+    if (st != TD_OK) return st;
+    st = fill_blend(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, &bp);
     if (st != TD_OK) return st;
     if (weights == nullptr || x_out == nullptr) { td_set_error("td_blend_multidiffusion_rows: null weights / x_out"); return TD_ERR_INVALID_ARG; }
     if (row_begin < 0 || row_end > g->H || row_begin > row_end || row_begin % 8 != 0 || (row_end % 8 != 0 && row_end != g->H)) {
@@ -1615,7 +1661,9 @@ extern "C" int td_blend_multidiffusion_peer(const td_grid* g, const void* const*
     BlendParams bp;
     tl_pdl = !(flags & TD_FLAG_NO_PDL);
     tl_ppc_max = (flags & TD_FLAG_ONE_PLANE) ? 1 : TD_AS_PPC;
-    int st = fill_blend(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, &bp);
+    int st = refuse_wrap(flags, "td_blend_multidiffusion_peer");
+    if (st != TD_OK) return st;
+    st = fill_blend(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, &bp);
     if (st != TD_OK) return st;
     if (weights == nullptr || x_out == nullptr) { td_set_error("td_blend_multidiffusion_peer: null weights / x_out"); return TD_ERR_INVALID_ARG; }
     if (wait_flags == nullptr || wait_value == nullptr || world <= 0 || world > TD_MAX_PEERS) { td_set_error("td_blend_multidiffusion_peer: bad wait table"); return TD_ERR_INVALID_ARG; }
@@ -1647,12 +1695,16 @@ extern "C" int td_blend_mixture(const td_grid* g, const void* const* batch_ptrs,
     BlendParams bp;
     tl_pdl = !(flags & TD_FLAG_NO_PDL);
     tl_ppc_max = (flags & TD_FLAG_ONE_PLANE) ? 1 : TD_AS_PPC;
-    int st = fill_blend(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, &bp);
+    int st = fill_blend(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, &bp, flags & kWrapBits);
     if (st != TD_OK) return st;
     if (tile_weights == nullptr || rescale == nullptr || x_buffer == nullptr) {
         td_set_error("td_blend_mixture: null tile_weights / rescale / x_buffer");
         return TD_ERR_INVALID_ARG;
     }
+    if ((st = refuse_opt_in(flags, "td_blend_mixture")) != TD_OK) return st;
+    if (flags & kWrapBits)
+        return td_wrap_blend(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, 1, nullptr, tile_weights, rescale, nullptr,
+                             x_buffer, flags, stream);
     cudaStream_t s = (cudaStream_t)stream;
     if (!(flags & TD_FLAG_FORCE_GENERIC) && blend_vec_ok(bp, tile_dtype, acc_dtype, {rescale, x_buffer})) {
         if (flags & TD_FLAG_ROWS) {   // opt-in: row-block form (td_rows.cu)

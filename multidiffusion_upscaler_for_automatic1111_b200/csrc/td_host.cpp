@@ -41,6 +41,14 @@ struct Split {
     double dx, dy;
 };
 
+// One axis of split_bboxes: tile count (utils.py:161-162) and origin stride (utils.py:163-164).  Requires t != ov.
+// NB: overlap > tile is legal when the tile was clamped to the canvas
+// (abstractdiffusion.py:176-178): (L-ov)/(t-ov) is then negative/negative.
+inline void axis_split(int L, int t, int ov, int* n, double* d) {
+    *n = std::max(0, ceil_div_py(L - ov, t - ov));  // Python: range(negative) is empty -> no tiles
+    *d = *n > 1 ? (double)(L - t) / (double)(*n - 1) : 0.0;
+}
+
 inline int split_counts(int w, int h, int tile_w, int tile_h, int overlap, Split* s) {
     if (w <= 0 || h <= 0 || tile_w <= 0 || tile_h <= 0 || overlap < 0) {
         td_set_error("split_bboxes: non-positive size (w=%d h=%d tile=%dx%d overlap=%d)", w, h, tile_w, tile_h, overlap);
@@ -54,14 +62,8 @@ inline int split_counts(int w, int h, int tile_w, int tile_h, int overlap, Split
         td_set_error("split_bboxes: tile %dx%d larger than canvas %dx%d", tile_w, tile_h, w, h);
         return TD_ERR_INVALID_ARG;
     }
-    // NB: overlap > tile is legal when the tile was clamped to the canvas
-    // (abstractdiffusion.py:176-178): (w-ov)/(tw-ov) is then negative/negative.
-    s->cols = ceil_div_py(w - overlap, tile_w - overlap);
-    s->rows = ceil_div_py(h - overlap, tile_h - overlap);
-    if (s->cols < 0) s->cols = 0;  // Python: range(negative) is empty -> no tiles
-    if (s->rows < 0) s->rows = 0;
-    s->dx = s->cols > 1 ? (double)(w - tile_w) / (double)(s->cols - 1) : 0.0;  // utils.py:163
-    s->dy = s->rows > 1 ? (double)(h - tile_h) / (double)(s->rows - 1) : 0.0;  // utils.py:164
+    axis_split(w, tile_w, overlap, &s->cols, &s->dx);
+    axis_split(h, tile_h, overlap, &s->rows, &s->dy);
     return TD_OK;
 }
 
@@ -219,6 +221,117 @@ extern "C" int td_grid_weights(const td_grid* g, const float* tile_weights, floa
                     for (int u = 0; u < tw; ++u) o[u] = o[u] + tw_row[u];
                 } else {
                     for (int u = 0; u < tw; ++u) o[u] = o[u] + 1.0f;
+                }
+            }
+        }
+    return TD_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Seamless (periodic) tile plans.  A wrapped axis of length L is tiled as a circle: tile k starts at
+// floor(k * L / n) with n = ceil(L / (t - overlap)), so the gap between neighbours -- the last and the first
+// included -- is at most ceil(L / n) <= t - overlap, and a tile may run past L, continuing at 0.
+// ---------------------------------------------------------------------------------------------------------
+namespace {
+
+// the bounded rule of td_grid_init for one axis (the same axis_split / origin)
+int linear_axis(int L, int t, int ov, int* n_out, int32_t* org) {
+    if (t == ov) {
+        td_set_error("grid_init_wrap: overlap %d equals the tile size %d: division by zero", ov, t);
+        return TD_ERR_INVALID_ARG;
+    }
+    int n = 0;
+    double d = 0.0;
+    axis_split(L, t, ov, &n, &d);
+    if (n > TD_MAX_GRID_DIM) {
+        td_set_error("grid_init_wrap: %d tiles on one axis exceed TD_MAX_GRID_DIM=%d", n, TD_MAX_GRID_DIM);
+        return TD_ERR_UNSUPPORTED;
+    }
+    for (int i = 0; i < n; ++i) org[i] = origin(i, d, L - t);
+    *n_out = n;
+    return TD_OK;
+}
+
+int periodic_axis(int L, int t, int ov, int* n_out, int32_t* org) {
+    if (t == L) {
+        org[0] = 0;
+        *n_out = 1;
+        return TD_OK;
+    }
+    if (t <= ov) {
+        td_set_error("grid_init_wrap: overlap %d leaves no stride on a tile of %d", ov, t);
+        return TD_ERR_INVALID_ARG;
+    }
+    const int n = ceil_div_py(L, t - ov);
+    if (n > TD_MAX_GRID_DIM) {
+        td_set_error("grid_init_wrap: %d tiles on one axis exceed TD_MAX_GRID_DIM=%d", n, TD_MAX_GRID_DIM);
+        return TD_ERR_UNSUPPORTED;
+    }
+    const double d = (double)L / (double)n;
+    for (int k = 0; k < n; ++k) org[k] = (int32_t)std::floor((double)k * d);
+    *n_out = n;
+    return TD_OK;
+}
+
+}  // namespace
+
+extern "C" int td_grid_init_wrap(td_grid* g, int w, int h, int tile_w, int tile_h, int overlap, int tile_bs, int wrap) {
+    if (wrap == 0) return td_grid_init(g, w, h, tile_w, tile_h, overlap, tile_bs);
+    if (g == nullptr || tile_bs <= 0 || (wrap & ~3) != 0) {
+        td_set_error("grid_init_wrap: bad args");
+        return TD_ERR_INVALID_ARG;
+    }
+    if (tile_w <= 0 || tile_h <= 0 || w <= 0 || h <= 0) {
+        td_set_error("grid_init_wrap: non-positive size");
+        return TD_ERR_INVALID_ARG;
+    }
+    std::memset(g, 0, sizeof(*g));
+    g->W = w; g->H = h;
+    g->tile_w = std::min(tile_w, w);
+    g->tile_h = std::min(tile_h, h);
+    g->overlap = std::max(0, std::min(overlap, std::min(tile_w, tile_h) - 4));
+    int cols = 0, rows = 0;
+    int st = (wrap & 1) ? periodic_axis(w, g->tile_w, g->overlap, &cols, g->xs) : linear_axis(w, g->tile_w, g->overlap, &cols, g->xs);
+    if (st != TD_OK) return st;
+    st = (wrap & 2) ? periodic_axis(h, g->tile_h, g->overlap, &rows, g->ys) : linear_axis(h, g->tile_h, g->overlap, &rows, g->ys);
+    if (st != TD_OK) return st;
+    g->rows = rows; g->cols = cols;
+    g->num_tiles = rows * cols;
+    if (g->num_tiles == 0) {
+        td_set_error("grid_init_wrap: the split produced no tiles (w=%d h=%d tile=%dx%d overlap=%d)", w, h, g->tile_w, g->tile_h, g->overlap);
+        return TD_ERR_INVALID_ARG;
+    }
+    g->num_batches = ceil_div_py(g->num_tiles, tile_bs);
+    g->tile_bs = ceil_div_py(g->num_tiles, g->num_batches);
+    return g->num_tiles;
+}
+
+extern "C" int td_grid_weights_wrap(const td_grid* g, int wrap, const float* tile_weights, float* out) {
+    if (g == nullptr || out == nullptr || (wrap & ~3) != 0) {
+        td_set_error("grid_weights_wrap: bad args");
+        return TD_ERR_INVALID_ARG;
+    }
+    const int W = g->W, H = g->H, tw = g->tile_w, th = g->tile_h;
+    for (int c = 0; c < g->cols; ++c)
+        if (g->xs[c] < 0 || g->xs[c] >= W || tw > W || (!(wrap & 1) && g->xs[c] + tw > W)) {
+            td_set_error("grid_weights_wrap: tile column %d (x=%d, w=%d) leaves the %d-wide canvas", c, g->xs[c], tw, W);
+            return TD_ERR_INVALID_ARG;
+        }
+    for (int r = 0; r < g->rows; ++r)
+        if (g->ys[r] < 0 || g->ys[r] >= H || th > H || (!(wrap & 2) && g->ys[r] + th > H)) {
+            td_set_error("grid_weights_wrap: tile row %d (y=%d, h=%d) leaves the %d-high canvas", r, g->ys[r], th, H);
+            return TD_ERR_INVALID_ARG;
+        }
+    std::fill(out, out + (size_t)W * H, 0.0f);
+    for (int r = 0; r < g->rows; ++r)
+        for (int c = 0; c < g->cols; ++c) {  // list order: row outer, col inner
+            const int x0 = g->xs[c], y0 = g->ys[r];
+            for (int v = 0; v < th; ++v) {
+                const int y = (y0 + v) % H;
+                float* o = out + (size_t)y * W;
+                for (int u = 0; u < tw; ++u) {
+                    const int x = (x0 + u) % W;
+                    o[x] = o[x] + (tile_weights ? tile_weights[(size_t)v * tw + u] : 1.0f);
                 }
             }
         }

@@ -84,6 +84,34 @@ nchw_to_nhwc_kernel(const T* __restrict__ x, T* __restrict__ y, int C, long long
     }
 }
 
+// The same for a tile of a periodic canvas (seamless tiling): the tile's rows / columns start at (row0, col0) in
+// unwrapped coordinates and are read modulo the canvas (H, W): y[n, i, j, c] = x[n, c, (row0 + i) mod H, (col0 + j) mod W].
+template <typename T>
+__global__ void __launch_bounds__(kNhwcThreads)
+nchw_to_nhwc_wrap_kernel(const T* __restrict__ x, T* __restrict__ y, int C, long long x_plane, long long x_pitch, long long x_img,
+                         int rows, int cols, int row0, int col0, int H, int W, int Cpad, long long total) {
+    const int cv = Cpad / 8;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const long long pix_total = total / cv;
+        const int v = (int)(i / pix_total);
+        const long long pix = i - (long long)v * pix_total;
+        const int j = (int)(pix % cols);
+        const long long t = pix / cols;
+        const int r = (int)(t % rows);
+        const long long n = t / rows;
+        int sy = (row0 + r) % H, sx = (col0 + j) % W;
+        if (sy < 0) sy += H;
+        if (sx < 0) sx += W;
+        float f[8];
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            const int c = v * 8 + k;
+            f[k] = c < C ? Elem<T>::to_f32(x[n * x_img + (long long)c * x_plane + (long long)sy * x_pitch + sx]) : 0.0f;
+        }
+        *reinterpret_cast<uint4*>(y + pix * Cpad + v * 8) = vpack<T>(f);
+    }
+}
+
 // NHWC -> NCHW region: y[n, c, i, j] = x[n, sy + i, sx + j, c] for c < C (crop + paste + layout in one pass)
 template <typename T>
 __global__ void __launch_bounds__(kNhwcThreads)
@@ -309,6 +337,25 @@ extern "C" int td_nchw_to_nhwc(const void* x, void* y, int N, int C, int rows, i
     else
         nchw_to_nhwc_kernel<__nv_bfloat16><<<grid, kNhwcThreads, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)y, C, x_plane_stride, x_pitch, x_img_stride, rows, cols, Cpad, total);
     return nhwc_check("td_nchw_to_nhwc");
+}
+
+extern "C" int td_nchw_to_nhwc_wrap(const void* x, void* y, int N, int C, int rows, int cols, int row0, int col0, int H, int W,
+                                    int64_t x_img_stride, int64_t x_plane_stride, int64_t x_pitch, int Cpad, int dtype, void* stream) {
+    if (x == nullptr || y == nullptr || N <= 0 || C <= 0 || rows <= 0 || cols <= 0 || H <= 0 || W <= 0 || Cpad < C || Cpad % 8 != 0 ||
+        !half_like(dtype)) {
+        td_set_error("td_nchw_to_nhwc_wrap: bad arguments (fp16 / bf16, Cpad >= C and a multiple of 8)");
+        return TD_ERR_INVALID_ARG;
+    }
+    const long long total = (long long)N * rows * cols * (Cpad / 8);
+    const int grid = grid_for(total, kNhwcThreads);
+    if (dtype == TD_F16)
+        nchw_to_nhwc_wrap_kernel<__half><<<grid, kNhwcThreads, 0, (cudaStream_t)stream>>>((const __half*)x, (__half*)y, C, x_plane_stride, x_pitch,
+                                                                                        x_img_stride, rows, cols, row0, col0, H, W, Cpad, total);
+    else
+        nchw_to_nhwc_wrap_kernel<__nv_bfloat16><<<grid, kNhwcThreads, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)y, C,
+                                                                                               x_plane_stride, x_pitch, x_img_stride, rows, cols,
+                                                                                               row0, col0, H, W, Cpad, total);
+    return nhwc_check("td_nchw_to_nhwc_wrap");
 }
 
 extern "C" int td_nhwc_to_nchw_region(const void* x, void* y, int N, int C, int rows, int cols, int64_t x_img_stride, int x_width,

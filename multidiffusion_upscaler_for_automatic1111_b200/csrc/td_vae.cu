@@ -17,6 +17,7 @@
 #include <cfloat>
 #include <cmath>
 #include <cstdint>
+#include <vector>
 
 #include "td_b200.h"
 #include "td_device.cuh"
@@ -417,27 +418,79 @@ extern "C" int td_vae_best_tile_size(int lowerbound, int upperbound) {  // tilev
     return lowerbound;
 }
 
-extern "C" int td_vae_split_tiles(int h, int w, int tile_size, int pad, int is_decoder, int32_t* in_bboxes, int32_t* out_bboxes,
-                                  int cap) {  // tilevae.py:405-462; bbox order [x1, x2, y1, y2]
-    if (h <= 0 || w <= 0 || tile_size <= 0 || pad < 0) { td_set_error("td_vae_split_tiles: bad arguments"); return TD_ERR_INVALID_ARG; }
-    auto ceil_div = [](int a, int b) { return (int)std::ceil((double)a / (double)b); };
-    const int n_h = std::max(ceil_div(h - 2 * pad, tile_size), 1);
-    const int n_w = std::max(ceil_div(w - 2 * pad, tile_size), 1);
-    const int real_h = td_vae_best_tile_size(ceil_div(h - 2 * pad, n_h), tile_size);
-    const int real_w = td_vae_best_tile_size(ceil_div(w - 2 * pad, n_w), tile_size);
-    const long long T = (long long)n_h * n_w;
+namespace {
+
+// One axis of split_tiles (tilevae.py:405-462): tile k's input span [in0, in1) and output span [out0, out1), the output
+// already scaled x8 (decoder) or //8 (encoder).  The bounded rule clips the input to [0, L) and snaps the outputs at
+// the borders.  The periodic rule (seamless tiling) cuts L at b_k = m * floor(k * L / (n * m)), n = max(ceil(L / tile), 1),
+// m = 8 for the encoder (whole latent pixels) and 1 for the decoder, b_n = L; the input span is [b_k - pad, b_{k+1} + pad)
+// in UNwrapped coordinates (it may start below 0 or end past L: the tile load reads it modulo L), so every output span
+// lies inside [0, L) and the output spans partition it.
+struct VaeAxis {
+    int n = 0;
+    std::vector<int> in0, in1, out0, out1;
+    void resize(int k) { n = k; in0.resize(k); in1.resize(k); out0.resize(k); out1.resize(k); }
+};
+
+int vae_axis(int L, int tile_size, int pad, int is_decoder, bool periodic, VaeAxis* a) {
+    auto ceil_div = [](int x, int y) { return (int)std::ceil((double)x / (double)y); };
+    auto scale = [&](int v) { return is_decoder ? v * 8 : (int)std::floor((double)v / 8.0); };
+    if (!periodic) {
+        const int n = std::max(ceil_div(L - 2 * pad, tile_size), 1);
+        const int real = td_vae_best_tile_size(ceil_div(L - 2 * pad, n), tile_size);
+        a->resize(n);
+        for (int j = 0; j < n; ++j) {
+            const int b0 = pad + j * real, b1 = std::min(pad + (j + 1) * real, L);
+            a->out0[j] = scale(b0 > pad ? b0 : 0);
+            a->out1[j] = scale(b1 < L - pad ? b1 : L);
+            a->in0[j] = std::max(0, b0 - pad);
+            a->in1[j] = std::min(L, b1 + pad);
+        }
+        return TD_OK;
+    }
+    const int m = is_decoder ? 1 : 8;
+    const int n = std::max(ceil_div(L, tile_size), 1);
+    a->resize(n);
+    auto cut = [&](int k) { return k == n ? L : m * (int)(((long long)k * L) / ((long long)n * m)); };
+    for (int k = 0; k < n; ++k) {
+        const int b0 = cut(k), b1 = cut(k + 1);
+        a->out0[k] = scale(b0);
+        a->out1[k] = scale(b1);
+        a->in0[k] = b0 - pad;
+        a->in1[k] = b1 + pad;
+    }
+    return TD_OK;
+}
+
+int split_impl(const char* what, int h, int w, int tile_size, int pad, int is_decoder, int wrap, int32_t* in_bboxes, int32_t* out_bboxes,
+               int cap) {
+    if (h <= 0 || w <= 0 || tile_size <= 0 || pad < 0 || (wrap & ~3) != 0) { td_set_error("%s: bad arguments", what); return TD_ERR_INVALID_ARG; }
+    VaeAxis ax, ay;
+    int st = vae_axis(w, tile_size, pad, is_decoder, (wrap & 1) != 0, &ax);
+    if (st != TD_OK) return st;
+    st = vae_axis(h, tile_size, pad, is_decoder, (wrap & 2) != 0, &ay);
+    if (st != TD_OK) return st;
+    const long long T = (long long)ay.n * ax.n;
     if (in_bboxes == nullptr || out_bboxes == nullptr) return (int)T;
-    if (T > cap) { td_set_error("td_vae_split_tiles: %lld tiles exceed capacity %d", T, cap); return TD_ERR_CAPACITY; }
-    auto floordiv8 = [](int v) { return (int)std::floor((double)v / 8.0); };
+    if (T > cap) { td_set_error("%s: %lld tiles exceed capacity %d", what, T, cap); return TD_ERR_CAPACITY; }
     int32_t* ib = in_bboxes;
     int32_t* ob = out_bboxes;
-    for (int i = 0; i < n_h; ++i)
-        for (int j = 0; j < n_w; ++j) {
-            const int b[4] = {pad + j * real_w, std::min(pad + (j + 1) * real_w, w), pad + i * real_h, std::min(pad + (i + 1) * real_h, h)};
-            int o[4] = {b[0] > pad ? b[0] : 0, b[1] < w - pad ? b[1] : w, b[2] > pad ? b[2] : 0, b[3] < h - pad ? b[3] : h};
-            for (int k = 0; k < 4; ++k) *ob++ = is_decoder ? o[k] * 8 : floordiv8(o[k]);
-            *ib++ = std::max(0, b[0] - pad); *ib++ = std::min(w, b[1] + pad);
-            *ib++ = std::max(0, b[2] - pad); *ib++ = std::min(h, b[3] + pad);
+    for (int i = 0; i < ay.n; ++i)
+        for (int j = 0; j < ax.n; ++j) {
+            *ob++ = ax.out0[j]; *ob++ = ax.out1[j]; *ob++ = ay.out0[i]; *ob++ = ay.out1[i];
+            *ib++ = ax.in0[j]; *ib++ = ax.in1[j]; *ib++ = ay.in0[i]; *ib++ = ay.in1[i];
         }
     return (int)T;
+}
+
+}  // namespace
+
+extern "C" int td_vae_split_tiles(int h, int w, int tile_size, int pad, int is_decoder, int32_t* in_bboxes, int32_t* out_bboxes,
+                                  int cap) {  // tilevae.py:405-462; bbox order [x1, x2, y1, y2]
+    return split_impl("td_vae_split_tiles", h, w, tile_size, pad, is_decoder, 0, in_bboxes, out_bboxes, cap);
+}
+
+extern "C" int td_vae_split_tiles_wrap(int h, int w, int tile_size, int pad, int is_decoder, int wrap, int32_t* in_bboxes,
+                                       int32_t* out_bboxes, int cap) {
+    return split_impl("td_vae_split_tiles_wrap", h, w, tile_size, pad, is_decoder, wrap, in_bboxes, out_bboxes, cap);
 }

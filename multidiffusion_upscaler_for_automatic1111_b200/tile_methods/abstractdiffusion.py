@@ -219,10 +219,19 @@ class AbstractDiffusion:
 
     # ------------------------------------------------------------ grid tiling
     @grid_bbox
-    def init_grid_bbox(self, tile_w: int, tile_h: int, overlap: int, tile_bs: int):
-        """abstractdiffusion.py:172-186, bookkeeping done by td_grid_init (C++, bit-exact)."""
+    def init_grid_bbox(self, tile_w: int, tile_h: int, overlap: int, tile_bs: int, wrap_x: bool = False, wrap_y: bool = False):
+        """abstractdiffusion.py:172-186, bookkeeping done by td_grid_init (C++, bit-exact).
+
+        wrap_x / wrap_y make the canvas periodic on that axis (seamless output: panoramas that close on themselves,
+        repeating textures).  The tiles are then spaced evenly around the circle and the last ones run past the edge
+        and continue at 0 (td_grid_init_wrap), so the blend mixes both sides of the seam.  On a wrapped axis a grid
+        BBox may therefore end past the canvas (x + w > W): its `slicer` is not a crop of the latent, every grid-tile
+        crop goes through the engine, which reads the plan's wrap bits."""
+        wrap = (engine.WRAP_X if wrap_x else 0) | (engine.WRAP_Y if wrap_y else 0)
+        if wrap and self.method == "DemoFusion":
+            raise NotImplementedError("DemoFusion builds its own window lists: seamless tiling (wrap_x / wrap_y) is not supported")
         self.enable_grid_bbox = True
-        g = engine.make_grid(self.w, self.h, tile_w, tile_h, overlap, tile_bs)
+        g = engine.make_grid(self.w, self.h, tile_w, tile_h, overlap, tile_bs, wrap=wrap)
         self._grid = g
         self.tile_w, self.tile_h = int(g.tile_w), int(g.tile_h)
         tile_weights = self.get_tile_weights()
@@ -264,6 +273,9 @@ class AbstractDiffusion:
         from .. import parallel
         if self._grid is None and not self.enable_custom_bbox:
             raise RuntimeError("init_tile_shard() must follow init_grid_bbox() or init_custom_bbox()")
+        if self._grid is not None and engine.grid_wrap(self._grid):
+            raise NotImplementedError("init_tile_shard() does not support a wrapped grid (wrap_x / wrap_y): the strip plan and the "
+                                      "peer-memory blends assume a bounded canvas")
         if mode is None:
             mode = "strip" if (fused and self.method == "MultiDiffusion" and self._grid is not None) else "replicate"
         if mode not in ("strip", "replicate"):
@@ -735,7 +747,13 @@ class AbstractDiffusion:
         dev = host.device()
         if t.device != dev:
             t = t.to(dev)
-        if max(self._grid.H, self._grid.W) * scale >= 32768 or tuple(t.shape[2:]) != (self._grid.H * scale, self._grid.W * scale) or not t.is_cuda:
+        exact = tuple(t.shape[2:]) == (self._grid.H * scale, self._grid.W * scale)
+        too_large = max(self._grid.H, self._grid.W) * scale >= 32768
+        if engine.grid_wrap(self._grid) and (too_large or not exact):
+            raise ValueError(f"a wrapped grid crops side inputs modulo the canvas, in the scatter kernel: the input's size "
+                             f"{tuple(t.shape[2:])} must be the canvas times {scale}, {(self._grid.H * scale, self._grid.W * scale)}, "
+                             "and below 32768")
+        if too_large or not exact or not t.is_cuda:
             # beyond the kernels' 16-bit tile origins (a 32k-pixel hint), or a hint whose size is not exactly the scaled
             # canvas (p.width not a multiple of 8, hints resized by the extension: the reference's slicing tolerates
             # both, abstractdiffusion.py:494-503): plain slicing, same tile order

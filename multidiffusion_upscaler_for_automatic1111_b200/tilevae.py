@@ -407,6 +407,10 @@ class VAEHook:
         # pinned host memory.  None: the free device memory at the start of the call, less the working reserve.
         self.max_resident_bytes: Optional[int] = None
         self.last_park_stats: Optional[dict] = None    # what the last call parked (see _run_tiles)
+        # Seamless tiling: the latent / image is periodic along x (y).  The tiles are then cut around the circle and read
+        # their halo from the opposite edge, so a wrapped decode of a seamless latent has no seam (td_vae_split_tiles_wrap).
+        self.wrap_x: bool = False
+        self.wrap_y: bool = False
         self._program = None
         self._shard_group = None
         self._shard_world = 1
@@ -427,7 +431,7 @@ class VAEHook:
             if self.to_gpu:
                 self.net = self.net.to(host.device())
             B, C, H, W = x.shape
-            if max(H, W) <= self.pad * 2 + self.tile_size:
+            if max(H, W) <= self.pad * 2 + self.tile_size and not self._wrap():   # a wrapped seam always gets its halo
                 if self.verbose:
                     print("[Tiled VAE]: the input size is tiny and unnecessary to tile.")
                 return self.net.original_forward(x)
@@ -438,14 +442,20 @@ class VAEHook:
     def get_best_tile_size(self, lowerbound, upperbound):
         return lib.td_vae_best_tile_size(int(lowerbound), int(upperbound))
 
+    def _wrap(self) -> int:
+        return (1 if self.wrap_x else 0) | (2 if self.wrap_y else 0)
+
     def split_tiles(self, h, w):
-        """tilevae.py:405-462 -> (tile_input_bboxes, tile_output_bboxes), each [x1, x2, y1, y2]."""
-        n = check(lib.td_vae_split_tiles(int(h), int(w), int(self.tile_size), int(self.pad), int(self.is_decoder), None, None, 0))
+        """tilevae.py:405-462 -> (tile_input_bboxes, tile_output_bboxes), each [x1, x2, y1, y2].  On a wrapped axis the
+        input bboxes are in unwrapped coordinates (td_vae_split_tiles_wrap)."""
+        wrap = self._wrap()
+        args = (int(h), int(w), int(self.tile_size), int(self.pad), int(self.is_decoder))
+        split = (lambda *a: lib.td_vae_split_tiles_wrap(*args, wrap, *a)) if wrap else (lambda *a: lib.td_vae_split_tiles(*args, *a))
+        n = check(split(None, None, 0))
         ib = np.empty((n, 4), dtype=np.int32)
         ob = np.empty((n, 4), dtype=np.int32)
         p = ctypes.POINTER(ctypes.c_int32)
-        check(lib.td_vae_split_tiles(int(h), int(w), int(self.tile_size), int(self.pad), int(self.is_decoder),
-                                     ib.ctypes.data_as(p), ob.ctypes.data_as(p), n))
+        check(split(ib.ctypes.data_as(p), ob.ctypes.data_as(p), n))
         return ib.tolist(), ob.tolist()
 
     def _cheap_fallback(self, z, device, dtype):
@@ -542,7 +552,7 @@ class VAEHook:
                         pk.resume(ex, i, st, [j for j in order[k + 1:] if states[j] is not None])
                     if st.act is None:
                         b = in_bboxes[i]
-                        st.act = backend.load(z[:, :, b[2]:b[3], b[0]:b[1]])
+                        st.act = backend.load_wrap(z, b) if self._wrap() else backend.load(z[:, :, b[2]:b[3], b[0]:b[1]])
                     stop = ex.run(st)
                     if stop is None:
                         backend.paste(st.act, result, in_bboxes[i], out_bboxes[i], self.is_decoder)

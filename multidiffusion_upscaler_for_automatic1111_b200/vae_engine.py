@@ -296,6 +296,17 @@ def _f32(t: Optional[torch.Tensor], device) -> Optional[torch.Tensor]:
     return None if t is None else t.detach().to(device=device, dtype=torch.float32).contiguous()
 
 
+def _periodic_pieces(lo: int, hi: int, L: int):
+    """[lo, hi) in unwrapped coordinates as (offset in the span, start in [0, L), length) pieces that stay inside one period."""
+    out, p = [], lo
+    while p < hi:
+        s = p % L
+        n = min(hi - p, L - s)
+        out.append((p - lo, s, n))
+        p += n
+    return out
+
+
 class ModuleBackend:
     """NCHW activations; dense ops through the host application's modules, GroupNorm through csrc/td_vae.cu."""
     name = "modules"
@@ -308,6 +319,18 @@ class ModuleBackend:
         from .tilevae import copy_region
         t = torch.empty(z_view.shape, dtype=self.dtype, device=self.device)
         copy_region(z_view, t)
+        return t
+
+    def load_wrap(self, z: torch.Tensor, bbox) -> torch.Tensor:
+        """Tile [x1, x2) x [y1, y2) of the periodic canvas z, bounds in unwrapped coordinates: one td_copy_region per piece
+        of the tile that lies in one period (four when the tile straddles both seams)."""
+        from .tilevae import copy_region
+        x1, x2, y1, y2 = (int(v) for v in bbox)
+        H, W = z.shape[2], z.shape[3]
+        t = torch.empty((z.shape[0], z.shape[1], y2 - y1, x2 - x1), dtype=self.dtype, device=self.device)
+        for ty0, sy0, ny in _periodic_pieces(y1, y2, H):
+            for tx0, sx0, nx in _periodic_pieces(x1, x2, W):
+                copy_region(z[:, :, sy0:sy0 + ny, sx0:sx0 + nx], t[:, :, ty0:ty0 + ny, tx0:tx0 + nx])
         return t
 
     def pixels(self, a: torch.Tensor) -> int:
@@ -428,6 +451,12 @@ class TensorCoreBackend:
     # ---- ops --------------------------------------------------------------------------------------------------
     def load(self, z_view: torch.Tensor) -> torch.Tensor:
         return ops.nchw_to_nhwc(z_view.to(self.dtype) if z_view.dtype != self.dtype else z_view, ops.round_up(z_view.shape[1], 64))
+
+    def load_wrap(self, z: torch.Tensor, bbox) -> torch.Tensor:
+        """Tile [x1, x2) x [y1, y2) of the periodic canvas z (bounds in unwrapped coordinates): one modular gather with the
+        layout change and channel padding of `load`."""
+        z = z.to(self.dtype) if z.dtype != self.dtype else z
+        return ops.nchw_to_nhwc_wrap(z.contiguous(), bbox, ops.round_up(z.shape[1], 64))
 
     def pixels(self, a) -> int:
         return a.shape[1] * a.shape[2]

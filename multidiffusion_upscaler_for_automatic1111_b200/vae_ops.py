@@ -181,6 +181,20 @@ def nchw_to_nhwc(x: torch.Tensor, cpad: int) -> torch.Tensor:
     return y
 
 
+def nchw_to_nhwc_wrap(z: torch.Tensor, bbox, cpad: int) -> torch.Tensor:
+    """Tile [x1, x2) x [y1, y2) of a periodic canvas z [N, C, H, W] (contiguous), bounds in unwrapped coordinates (they may
+    be negative or pass the canvas) -> contiguous [N, y2 - y1, x2 - x1, cpad], channels zero-padded."""
+    _cuda(z, "z")
+    N, C, H, W = z.shape
+    assert z.is_contiguous()
+    x1, x2, y1, y2 = (int(v) for v in bbox)
+    y = torch.empty((N, y2 - y1, x2 - x1, cpad), dtype=z.dtype, device=z.device)
+    with torch.cuda.device(z.device):
+        check(lib.td_nchw_to_nhwc_wrap(z.data_ptr(), y.data_ptr(), N, C, y2 - y1, x2 - x1, y1, x1, H, W, z.stride(0), z.stride(1), z.stride(2),
+                                       cpad, dtype_code(z.dtype), current_stream_ptr(z.device)))
+    return y
+
+
 def nhwc_to_nchw_region(x: torch.Tensor, dst: torch.Tensor, channels: int) -> None:
     """dst[n, c, i, j] = x[n, i, j, c] for c < channels; x: NHWC view [N, rows, cols, >=channels] (unit channel stride),
     dst: NCHW view [N, channels, rows, cols] (unit inner stride)."""
