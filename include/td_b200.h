@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define TD_ABI_VERSION 9
+#define TD_ABI_VERSION 10
 
 typedef enum td_status {
     TD_OK = 0,
@@ -51,10 +51,6 @@ typedef enum td_dtype { TD_F16 = 0, TD_BF16 = 1, TD_F32 = 2 } td_dtype;
 #define TD_FLAG_ROWS 0x400u      /* row-block form (csrc/td_rows.cu: one persistent CTA per SM, bulk-copy staging), bit-identical:
                                     the scatter's default; opt-in for the blends, whose defaults stay many small co-resident
                                     CTAs (DESIGN.md section 4) */
-#define TD_FLAG_WRAP_X 0x800u    /* scatter / blends: the canvas is periodic in x (seamless tiling, see td_grid_init_wrap):
-                                    a tile column may run past W and continue at column 0; csrc/td_wrap.cu */
-#define TD_FLAG_WRAP_Y 0x1000u   /* the same in y.  Either bit selects the wrap kernels; the opt-in forms (ROWS, STRIP, TMA,
-                                    PIPELINE), the peer blend and the row-strip blend return TD_ERR_UNSUPPORTED with it */
 
 #define TD_MAX_GRID_DIM 256   /* max tile rows / cols of a grid plan            */
 #define TD_MAX_BATCH_PTRS 128 /* max UNet output batch tensors per blend launch */
@@ -97,7 +93,10 @@ int td_custom_bbox_rect(double x, double y, double w, double h, int canvas_w, in
 
 /* Grid plan = what init_grid_bbox leaves on the delegate
  * (tile_methods/abstractdiffusion.py:172-186): clamped tile size and overlap,
- * separable tile origins, tile count and re-balanced tile batch size. */
+ * separable tile origins, tile count and re-balanced tile batch size, and the
+ * axes on which the canvas is periodic (seamless tiling). */
+#define TD_WRAP_X 1u /* td_grid.wrap: the canvas is periodic in x */
+#define TD_WRAP_Y 2u /* td_grid.wrap: the canvas is periodic in y */
 typedef struct td_grid {
     int32_t H, W;           /* latent canvas, abstractdiffusion.py:25-26           */
     int32_t tile_h, tile_w; /* min(tile, canvas), :176-177                         */
@@ -106,29 +105,26 @@ typedef struct td_grid {
     int32_t num_tiles;      /* rows*cols                                           */
     int32_t num_batches;    /* ceil(T / tile_bs), :184                             */
     int32_t tile_bs;        /* ceil(T / num_batches), :185                         */
+    int32_t wrap;           /* TD_WRAP_X | TD_WRAP_Y: periodic axes (new)          */
     int32_t ys[TD_MAX_GRID_DIM]; /* tile-row origins, utils.py:169                 */
     int32_t xs[TD_MAX_GRID_DIM]; /* tile-col origins, utils.py:171                 */
 } td_grid;
 
-/* init_grid_bbox -- abstractdiffusion.py:172-186.  w, h are LATENT sizes. */
-int td_grid_init(td_grid* g, int w, int h, int tile_w, int tile_h, int overlap, int tile_bs);
+/* init_grid_bbox -- abstractdiffusion.py:172-186.  w, h are LATENT sizes.  Returns T or a td_status.
+ * `wrap` (TD_WRAP_X | TD_WRAP_Y, stored in g->wrap) tiles those axes as a circle -- seamless tiling, new: the reference
+ * has no periodic plan.  A wrapped axis of length L with (clamped) tile t has one tile at 0 when t == L, else
+ * n = ceil(L / (t - overlap)) tiles at floor(k * (L / n)) (float64): origins lie in [0, L), a tile may run past L and
+ * continue at 0, and cyclic neighbours -- the last and the first included -- overlap by at least `overlap`.  A bounded
+ * axis, the clamps, the tile order, num_batches and tile_bs follow the reference. */
+int td_grid_init(td_grid* g, int w, int h, int tile_w, int tile_h, int overlap, int tile_bs, int wrap);
 
 /* Weight canvas of split_bboxes -- utils.py:167,175: fp32 [H*W] zeros, then
  * `+= init_weight` per tile in list order.  tile_weights NULL => 1.0
  * (abstractdiffusion.py:188-190), else fp32 [tile_h*tile_w]
- * (mixtureofdiffusers.py:38-43).  HOST arrays. */
+ * (mixtureofdiffusers.py:38-43).  HOST arrays.  On an axis whose g->wrap bit is set
+ * the placement is modular: tile (r, c) adds at ((ys[r]+v) mod H, (xs[c]+u) mod W).
+ * Rejects (TD_ERR_INVALID_ARG) a tile that leaves the canvas on a bounded axis. */
 int td_grid_weights(const td_grid* g, const float* tile_weights, float* out_weights);
-
-/* Seamless tiling (new: the reference has no periodic plan).  `wrap`: bit 0 = x, bit 1 = y.  A wrapped axis of
- * length L with (clamped) tile t has one tile at 0 when t == L, else n = ceil(L / (t - overlap)) tiles at
- * floor(k * (L / n)) (float64): origins lie in [0, L), a tile may run past L and continue at 0, and cyclic
- * neighbours -- the last and the first included -- overlap by at least `overlap`.  A non-wrapped axis, the clamps,
- * the tile order, num_batches and tile_bs follow td_grid_init; wrap = 0 IS td_grid_init.  Returns T or a td_status. */
-int td_grid_init_wrap(td_grid* g, int w, int h, int tile_w, int tile_h, int overlap, int tile_bs, int wrap);
-
-/* td_grid_weights with modular placement: tile (r, c) adds its weights at ((ys[r]+v) mod H, (xs[c]+u) mod W), in
- * list order.  Rejects (TD_ERR_INVALID_ARG) a tile that leaves the canvas on an axis whose wrap bit is clear. */
-int td_grid_weights_wrap(const td_grid* g, int wrap, const float* tile_weights, float* out_weights);
 
 /* rescale_factor = 1 / weights -- mixtureofdiffusers.py:32 (fp32 IEEE divide). */
 int td_rescale_factor(const float* weights, float* out, int64_t n);
@@ -145,7 +141,7 @@ int td_rescale_factor(const float* weights, float* out, int64_t n);
 int td_scatter_tiles(const td_grid* g, const void* x, void* tiles, int N, int C, int dtype,
                      int tile_begin, int tile_end, uint32_t flags, void* stream);
 /* Every grid entry below (and td_scatter_tiles) rejects with TD_ERR_INVALID_ARG a plan whose tiles leave the canvas
- * (origin < 0, origin + tile > extent) on an axis whose TD_FLAG_WRAP_* bit is clear.  With the bit set, coverage on
+ * (origin < 0, origin + tile > extent) on an axis whose g->wrap bit is clear.  With the bit set, coverage on
  * that axis is modular: canvas pixel x is covered by tile column c when (x - xs[c]) mod W < tile_w, and the tile
  * element is taken at that residue (the same in y).  The arithmetic -- tile order, per-add rounding, the MultiDiffusion
  * normalisation and the Mixture of Diffusers products -- is unchanged. */
@@ -187,16 +183,14 @@ int td_vae_best_tile_size(int lowerbound, int upperbound);
 /* split_tiles -- tilevae.py:405-462.  Writes T input and T output bboxes as int32
  * [x1, x2, y1, y2] quadruples (input bbox already expanded by `pad` and clipped;
  * output bbox snapped to the borders and scaled x8 (decoder) or //8 (encoder)).
- * Pass NULL arrays to query T.  Returns T or a td_status. */
-int td_vae_split_tiles(int h, int w, int tile_size, int pad, int is_decoder,
-                       int32_t* in_bboxes, int32_t* out_bboxes, int cap);
-/* Seamless tiling (new): td_vae_split_tiles with the axes whose `wrap` bit is set (bit 0 = x, bit 1 = y) split as a circle.
+ * Pass NULL arrays to query T.  Returns T or a td_status.
+ * `wrap` (TD_WRAP_X | TD_WRAP_Y; 0 = the reference's split) splits those axes as a circle -- seamless tiling, new.
  * A wrapped axis of length L gets n = max(ceil(L / tile_size), 1) tiles cut at b_k = m * floor(k * L / (n * m)), b_n = L
  * (m = 8 for the encoder, 1 for the decoder); output bbox [b_k, b_{k+1}) (x8 decoder, /8 encoder), input bbox
  * [b_k - pad, b_{k+1} + pad) in UNwrapped coordinates: it may be negative or exceed L, the tile load reads it modulo L
- * (td_nchw_to_nhwc_wrap, or td_copy_region per piece).  A non-wrapped axis is split exactly as td_vae_split_tiles does. */
-int td_vae_split_tiles_wrap(int h, int w, int tile_size, int pad, int is_decoder, int wrap,
-                            int32_t* in_bboxes, int32_t* out_bboxes, int cap);
+ * (td_nchw_to_nhwc_wrap, or td_copy_region per piece). */
+int td_vae_split_tiles(int h, int w, int tile_size, int pad, int is_decoder, int wrap,
+                       int32_t* in_bboxes, int32_t* out_bboxes, int cap);
 
 /* Statistics of `nseg` contiguous segments of `seg_len` elements each, ONE read:
  * get_var_mean -- tilevae.py:207-215 with nseg = B*32, seg_len = (C/32)*H*W (the

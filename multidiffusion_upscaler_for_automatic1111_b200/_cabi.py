@@ -28,13 +28,12 @@ TD_FLAG_ONE_PLANE = 64
 TD_FLAG_STRIP = 128
 TD_FLAG_DBG_NO_TILES = 0x100
 TD_FLAG_ROWS = 0x400
-TD_FLAG_WRAP_X = 0x800
-TD_FLAG_WRAP_Y = 0x1000
+TD_WRAP_X, TD_WRAP_Y = 1, 2
 TD_MAX_GRID_DIM = 256
 TD_MAX_BATCH_PTRS = 128
 TD_MAX_PEERS = 16
 TD_IPC_HANDLE_BYTES = 64
-ABI_VERSION = 9
+ABI_VERSION = 10
 
 DTYPE_CODE = {torch.float16: TD_F16, torch.bfloat16: TD_BF16, torch.float32: TD_F32}
 
@@ -53,6 +52,7 @@ class TdGrid(ctypes.Structure):
         ("overlap", c_int32),
         ("rows", c_int32), ("cols", c_int32),
         ("num_tiles", c_int32), ("num_batches", c_int32), ("tile_bs", c_int32),
+        ("wrap", c_int32),
         ("ys", c_int32 * TD_MAX_GRID_DIM),
         ("xs", c_int32 * TD_MAX_GRID_DIM),
     ]
@@ -99,18 +99,15 @@ _SIGNATURES = {
     "td_gaussian_weights": (c_int, [c_int, c_int, POINTER(c_float)]),
     "td_feather_mask": (c_int, [c_int, c_int, c_double, POINTER(c_float)]),
     "td_custom_bbox_rect": (c_int, [c_double, c_double, c_double, c_double, c_int, c_int, POINTER(c_int32)]),
-    "td_grid_init": (c_int, [POINTER(TdGrid), c_int, c_int, c_int, c_int, c_int, c_int]),
+    "td_grid_init": (c_int, [POINTER(TdGrid), c_int, c_int, c_int, c_int, c_int, c_int, c_int]),
     "td_grid_weights": (c_int, [POINTER(TdGrid), POINTER(c_float), POINTER(c_float)]),
-    "td_grid_init_wrap": (c_int, [POINTER(TdGrid), c_int, c_int, c_int, c_int, c_int, c_int, c_int]),
-    "td_grid_weights_wrap": (c_int, [POINTER(TdGrid), c_int, POINTER(c_float), POINTER(c_float)]),
     "td_rescale_factor": (c_int, [POINTER(c_float), POINTER(c_float), c_int64]),
     "td_scatter_tiles": (c_int, [POINTER(TdGrid), c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_uint32, c_void_p]),
     "td_blend_multidiffusion": (c_int, [POINTER(TdGrid), POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_int,
                                         c_void_p, c_void_p, c_void_p, c_void_p, c_uint32, c_void_p]),
     "td_debug_check_fast_div": (c_int, [c_int, c_int, c_void_p, c_void_p]),
     "td_vae_best_tile_size": (c_int, [c_int, c_int]),
-    "td_vae_split_tiles": (c_int, [c_int, c_int, c_int, c_int, c_int, POINTER(c_int32), POINTER(c_int32), c_int]),
-    "td_vae_split_tiles_wrap": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_int32), POINTER(c_int32), c_int]),
+    "td_vae_split_tiles": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_int32), POINTER(c_int32), c_int]),
     "td_nchw_to_nhwc_wrap": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int64, c_int64, c_int64,
                                      c_int, c_int, c_void_p]),
     "td_gn_stats_workspace_bytes": (c_int64, [c_int64, c_int64, c_int]),

@@ -1091,17 +1091,16 @@ blend_grid_generic_kernel(const __grid_constant__ BlendParams p, const float* __
 // magic = ceil(2^32 / d) for fastdiv(); 0 encodes d == 1
 unsigned magic_u16(unsigned d) { return d <= 1 ? 0u : (unsigned)(((1ull << 32) + d - 1) / d); }
 
-constexpr uint32_t kWrapBits = TD_FLAG_WRAP_X | TD_FLAG_WRAP_Y;
 constexpr uint32_t kOptInForms = TD_FLAG_ROWS | TD_FLAG_STRIP | TD_FLAG_TMA | TD_FLAG_PIPELINE;
 
-// `wrap`: the TD_FLAG_WRAP_* bits of the call.  On an axis whose bit is clear every tile must lie inside the canvas
-// (the kernels of this file index the canvas without bounds checks); on a periodic axis an origin lies in [0, extent).
-int fill_geom(const td_grid* g, int N, int C, GeomParams* o, uint32_t wrap = 0) {
+// On an axis whose g->wrap bit is clear every tile must lie inside the canvas (the kernels of this file index the canvas
+// without bounds checks); on a periodic axis an origin lies in [0, extent).
+int fill_geom(const td_grid* g, int N, int C, GeomParams* o) {
     if (g == nullptr) { td_set_error("null grid"); return TD_ERR_INVALID_ARG; }
     if (N <= 0 || C <= 0) { td_set_error("N and C must be positive (N=%d C=%d)", N, C); return TD_ERR_INVALID_ARG; }
     if (g->rows <= 0 || g->cols <= 0 || g->rows > TD_MAX_GRID_DIM || g->cols > TD_MAX_GRID_DIM ||
-        g->num_tiles != g->rows * g->cols) {
-        td_set_error("grid not initialised (rows=%d cols=%d)", g->rows, g->cols);
+        g->num_tiles != g->rows * g->cols || (g->wrap & ~(int)(TD_WRAP_X | TD_WRAP_Y)) != 0) {
+        td_set_error("grid not initialised (rows=%d cols=%d wrap=%d)", g->rows, g->cols, g->wrap);
         return TD_ERR_INVALID_ARG;
     }
     if (g->H >= 32768 || g->W >= 32768) { td_set_error("canvas %dx%d too large", g->H, g->W); return TD_ERR_UNSUPPORTED; }
@@ -1110,15 +1109,13 @@ int fill_geom(const td_grid* g, int N, int C, GeomParams* o, uint32_t wrap = 0) 
         return TD_ERR_INVALID_ARG;
     }
     for (int c = 0; c < g->cols; ++c)
-        if (g->xs[c] < 0 || g->xs[c] >= g->W || (!(wrap & TD_FLAG_WRAP_X) && g->xs[c] + g->tile_w > g->W)) {
-            td_set_error("tile column %d (x=%d, w=%d) leaves the %d-wide canvas%s", c, g->xs[c], g->tile_w, g->W,
-                         (wrap & TD_FLAG_WRAP_X) ? "" : " (a periodic plan needs TD_FLAG_WRAP_X)");
+        if (g->xs[c] < 0 || g->xs[c] >= g->W || (!(g->wrap & TD_WRAP_X) && g->xs[c] + g->tile_w > g->W)) {
+            td_set_error("tile column %d (x=%d, w=%d) leaves the %d-wide canvas", c, g->xs[c], g->tile_w, g->W);
             return TD_ERR_INVALID_ARG;
         }
     for (int r = 0; r < g->rows; ++r)
-        if (g->ys[r] < 0 || g->ys[r] >= g->H || (!(wrap & TD_FLAG_WRAP_Y) && g->ys[r] + g->tile_h > g->H)) {
-            td_set_error("tile row %d (y=%d, h=%d) leaves the %d-high canvas%s", r, g->ys[r], g->tile_h, g->H,
-                         (wrap & TD_FLAG_WRAP_Y) ? "" : " (a periodic plan needs TD_FLAG_WRAP_Y)");
+        if (g->ys[r] < 0 || g->ys[r] >= g->H || (!(g->wrap & TD_WRAP_Y) && g->ys[r] + g->tile_h > g->H)) {
+            td_set_error("tile row %d (y=%d, h=%d) leaves the %d-high canvas", r, g->ys[r], g->tile_h, g->H);
             return TD_ERR_INVALID_ARG;
         }
     o->H = g->H; o->W = g->W; o->th = g->tile_h; o->tw = g->tile_w;
@@ -1454,8 +1451,8 @@ int dispatch_generic(int tile_dtype, int acc_dtype, const BlendParams& bp, const
 }
 
 int fill_blend(const td_grid* g, const void* const* batch_ptrs, int num_batches, int tile_bs, int N, int C, int tile_dtype,
-               int acc_dtype, BlendParams* bp, uint32_t wrap = 0) {
-    int st = fill_geom(g, N, C, &bp->g, wrap);
+               int acc_dtype, BlendParams* bp) {
+    int st = fill_geom(g, N, C, &bp->g);
     if (st != TD_OK) return st;
     if (td_dtype_size(tile_dtype) == 0 || td_dtype_size(acc_dtype) == 0) { td_set_error("unknown dtype"); return TD_ERR_INVALID_ARG; }
     if (batch_ptrs == nullptr || num_batches <= 0 || tile_bs <= 0) { td_set_error("bad batch pointer table"); return TD_ERR_INVALID_ARG; }
@@ -1481,18 +1478,11 @@ int fill_blend(const td_grid* g, const void* const* batch_ptrs, int num_batches,
     return TD_OK;
 }
 
-// the wrap bits select td_wrap.cu, which has one form: the opt-in forms of this file do not take them
-int refuse_opt_in(uint32_t flags, const char* what) {
-    if ((flags & kWrapBits) && (flags & kOptInForms)) {
-        td_set_error("%s: TD_FLAG_WRAP_X / TD_FLAG_WRAP_Y do not combine with the ROWS / STRIP / TMA / PIPELINE forms", what);
-        return TD_ERR_UNSUPPORTED;
-    }
-    return TD_OK;
-}
-
-int refuse_wrap(uint32_t flags, const char* what) {
-    if (flags & kWrapBits) {
-        td_set_error("%s: no form for a periodic canvas (TD_FLAG_WRAP_X / TD_FLAG_WRAP_Y)", what);
+// A periodic plan runs on td_wrap.cu, which has one form per operation: the opt-in forms of this file (ROWS / STRIP /
+// TMA / PIPELINE), the peer blend and the row-strip blend do not take one.
+int refuse_wrapped(const td_grid* g, const char* what) {
+    if (g->wrap != 0) {
+        td_set_error("%s: no form for a periodic plan (wrap=%d)", what, g->wrap);
         return TD_ERR_UNSUPPORTED;
     }
     return TD_OK;
@@ -1523,9 +1513,9 @@ extern "C" int td_debug_launch_empty(int blocks, int threads, void* stream) {
 extern "C" int td_scatter_tiles(const td_grid* g, const void* x, void* tiles, int N, int C, int dtype, int tile_begin,
                                 int tile_end, uint32_t flags, void* stream) {
     GeomParams gp;
-    int st = fill_geom(g, N, C, &gp, flags & kWrapBits);
+    int st = fill_geom(g, N, C, &gp);
     if (st != TD_OK) return st;
-    if ((st = refuse_opt_in(flags, "td_scatter_tiles")) != TD_OK) return st;
+    if ((flags & kOptInForms) && (st = refuse_wrapped(g, "td_scatter_tiles")) != TD_OK) return st;
     if (x == nullptr || tiles == nullptr) { td_set_error("td_scatter_tiles: null tensor"); return TD_ERR_INVALID_ARG; }
     if (tile_begin < 0 || tile_end < tile_begin || tile_end > g->num_tiles) {
         td_set_error("td_scatter_tiles: tile range [%d,%d) outside [0,%d)", tile_begin, tile_end, g->num_tiles);
@@ -1533,10 +1523,10 @@ extern "C" int td_scatter_tiles(const td_grid* g, const void* x, void* tiles, in
     }
     const int es = td_dtype_size(dtype);
     if (es == 0) { td_set_error("td_scatter_tiles: unknown dtype %d", dtype); return TD_ERR_INVALID_ARG; }
-    if (flags & kWrapBits) return td_wrap_scatter(g, x, tiles, N, C, dtype, tile_begin, tile_end, flags, stream);
     const int vec = 16 / es;
     tl_pdl = !(flags & TD_FLAG_NO_PDL);
     const bool vec_ok = !(flags & TD_FLAG_FORCE_GENERIC) && gp.W % vec == 0 && gp.tw % vec == 0 && aligned16(x) && aligned16(tiles);
+    if (g->wrap) return td_wrap_scatter(g, x, tiles, N, C, dtype, tile_begin, tile_end, vec_ok, tl_pdl, stream);
     cudaStream_t s = (cudaStream_t)stream;
     if (vec_ok && !(flags & TD_FLAG_NO_TMA)) {   // default: row-block form (td_rows.cu); falls through when not applicable
         const int rc = td_rows_try_launch_scatter(g, x, tiles, N, C, dtype, tile_begin, tile_end, (flags & TD_FLAG_NO_PDL) ? 0 : 1, stream);
@@ -1553,16 +1543,17 @@ extern "C" int td_blend_multidiffusion(const td_grid* g, const void* const* batc
     BlendParams bp;
     tl_pdl = !(flags & TD_FLAG_NO_PDL);
     tl_ppc_max = (flags & TD_FLAG_ONE_PLANE) ? 1 : TD_AS_PPC;
-    int st = fill_blend(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, &bp, flags & kWrapBits);
+    int st = fill_blend(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, &bp);
     if (st != TD_OK) return st;
     if (weights == nullptr || x_out == nullptr) { td_set_error("td_blend_multidiffusion: null weights / x_out"); return TD_ERR_INVALID_ARG; }
-    if ((st = refuse_opt_in(flags, "td_blend_multidiffusion")) != TD_OK) return st;
-    if (flags & kWrapBits)
+    if ((flags & kOptInForms) && (st = refuse_wrapped(g, "td_blend_multidiffusion")) != TD_OK) return st;
+    const bool vec_ok = !(flags & TD_FLAG_FORCE_GENERIC) && blend_vec_ok(bp, tile_dtype, acc_dtype, {weights, rcp_weights, x_out, x_buffer});
+    if (g->wrap)
         return td_wrap_blend(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, 0, weights, nullptr, nullptr, x_out, x_buffer,
-                             flags, stream);
+                             vec_ok, tl_pdl, stream);
     bp.g.dbg_no_tiles = (flags & TD_FLAG_DBG_NO_TILES) ? 1 : 0;
     cudaStream_t s = (cudaStream_t)stream;
-    if (!(flags & TD_FLAG_FORCE_GENERIC) && blend_vec_ok(bp, tile_dtype, acc_dtype, {weights, rcp_weights, x_out, x_buffer})) {
+    if (vec_ok) {
         int rc = 1;
         if (flags & TD_FLAG_ROWS) {
             // opt-in: row-block form (td_rows.cu); falls through to the default kernels when not applicable
@@ -1607,10 +1598,9 @@ extern "C" int td_blend_multidiffusion_rows(const td_grid* g, const void* const*
     BlendParams bp;
     tl_pdl = !(flags & TD_FLAG_NO_PDL);
     tl_ppc_max = (flags & TD_FLAG_ONE_PLANE) ? 1 : TD_AS_PPC;
-    int st = refuse_wrap(flags, "td_blend_multidiffusion_rows");
+    int st = fill_blend(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, &bp);
     if (st != TD_OK) return st;
-    st = fill_blend(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, &bp);
-    if (st != TD_OK) return st;
+    if ((st = refuse_wrapped(g, "td_blend_multidiffusion_rows")) != TD_OK) return st;
     if (weights == nullptr || x_out == nullptr) { td_set_error("td_blend_multidiffusion_rows: null weights / x_out"); return TD_ERR_INVALID_ARG; }
     if (row_begin < 0 || row_end > g->H || row_begin > row_end || row_begin % 8 != 0 || (row_end % 8 != 0 && row_end != g->H)) {
         td_set_error("td_blend_multidiffusion_rows: rows [%d,%d) must lie in [0,%d) on multiples of 8", row_begin, row_end, g->H);
@@ -1661,10 +1651,9 @@ extern "C" int td_blend_multidiffusion_peer(const td_grid* g, const void* const*
     BlendParams bp;
     tl_pdl = !(flags & TD_FLAG_NO_PDL);
     tl_ppc_max = (flags & TD_FLAG_ONE_PLANE) ? 1 : TD_AS_PPC;
-    int st = refuse_wrap(flags, "td_blend_multidiffusion_peer");
+    int st = fill_blend(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, &bp);
     if (st != TD_OK) return st;
-    st = fill_blend(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, &bp);
-    if (st != TD_OK) return st;
+    if ((st = refuse_wrapped(g, "td_blend_multidiffusion_peer")) != TD_OK) return st;
     if (weights == nullptr || x_out == nullptr) { td_set_error("td_blend_multidiffusion_peer: null weights / x_out"); return TD_ERR_INVALID_ARG; }
     if (wait_flags == nullptr || wait_value == nullptr || world <= 0 || world > TD_MAX_PEERS) { td_set_error("td_blend_multidiffusion_peer: bad wait table"); return TD_ERR_INVALID_ARG; }
     if (!blend_vec_ok(bp, tile_dtype, acc_dtype, {weights, x_out, x_buffer})) {
@@ -1695,18 +1684,19 @@ extern "C" int td_blend_mixture(const td_grid* g, const void* const* batch_ptrs,
     BlendParams bp;
     tl_pdl = !(flags & TD_FLAG_NO_PDL);
     tl_ppc_max = (flags & TD_FLAG_ONE_PLANE) ? 1 : TD_AS_PPC;
-    int st = fill_blend(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, &bp, flags & kWrapBits);
+    int st = fill_blend(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, &bp);
     if (st != TD_OK) return st;
     if (tile_weights == nullptr || rescale == nullptr || x_buffer == nullptr) {
         td_set_error("td_blend_mixture: null tile_weights / rescale / x_buffer");
         return TD_ERR_INVALID_ARG;
     }
-    if ((st = refuse_opt_in(flags, "td_blend_mixture")) != TD_OK) return st;
-    if (flags & kWrapBits)
+    if ((flags & kOptInForms) && (st = refuse_wrapped(g, "td_blend_mixture")) != TD_OK) return st;
+    const bool vec_ok = !(flags & TD_FLAG_FORCE_GENERIC) && blend_vec_ok(bp, tile_dtype, acc_dtype, {rescale, x_buffer});
+    if (g->wrap)
         return td_wrap_blend(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, 1, nullptr, tile_weights, rescale, nullptr,
-                             x_buffer, flags, stream);
+                             x_buffer, vec_ok, tl_pdl, stream);
     cudaStream_t s = (cudaStream_t)stream;
-    if (!(flags & TD_FLAG_FORCE_GENERIC) && blend_vec_ok(bp, tile_dtype, acc_dtype, {rescale, x_buffer})) {
+    if (vec_ok) {
         if (flags & TD_FLAG_ROWS) {   // opt-in: row-block form (td_rows.cu)
             const int rc = td_rows_try_launch_mod(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, tile_weights, rescale, x_buffer,
                                                   (flags & TD_FLAG_NO_PDL) ? 0 : 1, stream);

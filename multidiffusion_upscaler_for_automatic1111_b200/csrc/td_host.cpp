@@ -170,8 +170,50 @@ extern "C" int td_custom_bbox_rect(double x, double y, double w, double h, int c
     return 1;
 }
 
-extern "C" int td_grid_init(td_grid* g, int w, int h, int tile_w, int tile_h, int overlap, int tile_bs) {
-    if (g == nullptr || tile_bs <= 0) {
+// ---------------------------------------------------------------------------------------------------------
+// One axis of a tile plan: tile count n and origin stride d.  A bounded axis follows split_bboxes (origins
+// min(int(k * d), L - t)).  A periodic axis of length L is tiled as a circle: tile k starts at floor(k * d),
+// d = L / n with n = ceil(L / (t - overlap)), so the gap between neighbours -- the last and the first
+// included -- is at most ceil(L / n) <= t - overlap, and a tile may run past L, continuing at 0.
+// ---------------------------------------------------------------------------------------------------------
+namespace {
+
+int linear_axis(int L, int t, int ov, int* n, double* d) {
+    if (t == ov) {  // Python: ZeroDivisionError at utils.py:161-162
+        td_set_error("grid_init: overlap %d equals the tile size %d: division by zero", ov, t);
+        return TD_ERR_INVALID_ARG;
+    }
+    axis_split(L, t, ov, n, d);
+    return TD_OK;
+}
+
+int periodic_axis(int L, int t, int ov, int* n, double* d) {
+    if (t == L) {
+        *n = 1;
+        *d = 0.0;
+        return TD_OK;
+    }
+    if (t <= ov) {
+        td_set_error("grid_init: overlap %d leaves no stride on a periodic axis with tile %d", ov, t);
+        return TD_ERR_INVALID_ARG;
+    }
+    *n = ceil_div_py(L, t - ov);
+    *d = (double)L / (double)*n;
+    return TD_OK;
+}
+
+int axis(int L, int t, int ov, bool periodic, int* n, double* d) {
+    return periodic ? periodic_axis(L, t, ov, n, d) : linear_axis(L, t, ov, n, d);
+}
+
+void fill_origins(int n, double d, int L, int t, bool periodic, int32_t* org) {
+    for (int k = 0; k < n; ++k) org[k] = periodic ? (int32_t)std::floor((double)k * d) : origin(k, d, L - t);
+}
+
+}  // namespace
+
+extern "C" int td_grid_init(td_grid* g, int w, int h, int tile_w, int tile_h, int overlap, int tile_bs, int wrap) {
+    if (g == nullptr || tile_bs <= 0 || (wrap & ~(int)(TD_WRAP_X | TD_WRAP_Y)) != 0) {
         td_set_error("grid_init: bad args");
         return TD_ERR_INVALID_ARG;
     }
@@ -181,20 +223,25 @@ extern "C" int td_grid_init(td_grid* g, int w, int h, int tile_w, int tile_h, in
     }
     std::memset(g, 0, sizeof(*g));
     g->W = w; g->H = h;
+    g->wrap = wrap;
     g->tile_w = std::min(tile_w, w);                                     // abstractdiffusion.py:176
     g->tile_h = std::min(tile_h, h);                                     // :177
     g->overlap = std::max(0, std::min(overlap, std::min(tile_w, tile_h) - 4));  // :178 (unclamped tile args)
-    Split s;
-    int st = split_counts(w, h, g->tile_w, g->tile_h, g->overlap, &s);
+    const bool px = (wrap & TD_WRAP_X) != 0, py = (wrap & TD_WRAP_Y) != 0;
+    int cols = 0, rows = 0;
+    double dx = 0.0, dy = 0.0;
+    int st = axis(w, g->tile_w, g->overlap, px, &cols, &dx);           // utils.py:161,163
     if (st != TD_OK) return st;
-    if (s.rows > TD_MAX_GRID_DIM || s.cols > TD_MAX_GRID_DIM) {
-        td_set_error("grid_init: %dx%d tile grid exceeds TD_MAX_GRID_DIM=%d", s.rows, s.cols, TD_MAX_GRID_DIM);
+    st = axis(h, g->tile_h, g->overlap, py, &rows, &dy);               // utils.py:162,164
+    if (st != TD_OK) return st;
+    if (rows > TD_MAX_GRID_DIM || cols > TD_MAX_GRID_DIM) {
+        td_set_error("grid_init: %dx%d tile grid exceeds TD_MAX_GRID_DIM=%d", rows, cols, TD_MAX_GRID_DIM);
         return TD_ERR_UNSUPPORTED;
     }
-    g->rows = s.rows; g->cols = s.cols;
-    for (int r = 0; r < s.rows; ++r) g->ys[r] = origin(r, s.dy, h - g->tile_h);
-    for (int c = 0; c < s.cols; ++c) g->xs[c] = origin(c, s.dx, w - g->tile_w);
-    g->num_tiles = s.rows * s.cols;                                      // :183
+    g->rows = rows; g->cols = cols;
+    fill_origins(rows, dy, h, g->tile_h, py, g->ys);                     // utils.py:169
+    fill_origins(cols, dx, w, g->tile_w, px, g->xs);                     // utils.py:171
+    g->num_tiles = rows * cols;                                          // :183
     if (g->num_tiles == 0) {  // Python: ZeroDivisionError at :185
         td_set_error("grid_init: the split produced no tiles (w=%d h=%d tile=%dx%d overlap=%d)", w, h, g->tile_w, g->tile_h, g->overlap);
         return TD_ERR_INVALID_ARG;
@@ -210,116 +257,15 @@ extern "C" int td_grid_weights(const td_grid* g, const float* tile_weights, floa
         return TD_ERR_INVALID_ARG;
     }
     const int W = g->W, H = g->H, tw = g->tile_w, th = g->tile_h;
-    std::fill(out, out + (size_t)W * H, 0.0f);
-    for (int r = 0; r < g->rows; ++r)
-        for (int c = 0; c < g->cols; ++c) {  // list order: row outer, col inner
-            const int x0 = g->xs[c], y0 = g->ys[r];
-            for (int v = 0; v < th; ++v) {
-                float* o = out + (size_t)(y0 + v) * W + x0;
-                if (tile_weights) {
-                    const float* tw_row = tile_weights + (size_t)v * tw;
-                    for (int u = 0; u < tw; ++u) o[u] = o[u] + tw_row[u];
-                } else {
-                    for (int u = 0; u < tw; ++u) o[u] = o[u] + 1.0f;
-                }
-            }
-        }
-    return TD_OK;
-}
-
-// ---------------------------------------------------------------------------------------------------------
-// Seamless (periodic) tile plans.  A wrapped axis of length L is tiled as a circle: tile k starts at
-// floor(k * L / n) with n = ceil(L / (t - overlap)), so the gap between neighbours -- the last and the first
-// included -- is at most ceil(L / n) <= t - overlap, and a tile may run past L, continuing at 0.
-// ---------------------------------------------------------------------------------------------------------
-namespace {
-
-// the bounded rule of td_grid_init for one axis (the same axis_split / origin)
-int linear_axis(int L, int t, int ov, int* n_out, int32_t* org) {
-    if (t == ov) {
-        td_set_error("grid_init_wrap: overlap %d equals the tile size %d: division by zero", ov, t);
-        return TD_ERR_INVALID_ARG;
-    }
-    int n = 0;
-    double d = 0.0;
-    axis_split(L, t, ov, &n, &d);
-    if (n > TD_MAX_GRID_DIM) {
-        td_set_error("grid_init_wrap: %d tiles on one axis exceed TD_MAX_GRID_DIM=%d", n, TD_MAX_GRID_DIM);
-        return TD_ERR_UNSUPPORTED;
-    }
-    for (int i = 0; i < n; ++i) org[i] = origin(i, d, L - t);
-    *n_out = n;
-    return TD_OK;
-}
-
-int periodic_axis(int L, int t, int ov, int* n_out, int32_t* org) {
-    if (t == L) {
-        org[0] = 0;
-        *n_out = 1;
-        return TD_OK;
-    }
-    if (t <= ov) {
-        td_set_error("grid_init_wrap: overlap %d leaves no stride on a tile of %d", ov, t);
-        return TD_ERR_INVALID_ARG;
-    }
-    const int n = ceil_div_py(L, t - ov);
-    if (n > TD_MAX_GRID_DIM) {
-        td_set_error("grid_init_wrap: %d tiles on one axis exceed TD_MAX_GRID_DIM=%d", n, TD_MAX_GRID_DIM);
-        return TD_ERR_UNSUPPORTED;
-    }
-    const double d = (double)L / (double)n;
-    for (int k = 0; k < n; ++k) org[k] = (int32_t)std::floor((double)k * d);
-    *n_out = n;
-    return TD_OK;
-}
-
-}  // namespace
-
-extern "C" int td_grid_init_wrap(td_grid* g, int w, int h, int tile_w, int tile_h, int overlap, int tile_bs, int wrap) {
-    if (wrap == 0) return td_grid_init(g, w, h, tile_w, tile_h, overlap, tile_bs);
-    if (g == nullptr || tile_bs <= 0 || (wrap & ~3) != 0) {
-        td_set_error("grid_init_wrap: bad args");
-        return TD_ERR_INVALID_ARG;
-    }
-    if (tile_w <= 0 || tile_h <= 0 || w <= 0 || h <= 0) {
-        td_set_error("grid_init_wrap: non-positive size");
-        return TD_ERR_INVALID_ARG;
-    }
-    std::memset(g, 0, sizeof(*g));
-    g->W = w; g->H = h;
-    g->tile_w = std::min(tile_w, w);
-    g->tile_h = std::min(tile_h, h);
-    g->overlap = std::max(0, std::min(overlap, std::min(tile_w, tile_h) - 4));
-    int cols = 0, rows = 0;
-    int st = (wrap & 1) ? periodic_axis(w, g->tile_w, g->overlap, &cols, g->xs) : linear_axis(w, g->tile_w, g->overlap, &cols, g->xs);
-    if (st != TD_OK) return st;
-    st = (wrap & 2) ? periodic_axis(h, g->tile_h, g->overlap, &rows, g->ys) : linear_axis(h, g->tile_h, g->overlap, &rows, g->ys);
-    if (st != TD_OK) return st;
-    g->rows = rows; g->cols = cols;
-    g->num_tiles = rows * cols;
-    if (g->num_tiles == 0) {
-        td_set_error("grid_init_wrap: the split produced no tiles (w=%d h=%d tile=%dx%d overlap=%d)", w, h, g->tile_w, g->tile_h, g->overlap);
-        return TD_ERR_INVALID_ARG;
-    }
-    g->num_batches = ceil_div_py(g->num_tiles, tile_bs);
-    g->tile_bs = ceil_div_py(g->num_tiles, g->num_batches);
-    return g->num_tiles;
-}
-
-extern "C" int td_grid_weights_wrap(const td_grid* g, int wrap, const float* tile_weights, float* out) {
-    if (g == nullptr || out == nullptr || (wrap & ~3) != 0) {
-        td_set_error("grid_weights_wrap: bad args");
-        return TD_ERR_INVALID_ARG;
-    }
-    const int W = g->W, H = g->H, tw = g->tile_w, th = g->tile_h;
+    const bool px = (g->wrap & TD_WRAP_X) != 0, py = (g->wrap & TD_WRAP_Y) != 0;
     for (int c = 0; c < g->cols; ++c)
-        if (g->xs[c] < 0 || g->xs[c] >= W || tw > W || (!(wrap & 1) && g->xs[c] + tw > W)) {
-            td_set_error("grid_weights_wrap: tile column %d (x=%d, w=%d) leaves the %d-wide canvas", c, g->xs[c], tw, W);
+        if (g->xs[c] < 0 || g->xs[c] >= W || tw > W || (!px && g->xs[c] + tw > W)) {
+            td_set_error("grid_weights: tile column %d (x=%d, w=%d) leaves the %d-wide canvas", c, g->xs[c], tw, W);
             return TD_ERR_INVALID_ARG;
         }
     for (int r = 0; r < g->rows; ++r)
-        if (g->ys[r] < 0 || g->ys[r] >= H || th > H || (!(wrap & 2) && g->ys[r] + th > H)) {
-            td_set_error("grid_weights_wrap: tile row %d (y=%d, h=%d) leaves the %d-high canvas", r, g->ys[r], th, H);
+        if (g->ys[r] < 0 || g->ys[r] >= H || th > H || (!py && g->ys[r] + th > H)) {
+            td_set_error("grid_weights: tile row %d (y=%d, h=%d) leaves the %d-high canvas", r, g->ys[r], th, H);
             return TD_ERR_INVALID_ARG;
         }
     std::fill(out, out + (size_t)W * H, 0.0f);
@@ -327,8 +273,7 @@ extern "C" int td_grid_weights_wrap(const td_grid* g, int wrap, const float* til
         for (int c = 0; c < g->cols; ++c) {  // list order: row outer, col inner
             const int x0 = g->xs[c], y0 = g->ys[r];
             for (int v = 0; v < th; ++v) {
-                const int y = (y0 + v) % H;
-                float* o = out + (size_t)y * W;
+                float* o = out + (size_t)((y0 + v) % H) * W;
                 for (int u = 0; u < tw; ++u) {
                     const int x = (x0 + u) % W;
                     o[x] = o[x] + (tile_weights ? tile_weights[(size_t)v * tw + u] : 1.0f);

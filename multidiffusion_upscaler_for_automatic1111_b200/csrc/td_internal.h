@@ -23,10 +23,11 @@ int td_rows_try_launch_mod(const struct td_grid* g, const void* const* batch_ptr
 int td_rows_try_launch_scatter(const struct td_grid* g, const void* x, void* tiles, int N, int C, int dtype, int tile_begin, int tile_end,
                                int pdl, void* stream);
 
-// td_wrap.cu: scatter / blends on a periodic canvas (TD_FLAG_WRAP_X / TD_FLAG_WRAP_Y).  Called by the C-ABI entries of
-// td_diffusion.cu after they validated the grid and the batch table.  mixture: 0 MultiDiffusion, 1 Mixture of Diffusers.
+// td_wrap.cu: scatter / blends on a periodic canvas (g->wrap != 0).  Called by the C-ABI entries of td_diffusion.cu after
+// they validated the grid and the batch table; `vec`: their vector-path test passed (else one element per thread, any
+// width, alignment or dtype pair).  mixture: 0 MultiDiffusion, 1 Mixture of Diffusers.
 int td_wrap_scatter(const struct td_grid* g, const void* x, void* tiles, int N, int C, int dtype, int tile_begin, int tile_end,
-                    uint32_t flags, void* stream);
+                    bool vec, bool pdl, void* stream);
 int td_wrap_blend(const struct td_grid* g, const void* const* batch_ptrs, int num_batches, int tile_bs, int N, int C, int tile_dtype,
                   int acc_dtype, int mixture, const float* weights, const float* tile_weights, const float* rescale, float* x_out,
-                  void* x_buffer, uint32_t flags, void* stream);
+                  void* x_buffer, bool vec, bool pdl, void* stream);

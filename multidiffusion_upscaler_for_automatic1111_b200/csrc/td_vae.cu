@@ -462,17 +462,22 @@ int vae_axis(int L, int tile_size, int pad, int is_decoder, bool periodic, VaeAx
     return TD_OK;
 }
 
-int split_impl(const char* what, int h, int w, int tile_size, int pad, int is_decoder, int wrap, int32_t* in_bboxes, int32_t* out_bboxes,
-               int cap) {
-    if (h <= 0 || w <= 0 || tile_size <= 0 || pad < 0 || (wrap & ~3) != 0) { td_set_error("%s: bad arguments", what); return TD_ERR_INVALID_ARG; }
+}  // namespace
+
+extern "C" int td_vae_split_tiles(int h, int w, int tile_size, int pad, int is_decoder, int wrap, int32_t* in_bboxes,
+                                  int32_t* out_bboxes, int cap) {  // tilevae.py:405-462; bbox order [x1, x2, y1, y2]
+    if (h <= 0 || w <= 0 || tile_size <= 0 || pad < 0 || (wrap & ~(int)(TD_WRAP_X | TD_WRAP_Y)) != 0) {
+        td_set_error("td_vae_split_tiles: bad arguments");
+        return TD_ERR_INVALID_ARG;
+    }
     VaeAxis ax, ay;
-    int st = vae_axis(w, tile_size, pad, is_decoder, (wrap & 1) != 0, &ax);
+    int st = vae_axis(w, tile_size, pad, is_decoder, (wrap & TD_WRAP_X) != 0, &ax);
     if (st != TD_OK) return st;
-    st = vae_axis(h, tile_size, pad, is_decoder, (wrap & 2) != 0, &ay);
+    st = vae_axis(h, tile_size, pad, is_decoder, (wrap & TD_WRAP_Y) != 0, &ay);
     if (st != TD_OK) return st;
     const long long T = (long long)ay.n * ax.n;
     if (in_bboxes == nullptr || out_bboxes == nullptr) return (int)T;
-    if (T > cap) { td_set_error("%s: %lld tiles exceed capacity %d", what, T, cap); return TD_ERR_CAPACITY; }
+    if (T > cap) { td_set_error("td_vae_split_tiles: %lld tiles exceed capacity %d", T, cap); return TD_ERR_CAPACITY; }
     int32_t* ib = in_bboxes;
     int32_t* ob = out_bboxes;
     for (int i = 0; i < ay.n; ++i)
@@ -481,16 +486,4 @@ int split_impl(const char* what, int h, int w, int tile_size, int pad, int is_de
             *ib++ = ax.in0[j]; *ib++ = ax.in1[j]; *ib++ = ay.in0[i]; *ib++ = ay.in1[i];
         }
     return (int)T;
-}
-
-}  // namespace
-
-extern "C" int td_vae_split_tiles(int h, int w, int tile_size, int pad, int is_decoder, int32_t* in_bboxes, int32_t* out_bboxes,
-                                  int cap) {  // tilevae.py:405-462; bbox order [x1, x2, y1, y2]
-    return split_impl("td_vae_split_tiles", h, w, tile_size, pad, is_decoder, 0, in_bboxes, out_bboxes, cap);
-}
-
-extern "C" int td_vae_split_tiles_wrap(int h, int w, int tile_size, int pad, int is_decoder, int wrap, int32_t* in_bboxes,
-                                       int32_t* out_bboxes, int cap) {
-    return split_impl("td_vae_split_tiles_wrap", h, w, tile_size, pad, is_decoder, wrap, in_bboxes, out_bboxes, cap);
 }

@@ -1,5 +1,4 @@
-// Seamless tiling on sm_90a: the scatter and both blends on a canvas that is periodic in x and / or y
-// (TD_FLAG_WRAP_X / TD_FLAG_WRAP_Y, plans from td_grid_init_wrap).
+// Seamless tiling on sm_90a: the scatter and both blends on a canvas that is periodic in x and / or y (td_grid.wrap).
 //
 // The arithmetic is that of td_diffusion.cu -- covering tiles visited in ascending tile index, one rounding through
 // the canvas dtype per add, MultiDiffusion's `weights > 1 ? acc / weights : acc` in fp32, Mixture of Diffusers'
@@ -284,13 +283,11 @@ wrap_blend_generic_kernel(const __grid_constant__ WrapParams p, const float* __r
 // ---------------------------------------------------------------------------
 // Host side
 // ---------------------------------------------------------------------------
-inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
-
-void fill_params(const td_grid* g, int N, int C, uint32_t flags, WrapParams* p) {
+void fill_params(const td_grid* g, int N, int C, WrapParams* p) {
     p->H = g->H; p->W = g->W; p->th = g->tile_h; p->tw = g->tile_w;
     p->rows = g->rows; p->cols = g->cols; p->N = N; p->C = C;
-    p->wrap_x = (flags & TD_FLAG_WRAP_X) ? 1 : 0;
-    p->wrap_y = (flags & TD_FLAG_WRAP_Y) ? 1 : 0;
+    p->wrap_x = (g->wrap & TD_WRAP_X) ? 1 : 0;
+    p->wrap_y = (g->wrap & TD_WRAP_Y) ? 1 : 0;
     // periodic origins are floor(k * L / n): k ~ p * n / L; bounded ones follow split_bboxes' stride
     p->inv_dx = p->wrap_x ? (float)g->cols / (float)g->W
                           : (g->cols > 1 ? (float)(g->cols - 1) / (float)std::max(1, g->W - g->tile_w) : 0.0f);
@@ -387,35 +384,24 @@ int blend_generic_impl(int tile_dtype, int acc_dtype, const WrapParams& p, const
 
 }  // namespace
 
-int td_wrap_scatter(const td_grid* g, const void* x, void* tiles, int N, int C, int dtype, int tile_begin, int tile_end, uint32_t flags,
+int td_wrap_scatter(const td_grid* g, const void* x, void* tiles, int N, int C, int dtype, int tile_begin, int tile_end, bool vec, bool pdl,
                     void* stream) {
     WrapParams p;
-    fill_params(g, N, C, flags, &p);
-    const int es = td_dtype_size(dtype);
-    const int vec = 16 / es;
-    const bool vec_ok = !(flags & TD_FLAG_FORCE_GENERIC) && p.W % vec == 0 && p.tw % vec == 0 && aligned16(x) && aligned16(tiles);
-    const bool pdl = !(flags & TD_FLAG_NO_PDL);
+    fill_params(g, N, C, &p);
     cudaStream_t st = (cudaStream_t)stream;
-    if (es == 2) return scatter_impl<__half>(p, x, tiles, tile_begin, tile_end - tile_begin, vec_ok, pdl, st);   // 16-bit words, opaque
-    return scatter_impl<float>(p, x, tiles, tile_begin, tile_end - tile_begin, vec_ok, pdl, st);
+    if (td_dtype_size(dtype) == 2) return scatter_impl<__half>(p, x, tiles, tile_begin, tile_end - tile_begin, vec, pdl, st);   // 16-bit words, opaque
+    return scatter_impl<float>(p, x, tiles, tile_begin, tile_end - tile_begin, vec, pdl, st);
 }
 
 int td_wrap_blend(const td_grid* g, const void* const* batch_ptrs, int num_batches, int tile_bs, int N, int C, int tile_dtype, int acc_dtype,
                   int mixture, const float* weights, const float* tile_weights, const float* rescale, float* x_out, void* x_buffer,
-                  uint32_t flags, void* stream) {
+                  bool vec, bool pdl, void* stream) {
     WrapParams p;
-    fill_params(g, N, C, flags, &p);
+    fill_params(g, N, C, &p);
     p.tile_bs = tile_bs;
     for (int b = 0; b < num_batches; ++b) p.batch_ptrs[b] = batch_ptrs[b];
-    const bool pdl = !(flags & TD_FLAG_NO_PDL);
     cudaStream_t st = (cudaStream_t)stream;
-    bool vec_ok = !(flags & TD_FLAG_FORCE_GENERIC) && tile_dtype == acc_dtype && p.tile_stride < (1ll << 31);
-    const int vec = 16 / td_dtype_size(tile_dtype);
-    vec_ok = vec_ok && p.W % vec == 0 && p.tw % vec == 0;
-    for (int b = 0; vec_ok && b < num_batches; ++b) vec_ok = aligned16(batch_ptrs[b]);
-    for (const void* q : {(const void*)weights, (const void*)rescale, (const void*)x_out, (const void*)x_buffer})
-        if (q != nullptr && !aligned16(q)) vec_ok = false;
-    if (vec_ok) {
+    if (vec) {
         if (mixture) {
             switch (tile_dtype) {
                 case TD_F16: return blend_vec_impl<__half, MODE_MOD>(p, nullptr, tile_weights, rescale, nullptr, x_buffer, pdl, st);

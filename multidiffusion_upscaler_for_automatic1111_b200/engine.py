@@ -11,34 +11,19 @@ from typing import Optional, Sequence
 import numpy as np
 import torch
 
-from ._cabi import TD_FLAG_WRAP_X, TD_FLAG_WRAP_Y, TdGrid, check, current_stream_ptr, dtype_code, lib
+from ._cabi import TD_WRAP_X, TD_WRAP_Y, TdGrid, check, current_stream_ptr, dtype_code, lib
 
-WRAP_X, WRAP_Y = 1, 2   # `wrap` bits of make_grid: the canvas is periodic in x / in y (seamless tiling)
+WRAP_X, WRAP_Y = TD_WRAP_X, TD_WRAP_Y   # `wrap` bits of make_grid: the canvas is periodic in x / in y (seamless tiling)
 
 
 def make_grid(w: int, h: int, tile_w: int, tile_h: int, overlap: int, tile_bs: int, wrap: int = 0) -> TdGrid:
     """init_grid_bbox bookkeeping (abstractdiffusion.py:172-186) -> td_grid.
 
-    `wrap` (WRAP_X | WRAP_Y) tiles those axes as a circle (td_grid_init_wrap): tiles may run past the canvas edge and
-    continue at 0, so the blend mixes both sides of the seam.  The plan remembers it (`g.wrap`): every wrapper below
-    reads it, callers never pass wrap flags themselves."""
+    `wrap` (WRAP_X | WRAP_Y) tiles those axes as a circle: tiles may run past the canvas edge and continue at 0, so the
+    blend mixes both sides of the seam.  The plan records it (`g.wrap`) and every kernel entry reads it from there."""
     g = TdGrid()
-    if wrap:
-        check(lib.td_grid_init_wrap(ctypes.byref(g), int(w), int(h), int(tile_w), int(tile_h), int(overlap), int(tile_bs), int(wrap)))
-    else:
-        check(lib.td_grid_init(ctypes.byref(g), int(w), int(h), int(tile_w), int(tile_h), int(overlap), int(tile_bs)))
-    g.wrap = int(wrap)
+    check(lib.td_grid_init(ctypes.byref(g), int(w), int(h), int(tile_w), int(tile_h), int(overlap), int(tile_bs), int(wrap)))
     return g
-
-
-def grid_wrap(g: TdGrid) -> int:
-    """The WRAP_X / WRAP_Y bits of a plan (0 for one built without make_grid's `wrap`)."""
-    return int(getattr(g, "wrap", 0))
-
-
-def _wrap_flags(g: TdGrid) -> int:
-    w = grid_wrap(g)
-    return (TD_FLAG_WRAP_X if w & WRAP_X else 0) | (TD_FLAG_WRAP_Y if w & WRAP_Y else 0)
 
 
 def grid_bboxes_xywh(g: TdGrid) -> np.ndarray:
@@ -56,15 +41,13 @@ def grid_bboxes_xywh(g: TdGrid) -> np.ndarray:
 def scaled_grid(g: TdGrid, scale: int) -> TdGrid:
     """The same tile plan in a space `scale` times finer: pixel-space side inputs (ControlNet hints, x8) are cropped
     with the latent tile list multiplied by opt_f (abstractdiffusion.py:499)."""
-    s = TdGrid()
+    s = TdGrid.from_buffer_copy(g)
     s.H, s.W = g.H * scale, g.W * scale
     s.tile_h, s.tile_w, s.overlap = g.tile_h * scale, g.tile_w * scale, g.overlap * scale
-    s.rows, s.cols, s.num_tiles, s.num_batches, s.tile_bs = g.rows, g.cols, g.num_tiles, g.num_batches, g.tile_bs
     for i in range(g.rows):
         s.ys[i] = g.ys[i] * scale
     for i in range(g.cols):
         s.xs[i] = g.xs[i] * scale
-    s.wrap = grid_wrap(g)
     return s
 
 
@@ -77,10 +60,7 @@ def grid_weights(g: TdGrid, tile_weights: Optional[np.ndarray] = None) -> np.nda
         if tile_weights.shape != (g.tile_h, g.tile_w):
             raise ValueError(f"tile_weights shape {tile_weights.shape} != tile {(g.tile_h, g.tile_w)}")
         tw_ptr = tile_weights.ctypes.data_as(ctypes.POINTER(ctypes.c_float))
-    if grid_wrap(g):
-        check(lib.td_grid_weights_wrap(ctypes.byref(g), grid_wrap(g), tw_ptr, out.ctypes.data_as(ctypes.POINTER(ctypes.c_float))))
-    else:
-        check(lib.td_grid_weights(ctypes.byref(g), tw_ptr, out.ctypes.data_as(ctypes.POINTER(ctypes.c_float))))
+    check(lib.td_grid_weights(ctypes.byref(g), tw_ptr, out.ctypes.data_as(ctypes.POINTER(ctypes.c_float))))
     return out
 
 
@@ -112,7 +92,7 @@ def scatter_tiles(g: TdGrid, x: torch.Tensor, out: Optional[torch.Tensor] = None
         out = torch.empty(shape, dtype=x.dtype, device=x.device)
     with torch.cuda.device(x.device):
         check(lib.td_scatter_tiles(ctypes.byref(g), x.data_ptr(), out.data_ptr(), N, C, dtype_code(x.dtype),
-                                   int(tile_begin), int(tile_end), int(flags) | _wrap_flags(g), current_stream_ptr(x.device)))
+                                   int(tile_begin), int(tile_end), int(flags), current_stream_ptr(x.device)))
     return out
 
 
@@ -161,7 +141,7 @@ def blend_multidiffusion(g: TdGrid, batch_outs: Sequence[torch.Tensor], N: int, 
         check(lib.td_blend_multidiffusion(ctypes.byref(g), ptrs, len(keep), int(tile_bs), N, C, dtype_code(tdt),
                                           dtype_code(acc_dtype), weights.data_ptr(),
                                           rcp_weights.data_ptr() if rcp_weights is not None else None, x_out.data_ptr(),
-                                          x_buffer.data_ptr() if x_buffer is not None else None, int(flags) | _wrap_flags(g),
+                                          x_buffer.data_ptr() if x_buffer is not None else None, int(flags),
                                           current_stream_ptr(dev)))
     return x_out
 
@@ -185,7 +165,7 @@ def blend_mixture(g: TdGrid, batch_outs: Sequence[torch.Tensor], N: int, C: int,
     with torch.cuda.device(dev):
         check(lib.td_blend_mixture(ctypes.byref(g), ptrs, len(keep), int(tile_bs), N, C, dtype_code(tdt),
                                    dtype_code(x_buffer.dtype), tile_weights.data_ptr(), rescale.data_ptr(),
-                                   x_buffer.data_ptr(), int(flags) | _wrap_flags(g), current_stream_ptr(dev)))
+                                   x_buffer.data_ptr(), int(flags), current_stream_ptr(dev)))
     return x_buffer
 
 

@@ -224,7 +224,7 @@ class AbstractDiffusion:
 
         wrap_x / wrap_y make the canvas periodic on that axis (seamless output: panoramas that close on themselves,
         repeating textures).  The tiles are then spaced evenly around the circle and the last ones run past the edge
-        and continue at 0 (td_grid_init_wrap), so the blend mixes both sides of the seam.  On a wrapped axis a grid
+        and continue at 0, so the blend mixes both sides of the seam.  On a wrapped axis a grid
         BBox may therefore end past the canvas (x + w > W): its `slicer` is not a crop of the latent, every grid-tile
         crop goes through the engine, which reads the plan's wrap bits."""
         wrap = (engine.WRAP_X if wrap_x else 0) | (engine.WRAP_Y if wrap_y else 0)
@@ -273,7 +273,7 @@ class AbstractDiffusion:
         from .. import parallel
         if self._grid is None and not self.enable_custom_bbox:
             raise RuntimeError("init_tile_shard() must follow init_grid_bbox() or init_custom_bbox()")
-        if self._grid is not None and engine.grid_wrap(self._grid):
+        if self._grid is not None and self._grid.wrap:
             raise NotImplementedError("init_tile_shard() does not support a wrapped grid (wrap_x / wrap_y): the strip plan and the "
                                       "peer-memory blends assume a bounded canvas")
         if mode is None:
@@ -749,7 +749,7 @@ class AbstractDiffusion:
             t = t.to(dev)
         exact = tuple(t.shape[2:]) == (self._grid.H * scale, self._grid.W * scale)
         too_large = max(self._grid.H, self._grid.W) * scale >= 32768
-        if engine.grid_wrap(self._grid) and (too_large or not exact):
+        if self._grid.wrap and (too_large or not exact):
             raise ValueError(f"a wrapped grid crops side inputs modulo the canvas, in the scatter kernel: the input's size "
                              f"{tuple(t.shape[2:])} must be the canvas times {scale}, {(self._grid.H * scale, self._grid.W * scale)}, "
                              "and below 32768")

@@ -408,7 +408,7 @@ class VAEHook:
         self.max_resident_bytes: Optional[int] = None
         self.last_park_stats: Optional[dict] = None    # what the last call parked (see _run_tiles)
         # Seamless tiling: the latent / image is periodic along x (y).  The tiles are then cut around the circle and read
-        # their halo from the opposite edge, so a wrapped decode of a seamless latent has no seam (td_vae_split_tiles_wrap).
+        # their halo from the opposite edge, so a wrapped decode of a seamless latent has no seam (td_vae_split_tiles' `wrap`).
         self.wrap_x: bool = False
         self.wrap_y: bool = False
         self._program = None
@@ -447,15 +447,13 @@ class VAEHook:
 
     def split_tiles(self, h, w):
         """tilevae.py:405-462 -> (tile_input_bboxes, tile_output_bboxes), each [x1, x2, y1, y2].  On a wrapped axis the
-        input bboxes are in unwrapped coordinates (td_vae_split_tiles_wrap)."""
-        wrap = self._wrap()
-        args = (int(h), int(w), int(self.tile_size), int(self.pad), int(self.is_decoder))
-        split = (lambda *a: lib.td_vae_split_tiles_wrap(*args, wrap, *a)) if wrap else (lambda *a: lib.td_vae_split_tiles(*args, *a))
-        n = check(split(None, None, 0))
+        input bboxes are in unwrapped coordinates."""
+        args = (int(h), int(w), int(self.tile_size), int(self.pad), int(self.is_decoder), self._wrap())
+        n = check(lib.td_vae_split_tiles(*args, None, None, 0))
         ib = np.empty((n, 4), dtype=np.int32)
         ob = np.empty((n, 4), dtype=np.int32)
         p = ctypes.POINTER(ctypes.c_int32)
-        check(split(ib.ctypes.data_as(p), ob.ctypes.data_as(p), n))
+        check(lib.td_vae_split_tiles(*args, ib.ctypes.data_as(p), ob.ctypes.data_as(p), n))
         return ib.tolist(), ob.tolist()
 
     def _cheap_fallback(self, z, device, dtype):

@@ -30,9 +30,10 @@ def test_abi_version_and_error_string():
     assert b"overlap" in _cabi.lib.td_last_error()
 
 
-def test_struct_layout_matches_header():
+def test_grid_struct_layout_matches_header():
     from multidiffusion_upscaler_for_automatic1111_b200 import _cabi
-    assert ctypes.sizeof(_cabi.TdGrid) == 4 * (10 + 2 * _cabi.TD_MAX_GRID_DIM)
+    assert ctypes.sizeof(_cabi.TdGrid) == 4 * (11 + 2 * _cabi.TD_MAX_GRID_DIM)
+    assert _cabi.TdGrid.wrap.offset == 4 * 10 and _cabi.TdGrid.ys.offset == 4 * 11
 
 
 def test_missing_library_fails_loudly(tmp_path, monkeypatch):

@@ -1,5 +1,5 @@
-"""Seamless tiling, host side (no GPU needed): the periodic tile plan (td_grid_init_wrap), its weight canvas
-(td_grid_weights_wrap) and the grid validation of the scatter / blend entries, against tests/wrap_oracle.py."""
+"""Seamless tiling, host side (no GPU needed): the periodic tile plan (td_grid_init's `wrap`), its weight canvas
+(td_grid_weights) and the grid validation of the scatter / blend entries, against tests/wrap_oracle.py."""
 import ctypes
 import math
 
@@ -57,13 +57,20 @@ def test_cfg2_and_panorama_shapes():
 
 @pytest.mark.parametrize("w,h,tw,th,ov,bs", [(64, 48, 16, 16, 8, 4), (128, 128, 96, 96, 48, 4), (100, 37, 33, 20, 8, 3),
                                              (512, 512, 96, 96, 48, 8), (40, 40, 64, 64, 16, 1)])
-def test_wrap_zero_is_grid_init(w, h, tw, th, ov, bs):
+def test_grid_init_wrap_zero_is_the_bounded_plan(w, h, tw, th, ov, bs):
+    """wrap = 0 is the reference's bounded plan: clamps, origins, batches and the weight canvas bit for bit."""
+    from oracle import tiling
+    from multidiffusion_upscaler_for_automatic1111_b200 import engine
     from multidiffusion_upscaler_for_automatic1111_b200._cabi import TdGrid, lib
-    a, b = TdGrid(), TdGrid()
-    ra = lib.td_grid_init(ctypes.byref(a), w, h, tw, th, ov, bs)
-    rb = lib.td_grid_init_wrap(ctypes.byref(b), w, h, tw, th, ov, bs, 0)
-    assert ra == rb
-    assert bytes(a) == bytes(b)
+    g = TdGrid()
+    plan = tiling.GridPlan(w, h, tw, th, ov, bs, False)
+    assert lib.td_grid_init(ctypes.byref(g), w, h, tw, th, ov, bs, 0) == plan.num_tiles
+    assert g.wrap == 0
+    assert not any(g.xs[g.cols:]) and not any(g.ys[g.rows:])      # the rest of the struct is zero, as before
+    assert (g.tile_w, g.tile_h, g.overlap, g.num_batches, g.tile_bs) == (plan.tile_w, plan.tile_h, plan.overlap, plan.num_batches,
+                                                                        plan.tile_bs)
+    assert engine.grid_bboxes_xywh(g).tolist() == [list(b) for b in plan.bboxes]
+    assert engine.grid_weights(g).view(np.uint32).tolist() == plan.weights.view(np.uint32).tolist()
 
 
 @pytest.mark.parametrize("wrap", [wo.WRAP_X, wo.WRAP_Y, wo.WRAP_X | wo.WRAP_Y])
@@ -79,57 +86,64 @@ def test_weights_bit_equal(wrap, gaussian, shape):
     assert got.min() > 0
 
 
-def test_weights_wrap_rejects_a_tile_past_a_bounded_edge():
+def test_grid_weights_rejects_a_tile_past_a_bounded_edge():
     from multidiffusion_upscaler_for_automatic1111_b200._cabi import TD_ERR_INVALID_ARG, lib
     g = _grid(64, 48, 16, 16, 8, 4, wo.WRAP_X)
     assert g.xs[g.cols - 1] + g.tile_w > 64          # the periodic plan runs past the right edge
+    g.wrap = wo.WRAP_Y                               # ... which is now bounded
     out = np.empty((48, 64), dtype=np.float32)
-    st = lib.td_grid_weights_wrap(ctypes.byref(g), wo.WRAP_Y, None, out.ctypes.data_as(ctypes.POINTER(ctypes.c_float)))
+    st = lib.td_grid_weights(ctypes.byref(g), None, out.ctypes.data_as(ctypes.POINTER(ctypes.c_float)))
     assert st == TD_ERR_INVALID_ARG
 
 
-def test_periodic_grid_without_wrap_flag_is_refused_before_launch():
-    """The entries validate the plan on the host: a grid whose tiles run past the canvas on an axis whose wrap bit is
-    clear returns TD_ERR_INVALID_ARG before anything touches the device (the pointers here are never dereferenced)."""
-    from multidiffusion_upscaler_for_automatic1111_b200._cabi import TD_ERR_INVALID_ARG, TD_F16, TD_FLAG_WRAP_Y, lib
-    g = _grid(64, 48, 16, 16, 8, 4, wo.WRAP_X)
+def test_bounded_grid_leaving_the_canvas_is_refused_before_launch():
+    """The entries validate the plan on the host: a bounded plan whose hand-edited origins put a tile past the canvas
+    returns TD_ERR_INVALID_ARG before anything is written (the weight canvas) or touches the device (the pointers here are
+    never dereferenced)."""
+    from multidiffusion_upscaler_for_automatic1111_b200._cabi import TD_ERR_INVALID_ARG, TD_F16, lib
     fake = ctypes.c_void_p(256)
-    st = lib.td_scatter_tiles(ctypes.byref(g), fake, fake, 2, 4, TD_F16, 0, g.num_tiles, 0, None)
-    assert st == TD_ERR_INVALID_ARG and b"WRAP_X" in lib.td_last_error()
-    st = lib.td_scatter_tiles(ctypes.byref(g), fake, fake, 2, 4, TD_F16, 0, g.num_tiles, TD_FLAG_WRAP_Y, None)
-    assert st == TD_ERR_INVALID_ARG
-    ptrs = (ctypes.c_void_p * g.num_batches)(*([256] * g.num_batches))
-    st = lib.td_blend_multidiffusion(ctypes.byref(g), ptrs, g.num_batches, g.tile_bs, 2, 4, TD_F16, TD_F16, fake, None, fake, None, 0, None)
-    assert st == TD_ERR_INVALID_ARG
-    st = lib.td_blend_mixture(ctypes.byref(g), ptrs, g.num_batches, g.tile_bs, 2, 4, TD_F16, TD_F16, fake, fake, fake, 0, None)
-    assert st == TD_ERR_INVALID_ARG
+    for axis in ("xs", "ys"):
+        g = _grid(64, 48, 16, 16, 8, 4, 0)
+        origins = getattr(g, axis)
+        n = g.cols if axis == "xs" else g.rows
+        origins[n - 1] += 1                          # the last tile column / row now ends one pixel past the edge
+        out = np.zeros((48, 64), dtype=np.float32)
+        st = lib.td_grid_weights(ctypes.byref(g), None, out.ctypes.data_as(ctypes.POINTER(ctypes.c_float)))
+        assert st == TD_ERR_INVALID_ARG and not out.any()
+        st = lib.td_scatter_tiles(ctypes.byref(g), fake, fake, 2, 4, TD_F16, 0, g.num_tiles, 0, None)
+        assert st == TD_ERR_INVALID_ARG and b"leaves the" in lib.td_last_error()
+        ptrs = (ctypes.c_void_p * g.num_batches)(*([256] * g.num_batches))
+        st = lib.td_blend_multidiffusion(ctypes.byref(g), ptrs, g.num_batches, g.tile_bs, 2, 4, TD_F16, TD_F16, fake, None, fake, None, 0,
+                                         None)
+        assert st == TD_ERR_INVALID_ARG
+        st = lib.td_blend_mixture(ctypes.byref(g), ptrs, g.num_batches, g.tile_bs, 2, 4, TD_F16, TD_F16, fake, fake, fake, 0, None)
+        assert st == TD_ERR_INVALID_ARG
 
 
-def test_wrap_flags_refuse_the_opt_in_forms():
+def test_wrapped_plan_refuses_the_opt_in_forms():
     from multidiffusion_upscaler_for_automatic1111_b200._cabi import (TD_ERR_UNSUPPORTED, TD_F16, TD_FLAG_ROWS, TD_FLAG_STRIP, TD_FLAG_TMA,
-                                                                      TD_FLAG_PIPELINE, TD_FLAG_WRAP_X, lib)
+                                                                      TD_FLAG_PIPELINE, lib)
     g = _grid(64, 48, 16, 16, 8, 4, wo.WRAP_X)
     fake = ctypes.c_void_p(256)
     ptrs = (ctypes.c_void_p * g.num_batches)(*([256] * g.num_batches))
-    for form in (TD_FLAG_ROWS, TD_FLAG_STRIP, TD_FLAG_TMA, TD_FLAG_PIPELINE):
-        f = TD_FLAG_WRAP_X | form
+    for f in (TD_FLAG_ROWS, TD_FLAG_STRIP, TD_FLAG_TMA, TD_FLAG_PIPELINE):
         assert lib.td_scatter_tiles(ctypes.byref(g), fake, fake, 2, 4, TD_F16, 0, g.num_tiles, f, None) == TD_ERR_UNSUPPORTED
         assert lib.td_blend_multidiffusion(ctypes.byref(g), ptrs, g.num_batches, g.tile_bs, 2, 4, TD_F16, TD_F16, fake, None, fake, None, f,
                                            None) == TD_ERR_UNSUPPORTED
         assert lib.td_blend_mixture(ctypes.byref(g), ptrs, g.num_batches, g.tile_bs, 2, 4, TD_F16, TD_F16, fake, fake, fake, f,
                                     None) == TD_ERR_UNSUPPORTED
     assert lib.td_blend_multidiffusion_peer(ctypes.byref(g), ptrs, g.num_batches, g.tile_bs, 2, 4, TD_F16, TD_F16, fake, fake, None, fake, 1,
-                                            fake, TD_FLAG_WRAP_X, None) == TD_ERR_UNSUPPORTED
+                                            fake, 0, None) == TD_ERR_UNSUPPORTED
     assert lib.td_blend_multidiffusion_rows(ctypes.byref(g), ptrs, g.num_batches, g.tile_bs, 2, 4, TD_F16, TD_F16, fake, None, fake, None, 0,
-                                            48, None, 0, None, 0, 0, TD_FLAG_WRAP_X, None) == TD_ERR_UNSUPPORTED
+                                            48, None, 0, None, 0, 0, 0, None) == TD_ERR_UNSUPPORTED
 
 
-def test_engine_carries_wrap_on_the_plan():
+def test_plan_records_its_wrap_bits():
     from multidiffusion_upscaler_for_automatic1111_b200 import engine
     g = engine.make_grid(64, 48, 16, 16, 8, 4, wrap=engine.WRAP_X)
-    assert engine.grid_wrap(g) == engine.WRAP_X
-    assert engine.grid_wrap(engine.scaled_grid(g, 8)) == engine.WRAP_X
-    assert engine.grid_wrap(engine.make_grid(64, 48, 16, 16, 8, 4)) == 0
+    assert g.wrap == engine.WRAP_X
+    assert engine.scaled_grid(g, 8).wrap == engine.WRAP_X
+    assert engine.make_grid(64, 48, 16, 16, 8, 4).wrap == 0
 
 
 # ------------------------------------------------------------------------------------------------ tiled VAE split

@@ -1,5 +1,5 @@
-"""Oracle for seamless (periodic) tiling: numpy / torch-CPU restatement of td_grid_init_wrap, td_grid_weights_wrap and the
-wrap forms of the scatter and both blends (TD_FLAG_WRAP_X / TD_FLAG_WRAP_Y).
+"""Oracle for seamless (periodic) tiling: numpy / torch-CPU restatement of td_grid_init and td_grid_weights on a plan with
+wrap bits, and of the scatter and both blends on such a plan.
 
 Written from the plan's definition, with explicit per-tile loops and the same dtype round trips as oracle/blend.py:
 the canvas accumulates in its dtype with one rounding per tile add in tile-list order, MultiDiffusion divides in fp32
@@ -147,7 +147,7 @@ def blur_denoise(x_tile: torch.Tensor, bboxes=None) -> torch.Tensor:
 
 # ------------------------------------------------------------------------------------------------ tiled VAE
 def vae_split_wrap(h: int, w: int, tile_size: int, pad: int, is_decoder: bool, wrap: int):
-    """td_vae_split_tiles_wrap: (in_bboxes, out_bboxes), [x1, x2, y1, y2] each, rows outer.  A non-wrapped axis is taken
+    """td_vae_split_tiles with wrap bits: (in_bboxes, out_bboxes), [x1, x2, y1, y2] each, rows outer.  A non-wrapped axis is taken
     from oracle/vae.py's split_tiles; a wrapped axis of length L is cut at b_k = m * floor(k * L / (n * m)),
     n = max(ceil(L / tile), 1), b_n = L, input [b_k - pad, b_{k+1} + pad) unclipped."""
     from oracle import vae as ovae
