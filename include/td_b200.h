@@ -265,7 +265,8 @@ int td_blend_multidiffusion_peer(const td_grid* g, const void* const* batch_ptrs
  * outputs or the halo buffer its neighbours pushed the overlapping tile rows into (entries of tile rows that do not
  * touch the range are never dereferenced).  Same arithmetic, same tile order: bit-identical to the whole-canvas blend.
  * own_band_begin / own_band_end: tile rows whose batch_ptrs entries are LOCAL outputs -- CTAs that read only those skip the
- * wait and are scheduled ahead of the ones that need a neighbour's halo (begin == end: every CTA waits). */
+ * wait and are scheduled ahead of the ones that need a neighbour's halo (begin == end: every CTA waits).  A build whose
+ * blend patches are taller than 8 rows (TD_AS_ROWS) refuses a window not aligned to them with TD_ERR_UNSUPPORTED. */
 int td_blend_multidiffusion_rows(const td_grid* g, const void* const* batch_ptrs, int num_batches, int tile_bs,
                                  int N, int C, int tile_dtype, int acc_dtype, const float* weights,
                                  const float* rcp_weights, float* x_out, void* x_buffer, int row_begin, int row_end,
@@ -284,7 +285,8 @@ int td_peer_wait(const uint32_t* flags, int count, const uint32_t* value, void* 
  * bump_next (NULL: none): a second expect counter advanced by TD_PUSH_CTAS at the end of the launch -- the tile-halo set's,
  * by the latent-halo push that closes a step, so that the next step's blend (td_blend_multidiffusion_rows: wait_value) reads a
  * value written on ITS stream while the tile-halo push itself may run on a side stream.  Expect counters of a set that is
- * only ever waited on through bump_next start at TD_PUSH_CTAS. */
+ * only ever waited on through bump_next start at TD_PUSH_CTAS.  n_regions 0 is a signal-only push: the slots still advance
+ * by TD_PUSH_CTAS (a rank inside a waiter's range that has no rows for it). */
 #define TD_MAX_PUSH_REGIONS 8
 #define TD_PUSH_CTAS 32
 typedef struct td_push_region {

@@ -1615,8 +1615,13 @@ extern "C" int td_blend_multidiffusion_rows(const td_grid* g, const void* const*
         td_set_error("td_blend_multidiffusion_rows: needs the vector path (same tile / canvas dtype, W and tile_w multiples of the vector, 16-byte aligned buffers)");
         return TD_ERR_UNSUPPORTED;
     }
-    bp.py0 = row_begin / 8;
-    bp.py_count = (row_end - row_begin + 7) / 8;
+    // the window is cut into whole patch rows of the cp.async kernel (kAsY rows, a build-time knob; 8 by default)
+    if (row_begin % kAsY != 0 || (row_end % kAsY != 0 && row_end != g->H)) {
+        td_set_error("td_blend_multidiffusion_rows: rows [%d,%d) are not aligned to the %d-row patches of this build", row_begin, row_end, kAsY);
+        return TD_ERR_UNSUPPORTED;
+    }
+    bp.py0 = row_begin / kAsY;
+    bp.py_count = (row_end - row_begin + kAsY - 1) / kAsY;
     if (wait_count > 0) { bp.wait_flags = wait_flags; bp.wait_world = wait_count; bp.wait_value = wait_value; }
     if (own_band_begin < 0 || own_band_end > g->rows || own_band_begin > own_band_end) {
         td_set_error("td_blend_multidiffusion_rows: own bands [%d,%d) outside the %d tile rows", own_band_begin, own_band_end, g->rows);

@@ -372,6 +372,40 @@ class StripShard:
         r = self.rank if r is None else r
         return [(p, a, b) for p in range(self.world) if p != r for (q, a, b) in self.x_in(p) if q == r]
 
+    # ---- flag bookkeeping of the two pushes of a step ("tiles": tile halo, "x": latent halo) ------------------------
+    # A waiter polls ONE contiguous run of flag slots, the span of the ranks that send it rows.  The span may hold a rank
+    # that has no rows for it (the latent-halo senders of a pitch-4 plan can skip a rank whose strip is empty), and such a
+    # rank must still bump its slot every step or the wait never ends: every rank inside a waiter's span pushes to it once
+    # per step, a signal-only push (no regions) when it has nothing to send.  The tile-halo span runs over lower ranks,
+    # the latent-halo span over higher ones, so no wait cycle can form.
+    def _flag_plan(self):
+        if not hasattr(self, "_flag_plan_cache"):
+            plan = {}
+            for kind in ("tiles", "x"):
+                spans = []
+                for r in range(self.world):
+                    s = sorted({p for (_, p, _, _) in self.halo_in(r)}) if kind == "tiles" else sorted({q for (q, _, _) in self.x_in(r)})
+                    spans.append((s[0], s[-1] - s[0] + 1) if s else (0, 0))
+                targets = [[q for q in range(self.world) if spans[q][0] <= r < spans[q][0] + spans[q][1]] for r in range(self.world)]
+                plan[kind] = (spans, targets)
+            self._flag_plan_cache = plan
+        return self._flag_plan_cache
+
+    def wait_range(self, kind: str, r: Optional[int] = None):
+        """(first, count): rank r's wait of flag set `kind` polls the slots of ranks [first, first + count) (count 0: no wait)."""
+        r = self.rank if r is None else r
+        return self._flag_plan()[kind][0][r]
+
+    def signallers(self, kind: str, r: Optional[int] = None) -> List[int]:
+        """The ranks that must push to rank r in set `kind` every step: exactly those of its wait range."""
+        first, count = self.wait_range(kind, r)
+        return list(range(first, first + count))
+
+    def push_targets(self, kind: str, r: Optional[int] = None) -> List[int]:
+        """The ranks rank r pushes to in set `kind` every step (with rows, or signal-only), ascending."""
+        r = self.rank if r is None else r
+        return list(self._flag_plan()[kind][1][r])
+
 
 # measurement switches (defaults = the shipped path): TD_STRIP_LATE_WAIT=0 -> every blend CTA waits for the halos (no own-band
 # test, no reordered schedule)
@@ -487,8 +521,8 @@ class StripExchange:
         self.x_out = self._xout.tensor(device).view(torch.float32).view(N, C, sh.H, W)
         self._side, self._join = None, None
         self.flags_tiles.set_expect(_cabi.TD_PUSH_CTAS)      # the first step's blend waits for ONE push of each sender
-        self._senders = sorted({p for (_, p, _, _) in sh.halo_in()})
-        self._x_senders = sorted({q for (q, _, _) in sh.x_in()})
+        self._tile_wait, self._x_wait = sh.wait_range("tiles"), sh.wait_range("x")
+        self._tile_targets, self._x_targets = sh.push_targets("tiles"), sh.push_targets("x")
         dist.barrier(group=group)
 
     # ---- this rank's tile outputs -----------------------------------------------------------------------------
@@ -504,20 +538,19 @@ class StripExchange:
         sh = self.shard
         plane = sh.tile_h * self.tw * self.es
         planes = sh.cols * self.N * self.C
-        targets, regions = set(), []
+        regions = []
         for (i, q, v0, v1) in sh.halo_out():
             src = self._own.data_ptr() + ((i - sh.band_begin[sh.rank]) * self.band_elems + v0 * self.tw) * self.es
             slot = self.peer_halo_bands[q].index(i)
             dst = self.peer_halo[q] + (slot * self.band_elems + v0 * self.tw) * self.es
             # rows v0..v1 of a tile are contiguous: one "row" of (v1 - v0) * tw elements per tile plane
             regions.append((src, dst, planes, 1, (v1 - v0) * self.tw * self.es, plane, plane, plane, plane))
-            targets.add(q)
         if not self._aligned(regions):
             raise ValueError("row-strip shard: tile width and halo offsets must be multiples of 16 bytes")
         # the blend's expect counter of this set is advanced by the latent-halo push that closed the PREVIOUS step (bump_next):
         # nothing this launch writes is read by this rank's own blend, so it may ride a side stream
         if not _OVERLAP_PUSH:
-            self.flags_tiles.push(regions, sorted(targets), bump_own=False)
+            self.flags_tiles.push(regions, self._tile_targets, bump_own=False)
             return
         # side stream: this rank's blend waits (in-kernel, only in the CTAs that read a halo) for the NEIGHBOUR's push, not
         # for this one -- the NVLink copy overlaps the blend of the interior rows; push_x_halos_and_wait joins the side
@@ -529,7 +562,7 @@ class StripExchange:
         fork.record(main)
         self._side.wait_event(fork)
         with torch.cuda.stream(self._side):
-            self.flags_tiles.push(regions, sorted(targets), bump_own=False)
+            self.flags_tiles.push(regions, self._tile_targets, bump_own=False)
             self._join = torch.cuda.Event()
             self._join.record(self._side)
 
@@ -557,9 +590,7 @@ class StripExchange:
         region composite starts from it)."""
         sh = self.shard
         lo, hi = sh.strip()
-        first = self._senders[0] if self._senders else 0
-        count = (self._senders[-1] - first + 1) if self._senders else 0
-        f, c, v = self.flags_tiles.wait_args(first, count)
+        f, count, v = self.flags_tiles.wait_args(*self._tile_wait)
         if hi <= lo:                       # this rank owns no canvas rows (more ranks than tile rows)
             return self.x_out
         if not hasattr(self, "_ptr_table"):
@@ -581,20 +612,19 @@ class StripExchange:
 
     def push_x_halos_and_wait(self):
         """Rows of my strip that lower ranks scatter from -> their latent buffers; then wait for mine to arrive
-        (copy + signal + wait in one launch: td_push_regions)."""
+        (copy + signal + wait in one launch: td_push_regions).  Every rank whose wait range holds mine is signalled, also
+        one I send no rows to (StripShard.push_targets)."""
         sh = self.shard
-        targets, regions = set(), []
+        regions = []
         plane = sh.H * self.W * 4
         for (p, a, b) in sh.x_out():
             off = a * self.W * 4
             regions.append((self._xout.ptr + off, self.peer_xout[p] + off, self.N * self.C, 1, (b - a) * self.W * 4, plane, plane, plane, plane))
-            targets.add(p)
-        first = self._x_senders[0] if self._x_senders else 0
-        count = (self._x_senders[-1] - first + 1) if self._x_senders else 0
+        first, count = self._x_wait
         self.join_side()
         if not self._aligned(regions):
             raise ValueError("row-strip shard: latent width must be a multiple of 4 elements")
-        self.flags_x.push(regions, sorted(targets), first, count, bump_own=True, bump_next=self.flags_tiles.counter_ptr)
+        self.flags_x.push(regions, self._x_targets, first, count, bump_own=True, bump_next=self.flags_tiles.counter_ptr)
 
     def gather_latent(self, x: torch.Tensor) -> torch.Tensor:
         """All ranks' strips of `x` (any tensor laid out like the latent) -> the full latent on every rank."""
