@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define TD_ABI_VERSION 10
+#define TD_ABI_VERSION 11
 
 typedef enum td_status {
     TD_OK = 0,
@@ -272,6 +272,17 @@ int td_blend_multidiffusion_rows(const td_grid* g, const void* const* batch_ptrs
                                  const float* rcp_weights, float* x_out, void* x_buffer, int row_begin, int row_end,
                                  const uint32_t* wait_flags, int wait_count, const uint32_t* wait_value,
                                  int own_band_begin, int own_band_end, uint32_t flags, void* stream);
+/* Row-strip tile shard, Mixture of Diffusers: td_blend_mixture restricted to canvas rows [row_begin, row_end) of x_buffer
+ * (whole-canvas, acc_dtype; the other rows are not written), with the row window, the per-tile-row batch_ptrs, the halo wait
+ * and the own bands of td_blend_multidiffusion_rows, and the same refusals.  Same arithmetic, same tile order: the union of
+ * the strips is bit-identical to td_blend_mixture over the whole canvas.  Needs the vector path (tile_dtype == acc_dtype,
+ * W and tile_w multiples of the vector, 16-byte aligned tile_weights / rescale / x_buffer) and tile_w % 8 == 0, else
+ * TD_ERR_UNSUPPORTED. */
+int td_blend_mixture_rows(const td_grid* g, const void* const* batch_ptrs, int num_batches, int tile_bs,
+                          int N, int C, int tile_dtype, int acc_dtype, const float* tile_weights,
+                          const float* rescale, void* x_buffer, int row_begin, int row_end,
+                          const uint32_t* wait_flags, int wait_count, const uint32_t* wait_value,
+                          int own_band_begin, int own_band_end, uint32_t flags, void* stream);
 /* One warp spins (acquire, system scope, bounded) until flags[i] >= *value for i < count: stream-ordered work after it
  * sees what the signalling ranks wrote before their td_peer_signal. */
 int td_peer_wait(const uint32_t* flags, int count, const uint32_t* value, void* stream);

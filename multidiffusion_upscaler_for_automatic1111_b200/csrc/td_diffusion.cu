@@ -453,6 +453,29 @@ struct __align__(16) VisitEntry {   // per tile visit of a CTA, computed once by
 };
 constexpr int kAsMaxVisits = 64;
 
+// Row-strip shard, cp.async blends: the peers' tile outputs must be complete before any copy of this CTA reads them.  Only
+// CTAs whose visits leave the own bands [own_r_lo, own_r_hi) wait (all of them when the range is empty); the last warp spins
+// and the CTA's next barrier publishes the wait to the other threads.
+__device__ __forceinline__ void halo_wait(const BlendParams& p, int by, int r_lo, int tid) {
+    const bool reads_halo = r_lo < p.own_r_lo || r_lo + (int)p.prow_n[by] > p.own_r_hi;   // always true when own_r_lo == own_r_hi
+    if (p.wait_flags != nullptr && reads_halo && tid >= kAsThreads - 32 && tid - (kAsThreads - 32) < p.wait_world) {
+        const uint32_t want = *p.wait_value;
+        uint32_t v;
+        unsigned long long spins = 0;
+        do {   // bounded: a peer that never signals becomes a launch error, not a hung GPU
+            asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p.wait_flags + (tid - (kAsThreads - 32))) : "memory");
+            if (++spins > (1ull << 31)) __trap();
+        } while ((int32_t)(v - want) < 0);
+    }
+}
+
+// Patch row and plane group of a cp.async blend CTA: sched 0 walks blockIdx.y = patch row, .z = plane group; sched 1 / 2 put
+// the patch row on blockIdx.z (slowest-varying), ascending / descending from the window's start py0.
+__device__ __forceinline__ int window_row_index(const BlendParams& p) {
+    return p.sched == 0 ? (int)blockIdx.y : (p.sched == 2 ? p.py_count - 1 - (int)blockIdx.z : (int)blockIdx.z);
+}
+__device__ __forceinline__ int plane_group_index(const BlendParams& p) { return p.sched == 0 ? (int)blockIdx.z : (int)blockIdx.y; }
+
 template <typename T, int S, int PPC>
 __device__ __forceinline__ void consume_planes(uint4 (&acc)[PPC], const unsigned char* p) {
 #pragma unroll
@@ -473,8 +496,8 @@ blend_md_async_kernel(const __grid_constant__ BlendParams p, const float* __rest
     __shared__ int s_shift[kAsMaxVisits];
     const GeomParams& g = p.g;
     const int tid = threadIdx.x;
-    const int zy = p.sched == 0 ? (int)blockIdx.y : (p.sched == 2 ? p.py_count - 1 - (int)blockIdx.z : (int)blockIdx.z);
-    const int plane = (p.sched == 0 ? (int)blockIdx.z : (int)blockIdx.y) * PPC;   // first plane of this CTA (PPC divides N*C)
+    const int zy = window_row_index(p);
+    const int plane = plane_group_index(p) * PPC;   // first plane of this CTA (PPC divides N*C)
     const int by = zy + p.py0;                // patch row (a row-range launch starts at py0)
     const int x_lo = blockIdx.x * BX, y_lo = by * kAsY;
     pdl_launch_dependents();
@@ -497,10 +520,10 @@ blend_md_async_kernel(const __grid_constant__ BlendParams p, const float* __rest
         if constexpr (FASTDIV) rv[h] = inside ? __ldg(reinterpret_cast<const float4*>(rcp_weights + wo) + h) : make_float4(1.f, 1.f, 1.f, 1.f);
     }
 
+    // halo_wait, written out: through the helper the compiler schedules this kernel's prologue differently (cfg2 blend
+    // measured about 0.5% slower on an H100 80GB HBM3 at 700 W)
     const bool reads_halo = r_lo < p.own_r_lo || r_lo + (int)p.prow_n[by] > p.own_r_hi;   // always true when own_r_lo == own_r_hi
     if (p.wait_flags != nullptr && reads_halo && tid >= kAsThreads - 32 && tid - (kAsThreads - 32) < p.wait_world) {
-        // tile shard: the peers' tile outputs must be complete before any copy reads them (last warp spins,
-        // the barrier below publishes it to the CTA)
         const uint32_t want = *p.wait_value;
         uint32_t v;
         unsigned long long spins = 0;
@@ -641,7 +664,9 @@ __device__ __forceinline__ void mod_accumulate(float (&acc)[Vec<T>::kElems], con
     }
 }
 
-template <typename T>
+// WINDOW: a row-window launch (td_blend_mixture_rows: py0 / py_count, sched, halo wait); without it the grid is the whole
+// canvas with blockIdx.y = patch row, and none of that code is compiled in (the whole-canvas blend keeps its instruction stream).
+template <typename T, bool WINDOW>
 __global__ void __launch_bounds__(kAsThreads)
 blend_mod_async_kernel(const __grid_constant__ BlendParams p, const float* __restrict__ tile_weights, const float* __restrict__ rescale,
                        T* __restrict__ out_buf) {
@@ -653,11 +678,12 @@ blend_mod_async_kernel(const __grid_constant__ BlendParams p, const float* __res
     __shared__ int s_shift[kAsMaxVisits];
     const GeomParams& g = p.g;
     const int tid = threadIdx.x;
-    const int plane = blockIdx.z;
-    const int x_lo = blockIdx.x * BX, y_lo = blockIdx.y * kAsY;
-    const int r_lo = p.prow_lo[blockIdx.y], c_lo = p.pcol_lo[blockIdx.x];
+    const int by = WINDOW ? window_row_index(p) + p.py0 : (int)blockIdx.y;
+    const int plane = WINDOW ? plane_group_index(p) : (int)blockIdx.z;
+    const int x_lo = blockIdx.x * BX, y_lo = by * kAsY;
+    const int r_lo = p.prow_lo[by], c_lo = p.pcol_lo[blockIdx.x];
     const int nc = p.pcol_n[blockIdx.x];
-    const int nv = (int)p.prow_n[blockIdx.y] * nc;
+    const int nv = (int)p.prow_n[by] * nc;
     pdl_launch_dependents();
 
     const int tx = tid % kAsX, ty = tid / kAsX;
@@ -673,6 +699,7 @@ blend_mod_async_kernel(const __grid_constant__ BlendParams p, const float* __res
 #pragma unroll
     for (int j = 0; j < VEC; ++j)   // 1/0 = inf marks a pixel no tile covers: it receives only zero fill, keep 0 * w finite
         if (isinf(rs[j])) rs[j] = 0.0f;
+    if constexpr (WINDOW) halo_wait(p, by, r_lo, tid);
 
     if (tid < nv) {
         const int ri = tid / nc, ci = tid - ri * nc;
@@ -1358,6 +1385,19 @@ int launch_blend_async_impl(const BlendParams& bp, const float* weights, const f
     return check_launch("td_blend_multidiffusion (cp.async)");
 }
 
+// Row-strip shard (patch tables filled): only the CTAs that read a neighbour's band wait; they sit at the end of the row range
+// the halo enters from and are scheduled last (patch row = slowest grid dimension, walked away from that end).
+void schedule_halo_waits_last(BlendParams& bp) {
+    if (bp.wait_flags == nullptr || bp.own_r_hi <= bp.own_r_lo || bp.py_count <= 0) return;
+    int first_wait = -1, last_wait = -1;
+    for (int by = bp.py0; by < bp.py0 + bp.py_count; ++by) {
+        const int lo = bp.prow_lo[by], n = bp.prow_n[by];
+        if (n > 0 && (lo < bp.own_r_lo || lo + n > bp.own_r_hi)) { if (first_wait < 0) first_wait = by; last_wait = by; }
+    }
+    const int mid2 = 2 * bp.py0 + bp.py_count - 1;      // 2 x centre of the range
+    bp.sched = (first_wait >= 0 && first_wait + last_wait <= mid2) ? 2 : 1;
+}
+
 template <typename T, bool WRITE_BUF>
 int launch_blend_async(const td_grid* g, const BlendParams& bp_in, const float* weights, const float* rcp_weights, float* out_f32,
                        void* out_buf, int nv_cap, bool pipelined, cudaStream_t st) {
@@ -1366,20 +1406,22 @@ int launch_blend_async(const td_grid* g, const BlendParams& bp_in, const float* 
     BlendParams bp = bp_in;
     fill_patch_table(g->ys, g->rows, g->tile_h, g->H, kAsY, bp.prow_lo, bp.prow_n);
     fill_patch_table(g->xs, g->cols, g->tile_w, g->W, BX, bp.pcol_lo, bp.pcol_n);
-    if (bp.wait_flags != nullptr && bp.own_r_hi > bp.own_r_lo && bp.py_count > 0 && !pipelined) {
-        // row-strip shard: only the CTAs that read a neighbour's band wait; they sit at the end of the row range the halo
-        // enters from and are scheduled last (patch row = slowest grid dimension, walked away from that end)
-        int first_wait = -1, last_wait = -1;
-        for (int by = bp.py0; by < bp.py0 + bp.py_count; ++by) {
-            const int lo = bp.prow_lo[by], n = bp.prow_n[by];
-            if (n > 0 && (lo < bp.own_r_lo || lo + n > bp.own_r_hi)) { if (first_wait < 0) first_wait = by; last_wait = by; }
-        }
-        const int mid2 = 2 * bp.py0 + bp.py_count - 1;      // 2 x centre of the range
-        bp.sched = (first_wait >= 0 && first_wait + last_wait <= mid2) ? 2 : 1;
-    }
+    if (!pipelined) schedule_halo_waits_last(bp);
     if (rcp_weights != nullptr && sizeof(T) == 2)
         return launch_blend_async_impl<T, WRITE_BUF, true>(bp, weights, rcp_weights, out_f32, out_buf, nv_cap, pipelined, st);
     return launch_blend_async_impl<T, WRITE_BUF, false>(bp, weights, nullptr, out_f32, out_buf, nv_cap, pipelined, st);
+}
+
+template <typename T, bool WINDOW>
+int launch_blend_mod_async(const BlendParams& bp, int smem, const float* tile_weights, const float* rescale, void* out_buf, cudaStream_t st) {
+    constexpr int BX = kAsX * Vec<T>::kElems;
+    static SmemOptIn configured;
+    int rc = ensure_dyn_smem(blend_mod_async_kernel<T, WINDOW>, smem, &configured);
+    if (rc != TD_OK) return rc;
+    const unsigned gy = (unsigned)(WINDOW ? bp.py_count : (bp.g.H + kAsY - 1) / kAsY), gz = (unsigned)(bp.g.N * bp.g.C);
+    dim3 grid((unsigned)((bp.g.W + BX - 1) / BX), bp.sched ? gz : gy, bp.sched ? gy : gz);
+    launch_pdl(blend_mod_async_kernel<T, WINDOW>, grid, dim3(kAsThreads), (size_t)smem, st, bp, tile_weights, rescale, (T*)out_buf);
+    return TD_OK;
 }
 
 // Mixture of Diffusers on the cp.async kernel; 0 launched, 1 not applicable, <0 error
@@ -1396,12 +1438,10 @@ int try_launch_blend_mod_async(const td_grid* g, const BlendParams& bp_in, const
     BlendParams bp = bp_in;
     fill_patch_table(g->ys, g->rows, g->tile_h, g->H, kAsY, bp.prow_lo, bp.prow_n);
     fill_patch_table(g->xs, g->cols, g->tile_w, g->W, BX, bp.pcol_lo, bp.pcol_n);
-    const int smem = nv_cap * kAsStage;
-    static SmemOptIn configured;
-    int rc = ensure_dyn_smem(blend_mod_async_kernel<T>, smem, &configured);
+    schedule_halo_waits_last(bp);
+    const int rc = bp.py_count > 0 ? launch_blend_mod_async<T, true>(bp, nv_cap * kAsStage, tile_weights, rescale, out_buf, st)
+                                   : launch_blend_mod_async<T, false>(bp, nv_cap * kAsStage, tile_weights, rescale, out_buf, st);
     if (rc != TD_OK) return rc;
-    dim3 grid((unsigned)((bp.g.W + BX - 1) / BX), (unsigned)((bp.g.H + kAsY - 1) / kAsY), (unsigned)(bp.g.N * bp.g.C));
-    launch_pdl(blend_mod_async_kernel<T>, grid, dim3(kAsThreads), (size_t)smem, st, bp, tile_weights, rescale, (T*)out_buf);
     return check_launch("td_blend_mixture (cp.async)");
 }
 
@@ -1590,6 +1630,41 @@ extern "C" int td_blend_multidiffusion(const td_grid* g, const void* const* batc
     return dispatch_generic<MODE_MD>(tile_dtype, acc_dtype, bp, weights, nullptr, nullptr, x_out, x_buffer, s);
 }
 
+// The row window and the halo wait of a rows blend (td_blend_multidiffusion_rows / td_blend_mixture_rows), checked and set in
+// bp.  `ptrs`: the buffers the vector path needs 16-byte aligned.  Returns TD_OK to launch, 1 for an empty window (nothing to
+// launch), or a td_status.
+static int setup_rows_window(const td_grid* g, BlendParams* bp, const char* what, int tile_dtype, int acc_dtype,
+                             std::initializer_list<const void*> ptrs, int row_begin, int row_end, const uint32_t* wait_flags,
+                             int wait_count, const uint32_t* wait_value, int own_band_begin, int own_band_end) {
+    if (row_begin < 0 || row_end > g->H || row_begin > row_end || row_begin % 8 != 0 || (row_end % 8 != 0 && row_end != g->H)) {
+        td_set_error("%s: rows [%d,%d) must lie in [0,%d) on multiples of 8", what, row_begin, row_end, g->H);
+        return TD_ERR_INVALID_ARG;
+    }
+    if (wait_count < 0 || wait_count > TD_MAX_PEERS || (wait_count > 0 && (wait_flags == nullptr || wait_value == nullptr))) {
+        td_set_error("%s: bad wait table", what);
+        return TD_ERR_INVALID_ARG;
+    }
+    if (row_begin == row_end) return 1;
+    if (!blend_vec_ok(*bp, tile_dtype, acc_dtype, ptrs)) {
+        td_set_error("%s: needs the vector path (same tile / canvas dtype, W and tile_w multiples of the vector, 16-byte aligned buffers)", what);
+        return TD_ERR_UNSUPPORTED;
+    }
+    // the window is cut into whole patch rows of the cp.async kernel (kAsY rows, a build-time knob; 8 by default)
+    if (row_begin % kAsY != 0 || (row_end % kAsY != 0 && row_end != g->H)) {
+        td_set_error("%s: rows [%d,%d) are not aligned to the %d-row patches of this build", what, row_begin, row_end, kAsY);
+        return TD_ERR_UNSUPPORTED;
+    }
+    bp->py0 = row_begin / kAsY;
+    bp->py_count = (row_end - row_begin + kAsY - 1) / kAsY;
+    if (wait_count > 0) { bp->wait_flags = wait_flags; bp->wait_world = wait_count; bp->wait_value = wait_value; }
+    if (own_band_begin < 0 || own_band_end > g->rows || own_band_begin > own_band_end) {
+        td_set_error("%s: own bands [%d,%d) outside the %d tile rows", what, own_band_begin, own_band_end, g->rows);
+        return TD_ERR_INVALID_ARG;
+    }
+    if (wait_count > 0 && own_band_end > own_band_begin) { bp->own_r_lo = own_band_begin; bp->own_r_hi = own_band_end; }   // -> schedule_halo_waits_last
+    return TD_OK;
+}
+
 extern "C" int td_blend_multidiffusion_rows(const td_grid* g, const void* const* batch_ptrs, int num_batches, int tile_bs, int N,
                                             int C, int tile_dtype, int acc_dtype, const float* weights, const float* rcp_weights,
                                             float* x_out, void* x_buffer, int row_begin, int row_end, const uint32_t* wait_flags,
@@ -1602,32 +1677,9 @@ extern "C" int td_blend_multidiffusion_rows(const td_grid* g, const void* const*
     if (st != TD_OK) return st;
     if ((st = refuse_wrapped(g, "td_blend_multidiffusion_rows")) != TD_OK) return st;
     if (weights == nullptr || x_out == nullptr) { td_set_error("td_blend_multidiffusion_rows: null weights / x_out"); return TD_ERR_INVALID_ARG; }
-    if (row_begin < 0 || row_end > g->H || row_begin > row_end || row_begin % 8 != 0 || (row_end % 8 != 0 && row_end != g->H)) {
-        td_set_error("td_blend_multidiffusion_rows: rows [%d,%d) must lie in [0,%d) on multiples of 8", row_begin, row_end, g->H);
-        return TD_ERR_INVALID_ARG;
-    }
-    if (wait_count < 0 || wait_count > TD_MAX_PEERS || (wait_count > 0 && (wait_flags == nullptr || wait_value == nullptr))) {
-        td_set_error("td_blend_multidiffusion_rows: bad wait table");
-        return TD_ERR_INVALID_ARG;
-    }
-    if (row_begin == row_end) return TD_OK;
-    if (!blend_vec_ok(bp, tile_dtype, acc_dtype, {weights, rcp_weights, x_out, x_buffer})) {
-        td_set_error("td_blend_multidiffusion_rows: needs the vector path (same tile / canvas dtype, W and tile_w multiples of the vector, 16-byte aligned buffers)");
-        return TD_ERR_UNSUPPORTED;
-    }
-    // the window is cut into whole patch rows of the cp.async kernel (kAsY rows, a build-time knob; 8 by default)
-    if (row_begin % kAsY != 0 || (row_end % kAsY != 0 && row_end != g->H)) {
-        td_set_error("td_blend_multidiffusion_rows: rows [%d,%d) are not aligned to the %d-row patches of this build", row_begin, row_end, kAsY);
-        return TD_ERR_UNSUPPORTED;
-    }
-    bp.py0 = row_begin / kAsY;
-    bp.py_count = (row_end - row_begin + kAsY - 1) / kAsY;
-    if (wait_count > 0) { bp.wait_flags = wait_flags; bp.wait_world = wait_count; bp.wait_value = wait_value; }
-    if (own_band_begin < 0 || own_band_end > g->rows || own_band_begin > own_band_end) {
-        td_set_error("td_blend_multidiffusion_rows: own bands [%d,%d) outside the %d tile rows", own_band_begin, own_band_end, g->rows);
-        return TD_ERR_INVALID_ARG;
-    }
-    if (wait_count > 0 && own_band_end > own_band_begin) { bp.own_r_lo = own_band_begin; bp.own_r_hi = own_band_end; }   // -> launch_blend_async
+    st = setup_rows_window(g, &bp, "td_blend_multidiffusion_rows", tile_dtype, acc_dtype, {weights, rcp_weights, x_out, x_buffer}, row_begin,
+                           row_end, wait_flags, wait_count, wait_value, own_band_begin, own_band_end);
+    if (st != TD_OK) return st == 1 ? TD_OK : st;
     cudaStream_t s = (cudaStream_t)stream;
     int rc;
     switch (tile_dtype) {
@@ -1728,4 +1780,31 @@ extern "C" int td_blend_mixture(const td_grid* g, const void* const* batch_ptrs,
         }
     }
     return dispatch_generic<MODE_MOD>(tile_dtype, acc_dtype, bp, nullptr, tile_weights, rescale, nullptr, x_buffer, s);
+}
+
+extern "C" int td_blend_mixture_rows(const td_grid* g, const void* const* batch_ptrs, int num_batches, int tile_bs, int N, int C,
+                                     int tile_dtype, int acc_dtype, const float* tile_weights, const float* rescale, void* x_buffer,
+                                     int row_begin, int row_end, const uint32_t* wait_flags, int wait_count, const uint32_t* wait_value,
+                                     int own_band_begin, int own_band_end, uint32_t flags, void* stream) {
+    BlendParams bp;
+    tl_pdl = !(flags & TD_FLAG_NO_PDL);
+    int st = fill_blend(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, &bp);
+    if (st != TD_OK) return st;
+    if ((st = refuse_wrapped(g, "td_blend_mixture_rows")) != TD_OK) return st;
+    if (tile_weights == nullptr || rescale == nullptr || x_buffer == nullptr) {
+        td_set_error("td_blend_mixture_rows: null tile_weights / rescale / x_buffer");
+        return TD_ERR_INVALID_ARG;
+    }
+    st = setup_rows_window(g, &bp, "td_blend_mixture_rows", tile_dtype, acc_dtype, {tile_weights, rescale, x_buffer}, row_begin, row_end,
+                           wait_flags, wait_count, wait_value, own_band_begin, own_band_end);
+    if (st != TD_OK) return st == 1 ? TD_OK : st;
+    cudaStream_t s = (cudaStream_t)stream;
+    int rc;
+    switch (tile_dtype) {
+        case TD_F16: rc = try_launch_blend_mod_async<__half>(g, bp, tile_weights, rescale, x_buffer, s); break;
+        case TD_BF16: rc = try_launch_blend_mod_async<__nv_bfloat16>(g, bp, tile_weights, rescale, x_buffer, s); break;
+        default: rc = try_launch_blend_mod_async<float>(g, bp, tile_weights, rescale, x_buffer, s); break;
+    }
+    if (rc == 1) { td_set_error("td_blend_mixture_rows: geometry outside the cp.async kernel's limits"); return TD_ERR_UNSUPPORTED; }
+    return rc;
 }

@@ -169,6 +169,24 @@ def blend_mixture(g: TdGrid, batch_outs: Sequence[torch.Tensor], N: int, C: int,
     return x_buffer
 
 
+def blend_mixture_rows(g: TdGrid, band_ptrs: Sequence[int], N: int, C: int, tile_dtype: torch.dtype, tile_weights: torch.Tensor,
+                       rescale: torch.Tensor, x_buffer: torch.Tensor, row_begin: int, row_end: int, wait=None,
+                       own_bands=(0, 0), flags: int = 0) -> torch.Tensor:
+    """`blend_mixture` of the canvas rows [row_begin, row_end) only (row-strip shard), written into those rows of the
+    whole-canvas x_buffer; returns it.  band_ptrs: one device pointer per tile ROW (the tiles of row i, [cols*N, C, th, tw]).
+    wait: (flags pointer, count, value pointer) -- the CTAs whose tiles leave the own bands [own_bands) first wait until
+    flags[0 .. count) >= *value (td_blend_mixture_rows)."""
+    _require_cuda(x_buffer, "x_buffer")
+    fptr, count, vptr = wait if wait is not None else (None, 0, None)
+    ptrs = (ctypes.c_void_p * len(band_ptrs))(*band_ptrs)
+    with torch.cuda.device(x_buffer.device):
+        check(lib.td_blend_mixture_rows(ctypes.byref(g), ptrs, len(band_ptrs), int(g.cols), N, C, dtype_code(tile_dtype),
+                                        dtype_code(x_buffer.dtype), tile_weights.data_ptr(), rescale.data_ptr(), x_buffer.data_ptr(),
+                                        int(row_begin), int(row_end), fptr if count else None, int(count), vptr if count else None,
+                                        int(own_bands[0]), int(own_bands[1]), int(flags), current_stream_ptr(x_buffer.device)))
+    return x_buffer
+
+
 # ---------------------------------------------------------------------------------------------------------
 # DemoFusion (tile_methods/demofusion.py): thin wrappers over the C-ABI, one launch each
 # ---------------------------------------------------------------------------------------------------------

@@ -22,7 +22,7 @@ from typing import List, Optional, Sequence
 import torch
 import torch.distributed as dist
 
-from . import _cabi
+from . import _cabi, engine
 from ._cabi import check, lib
 
 
@@ -486,19 +486,27 @@ class StripExchange:
     and mapped into their neighbours through CUDA IPC; halos are PUSHED over NVLink and published in the same launch
     (td_push_regions: 128-bit stores into peer memory, one release add per CTA into the target's flag slot), and awaited
     inside the blend kernel (only by the CTAs that read a halo band) / by the latent-halo push that closes the step.
-    No NCCL call on the data path; every launch is replayable from a CUDA graph (all counters live on the device)."""
+    No NCCL call on the data path; every launch is replayable from a CUDA graph (all counters live on the device).
 
-    def __init__(self, shard: StripShard, N: int, C: int, tile_w: int, W: int, dtype: torch.dtype, device: torch.device, group=None):
+    `dtype` is the tile dtype, `latent_dtype` the dtype of the blended latent `x_out`: fp32 for MultiDiffusion (`blend`), the
+    latent dtype for Mixture of Diffusers (`blend_mixture`), fp32 again when FOREGROUND regions are composited over it."""
+
+    def __init__(self, shard: StripShard, N: int, C: int, tile_w: int, W: int, dtype: torch.dtype, device: torch.device, group=None,
+                 latent_dtype: torch.dtype = torch.float32):
         self.shard, self.N, self.C, self.tw, self.W, self.dtype, self.device, self.group = shard, N, C, tile_w, W, dtype, device, group
         sh = shard
         self.es = torch.empty((), dtype=dtype).element_size()
+        self.latent_dtype = latent_dtype
+        self.xes = torch.empty((), dtype=latent_dtype).element_size()
+        if (W * self.xes) % 16 != 0:      # the latent-halo rows are pushed as 16-byte vectors
+            raise ValueError(f"row-strip shard: a {latent_dtype} latent needs W % {16 // self.xes} == 0 (W = {W})")
         self.band_elems = sh.cols * N * C * sh.tile_h * tile_w                 # one band of tiles [cols*N, C, th, tw]
         self.halo_bands = [i for (i, _, _, _) in sh.halo_in()]
         n_own = len(sh.bands())
         with torch.cuda.device(device):
             self._own = torch.empty(max(1, n_own) * self.band_elems, dtype=dtype, device=device)
             self._halo = _RawCudaBuffer(max(1, len(self.halo_bands)) * self.band_elems * self.es)
-            self._xout = _RawCudaBuffer(N * C * sh.H * W * 4)
+            self._xout = _RawCudaBuffer(N * C * sh.H * W * self.xes)
             self.flags_tiles, self.flags_x = _PeerFlags(device, group), _PeerFlags(device, group)
             torch.cuda.synchronize(device)
         mine = [self._halo.handle(), self._xout.handle(), self.flags_tiles.handle(), self.flags_x.handle(), self.halo_bands]
@@ -518,7 +526,7 @@ class StripExchange:
                 self._opened.append(p.value)
         self.flags_tiles.open([e[2] for e in everyone])
         self.flags_x.open([e[3] for e in everyone])
-        self.x_out = self._xout.tensor(device).view(torch.float32).view(N, C, sh.H, W)
+        self.x_out = self._xout.tensor(device).view(latent_dtype).view(N, C, sh.H, W)
         self._side, self._join = None, None
         self.flags_tiles.set_expect(_cabi.TD_PUSH_CTAS)      # the first step's blend waits for ONE push of each sender
         self._tile_wait, self._x_wait = sh.wait_range("tiles"), sh.wait_range("x")
@@ -604,6 +612,23 @@ class StripExchange:
                                                    _cabi.current_stream_ptr(self.device)))
         return self.x_out
 
+    def blend_mixture(self, g, tile_weights: torch.Tensor, rescale: torch.Tensor, flags: int = 0,
+                      x_buffer: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Mixture of Diffusers: the gaussian blend of this rank's strip (waits in-kernel for the tile halos) into its
+        IPC-mapped latent buffer, or into `x_buffer` ([N, C, H, W] of the latent dtype) instead when regions are composited
+        over the strip next.  Returns the buffer written."""
+        from . import engine
+        sh = self.shard
+        lo, hi = sh.strip()
+        out = x_buffer if x_buffer is not None else self.x_out
+        if hi <= lo:                       # this rank owns no canvas rows (more ranks than tile rows)
+            return out
+        if not hasattr(self, "_ptr_table"):
+            self._ptr_table = self.band_pointer_table()
+        own = (sh.band_begin[sh.rank], sh.band_end[sh.rank]) if _LATE_WAIT else (0, 0)
+        return engine.blend_mixture_rows(g, list(self._ptr_table), self.N, self.C, self.dtype, tile_weights, rescale, out, lo, hi,
+                                         wait=self.flags_tiles.wait_args(*self._tile_wait), own_bands=own, flags=flags)
+
     def join_side(self):
         """The caller's stream waits for the side-stream tile-halo push of this step (no-op when there is none)."""
         if self._join is not None:
@@ -616,14 +641,12 @@ class StripExchange:
         one I send no rows to (StripShard.push_targets)."""
         sh = self.shard
         regions = []
-        plane = sh.H * self.W * 4
+        row = self.W * self.xes
+        plane = sh.H * row
         for (p, a, b) in sh.x_out():
-            off = a * self.W * 4
-            regions.append((self._xout.ptr + off, self.peer_xout[p] + off, self.N * self.C, 1, (b - a) * self.W * 4, plane, plane, plane, plane))
+            regions.append((self._xout.ptr + a * row, self.peer_xout[p] + a * row, self.N * self.C, 1, (b - a) * row, plane, plane, plane, plane))
         first, count = self._x_wait
         self.join_side()
-        if not self._aligned(regions):
-            raise ValueError("row-strip shard: latent width must be a multiple of 4 elements")
         self.flags_x.push(regions, self._x_targets, first, count, bump_own=True, bump_next=self.flags_tiles.counter_ptr)
 
     def gather_latent(self, x: torch.Tensor) -> torch.Tensor:

@@ -310,14 +310,19 @@ class AbstractDiffusion:
         return self._strip_exchange.gather_latent(x)
 
     def _strip_step(self, outs, x: Tensor, N: int, C: int, regions_done=None) -> Tensor:
-        """Strip-shard tail of MultiDiffusion.sample_one_step: own tile outputs -> halo push -> strip blend (-> region composite
-        of the own rows over the blend's accumulator) -> latent halo."""
+        """Strip-shard tail of a sharded step (MultiDiffusion and Mixture of Diffusers): own tile outputs -> halo push -> strip
+        blend (`_strip_blend`; with regions into the accumulator x_buffer) -> region composite of the own rows -> latent halo.
+        Returns the exchange's latent buffer, valid on the strip and its latent halo."""
         from .. import parallel
         g = self._grid
         if self._strip_exchange is None:
-            self._strip_exchange = parallel.StripExchange(self._strip, N, C, g.tile_w, g.W, x.dtype, x.device, self._shard_group)
+            self._strip_exchange = parallel.StripExchange(self._strip, N, C, g.tile_w, g.W, x.dtype, x.device, self._shard_group,
+                                                          latent_dtype=self._strip_latent_dtype(x.dtype))
         ex = self._strip_exchange
+        if ex.N != N or ex.dtype != x.dtype:
+            raise ValueError(f"row-strip shard: the exchange was built for N={ex.N}, {ex.dtype}; this step has N={N}, {x.dtype}")
         lo, hi = self._strip.strip()
+        x_out = ex.x_out
         if self.enable_grid_bbox:
             own = ex.own_tiles()
             off = 0
@@ -325,16 +330,34 @@ class AbstractDiffusion:
                 own[off:off + o.shape[0]].copy_(o)
                 off += o.shape[0]
             ex.push_tile_halos()
-            x_out = ex.blend(g, self.weights, self._rcp_weights if x.dtype != torch.float32 else None, flags=self._blend_flags,
-                             x_buffer=self.x_buffer if regions_done is not None else None)
+            self._strip_blend(ex, x, self.x_buffer if regions_done is not None else None)
         else:
             # draw_background=False: no grid pass, the regions paint over zeros (the tile halos are not exchanged at all)
-            x_out = ex.x_out
             self.x_buffer[:, :, lo:hi].zero_()
         if regions_done is not None:
-            self._composite_regions(self.x_buffer, self.weights, regions_done, rows=(lo, hi), out=x_out)
+            weights, background_aux = self._region_composite_terms()
+            if x_out.dtype == torch.float32:
+                self._composite_regions(self.x_buffer, weights, regions_done, background_aux, rows=(lo, hi), out=x_out)
+            else:        # the composite writes fp32; BACKGROUND-only results are values of the latent dtype (lossless copy)
+                if getattr(self, "_strip_composite_f32", None) is None or self._strip_composite_f32.shape != x_out.shape:
+                    self._strip_composite_f32 = torch.empty(x_out.shape, dtype=torch.float32, device=x_out.device)
+                f32 = self._composite_regions(self.x_buffer, weights, regions_done, background_aux, rows=(lo, hi),
+                                              out=self._strip_composite_f32)
+                x_out[:, :, lo:hi].copy_(f32[:, :, lo:hi])
         ex.push_x_halos_and_wait()
         return x_out
+
+    def _strip_latent_dtype(self, x_dtype: torch.dtype) -> torch.dtype:
+        """Dtype of the latent a strip step returns (and of the exchange's latent buffer)."""
+        raise NotImplementedError(f"{self.method} has no row-strip shard")
+
+    def _strip_blend(self, ex, x: Tensor, x_buffer: Optional[Tensor]):
+        """Blend this rank's strip (the exchange's latent buffer; with `x_buffer` also / instead the accumulator there)."""
+        raise NotImplementedError(f"{self.method} has no row-strip shard")
+
+    def _region_composite_terms(self):
+        """(weights, background_aux) of `_composite_regions` for this method."""
+        raise NotImplementedError(f"{self.method} has no region composite")
 
     def _region_pass_sharded(self, x: Tensor, custom_func: Callable, poll_interrupt: bool, interrupted: bool):
         """`_custom_region_pass` under the tile shard: this rank denoises its regions (parallel.RegionShard: region j on rank

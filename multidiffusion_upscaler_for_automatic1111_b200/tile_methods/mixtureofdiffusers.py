@@ -9,7 +9,7 @@ roundings, so results are bit-identical to the reference.
 """
 from __future__ import annotations
 
-from typing import List
+from typing import List, Optional
 
 import torch
 from torch import Tensor
@@ -17,6 +17,8 @@ from torch import Tensor
 from .. import engine, host
 from ..tile_utils.utils import BBox, BlendMode, Condition, CustomBBox, custom_bbox, gaussian_weights, grid_bbox, keep_signature
 from .abstractdiffusion import AbstractDiffusion, CondDict
+
+_STRIP_NO_INVERSION = "the row-strip shard of Mixture of Diffusers does not run tiled noise inversion: use mode='replicate'"
 
 
 class MixtureOfDiffusers(AbstractDiffusion):
@@ -89,6 +91,21 @@ class MixtureOfDiffusers(AbstractDiffusion):
         x = self._check_input(x_in)
         self.reset_buffer(x)
         regions = self.enable_custom_bbox and len(self.custom_bboxes) > 0
+
+        def custom_func(x_tile: Tensor, bbox_id: int, bbox: CustomBBox) -> Tensor:
+            if noise_inverse_step < 0:
+                return self.custom_apply_model(x_tile, t_in, c_in, bbox_id, bbox)
+            tcond = Condition.reconstruct_cond(bbox.cond, noise_inverse_step)
+            icond = self.get_icond(c_in)
+            if tuple(icond.shape[2:]) == (self.h, self.w):
+                icond = icond[bbox.slicer]
+            c_out = self.make_cond_dict(c_in, tcond, icond, self.get_vcond(c_in))
+            return sd_model.apply_model(x_tile, t_in, cond=c_out)
+
+        if self._strip is not None:
+            if noise_inverse_step >= 0:
+                raise NotImplementedError(_STRIP_NO_INVERSION)
+            return self._apply_strip(x_in, x, t_in, c_in, sd_model, N, C, custom_func if regions else None)
         interrupted = False
 
         if self.enable_grid_bbox:
@@ -102,16 +119,6 @@ class MixtureOfDiffusers(AbstractDiffusion):
             self.x_buffer.zero_()
         if not regions:
             return self.x_buffer
-
-        def custom_func(x_tile: Tensor, bbox_id: int, bbox: CustomBBox) -> Tensor:
-            if noise_inverse_step < 0:
-                return self.custom_apply_model(x_tile, t_in, c_in, bbox_id, bbox)
-            tcond = Condition.reconstruct_cond(bbox.cond, noise_inverse_step)
-            icond = self.get_icond(c_in)
-            if tuple(icond.shape[2:]) == (self.h, self.w):
-                icond = icond[bbox.slicer]
-            c_out = self.make_cond_dict(c_in, tcond, icond, self.get_vcond(c_in))
-            return sd_model.apply_model(x_tile, t_in, cond=c_out)
 
         if self._shard is not None:
             done, interrupted = self._region_pass_sharded(x, custom_func, False, interrupted)
@@ -148,10 +155,7 @@ class MixtureOfDiffusers(AbstractDiffusion):
     def _grid_pass(self, x_in: Tensor, x: Tensor, t_in: Tensor, c_in: CondDict, sd_model, N: int, C: int):
         """Grid tiles of one UNet call: scatter, denoise per batch, fused gaussian blend into x_buffer.
         Returns x_buffer, or None when the job was interrupted."""
-        if self.rescale_factor.device != x.device:
-            self.rescale_factor = self.rescale_factor.to(x.device)
-        if self.tile_weights.device != x.device:
-            self.tile_weights = self.tile_weights.to(x.device)
+        self._blend_inputs_to(x.device)
         if self._shard is not None:
             return self._grid_pass_sharded(x, t_in, c_in, sd_model, N, C)
 
@@ -176,12 +180,16 @@ class MixtureOfDiffusers(AbstractDiffusion):
         return engine.blend_mixture(self._grid, outs, N, C, self.tile_bs, self.tile_weights, self.rescale_factor,
                                     self.x_buffer, flags=self._blend_flags)
 
-    def _grid_pass_sharded(self, x: Tensor, t_in: Tensor, c_in: CondDict, sd_model, N: int, C: int):
-        """Tile shard (init_tile_shard): this rank denoises its contiguous chunk of the tile list, the eps tiles are
-        all-gathered, and every rank runs the same ordered gaussian blend over all tiles -- bit-identical to the
-        single-GPU result on every rank.  An interrupted rank stops its denoiser calls but still joins the all-gather
-        (placeholder tiles) so that the collectives stay in lock-step, then returns None."""
-        from .. import parallel
+    def _blend_inputs_to(self, device):
+        if self.rescale_factor.device != device:
+            self.rescale_factor = self.rescale_factor.to(device)
+        if self.tile_weights.device != device:
+            self.tile_weights = self.tile_weights.to(device)
+
+    def _denoise_local_tiles(self, x: Tensor, t_in: Tensor, c_in: CondDict, sd_model, N: int):
+        """Tile shard: scatter and denoise this rank's tiles `[shard.begin, shard.end)`.  An interrupted rank stops its
+        denoiser calls but keeps placeholder outputs (its inputs) so that the exchange still happens.
+        Returns (outputs per local batch, interrupted)."""
         sh, g = self._shard, self._grid
         outs = []
         interrupted = False
@@ -205,6 +213,16 @@ class MixtureOfDiffusers(AbstractDiffusion):
                     continue
                 outs.append(self._denoise_tile_batch(sd_model, x_tile, n_rep, t_in, c_in, icond_tile, batch_id, N))
                 self.update_pbar()
+        return outs, interrupted
+
+    def _grid_pass_sharded(self, x: Tensor, t_in: Tensor, c_in: CondDict, sd_model, N: int, C: int):
+        """Tile shard (init_tile_shard): this rank denoises its contiguous chunk of the tile list, the eps tiles are
+        all-gathered, and every rank runs the same ordered gaussian blend over all tiles -- bit-identical to the
+        single-GPU result on every rank.  An interrupted rank stops its denoiser calls but still joins the all-gather
+        (placeholder tiles) so that the collectives stay in lock-step, then returns None."""
+        from .. import parallel
+        sh, g = self._shard, self._grid
+        outs, interrupted = self._denoise_local_tiles(x, t_in, c_in, sd_model, N)
         dt = outs[0].dtype if outs else x.dtype
         local = torch.zeros((sh.chunk * N, C, g.tile_h, g.tile_w), dtype=dt, device=x.device)
         if outs:
@@ -217,6 +235,41 @@ class MixtureOfDiffusers(AbstractDiffusion):
         x_out = engine.blend_mixture(g, chunks, N, C, sh.chunk, self.tile_weights, self.rescale_factor, self.x_buffer,
                                      flags=self._blend_flags)
         return None if interrupted else x_out
+
+    # ------------------------------------------------------------------ row-strip shard
+    def init_tile_shard(self, group=None, fused: bool = True, mode: Optional[str] = None):
+        """AbstractDiffusion.init_tile_shard; the default stays "replicate".  mode="strip": rank r denoises a run of tile rows
+        and blends only its own canvas rows (row-window gaussian blend), exchanging only the overlapping tile rows and the
+        latent halo -- bit-identical to one GPU.  Not with tiled noise inversion."""
+        if mode == "strip" and self.noise_inverse_enabled:
+            raise NotImplementedError(_STRIP_NO_INVERSION)
+        return super().init_tile_shard(group, fused, mode)
+
+    def _apply_strip(self, x_in: Tensor, x: Tensor, t_in: Tensor, c_in: CondDict, sd_model, N: int, C: int, custom_func):
+        """One UNet call under the row-strip shard: this rank's tiles (`x` is valid on its strip plus latent halo), its custom
+        regions, then the strip tail (`_strip_step`).  An interrupted rank still publishes, blends and signals (placeholder
+        tiles), so the flag counters stay in lock-step, and then returns x_in."""
+        outs, interrupted = [], False
+        if self.enable_grid_bbox:
+            self._blend_inputs_to(x.device)
+            outs, interrupted = self._denoise_local_tiles(x, t_in, c_in, sd_model, N)
+        done = None
+        if custom_func is not None:
+            # the region exchange (NCCL) comes before the tile exchange: its in-kernel waits then never sit in front of a collective
+            done, interrupted = self._region_pass_sharded(x, custom_func, False, interrupted)
+        out = self._strip_step(outs, x, N, C, done)
+        return x_in if interrupted else out
+
+    def _strip_latent_dtype(self, x_dtype: torch.dtype) -> torch.dtype:
+        # the reference's feather overlay promotes to fp32 (fp32 mask, mixtureofdiffusers.py:124-128)
+        fg = self.enable_custom_bbox and any(b.blend_mode == BlendMode.FOREGROUND for b in self.custom_bboxes)
+        return torch.float32 if fg else x_dtype
+
+    def _strip_blend(self, ex, x: Tensor, x_buffer: Optional[Tensor]):
+        ex.blend_mixture(self._grid, self.tile_weights, self.rescale_factor, flags=self._blend_flags, x_buffer=x_buffer)
+
+    def _region_composite_terms(self):
+        return None, lambda bbox_id: self.custom_weights[bbox_id]
 
     def custom_apply_model(self, x_in: Tensor, t_in: Tensor, c_in: CondDict, bbox_id: int, bbox: CustomBBox) -> Tensor:
         """mixtureofdiffusers.py:181-196: a region goes through the un-hijacked `apply_model` with its own prompts."""

@@ -232,6 +232,15 @@ class MultiDiffusion(AbstractDiffusion):
             out = self._composite_regions(self.x_buffer, self.weights, done)
         return x_in if interrupted else out
 
+    def _strip_latent_dtype(self, x_dtype: torch.dtype) -> torch.dtype:
+        return torch.float32            # the normalising divide (multidiffusion.py:208) is fp32
+
+    def _strip_blend(self, ex, x: Tensor, x_buffer: Optional[Tensor]):
+        ex.blend(self._grid, self.weights, self._rcp_weights if x.dtype != torch.float32 else None, flags=self._blend_flags, x_buffer=x_buffer)
+
+    def _region_composite_terms(self):
+        return self.weights, None
+
     def get_noise(self, x_in: Tensor, sigma_in: Tensor, cond_in: CondDict, step: int) -> Tensor:
         """Tiled eps prediction used by noise inversion (multidiffusion.py:220-243)."""
         from ..tile_utils.utils import Condition
