@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define TD_ABI_VERSION 11
+#define TD_ABI_VERSION 12
 
 typedef enum td_status {
     TD_OK = 0,
@@ -283,6 +283,22 @@ int td_blend_mixture_rows(const td_grid* g, const void* const* batch_ptrs, int n
                           const float* rescale, void* x_buffer, int row_begin, int row_end,
                           const uint32_t* wait_flags, int wait_count, const uint32_t* wait_value,
                           int own_band_begin, int own_band_end, uint32_t flags, void* stream);
+/* Row-strip tile shard on a periodic plan (g->wrap != 0, seamless tiling): td_blend_multidiffusion / td_blend_mixture of the
+ * canvas rows [row_begin, row_end) only, with the per-tile-row batch_ptrs (tile_bs = cols), the in-kernel halo wait and the
+ * own bands of td_blend_multidiffusion_rows.  Coverage is modular: under TD_WRAP_Y a row near the top of the canvas is also
+ * covered by the last tile row(s), and a CTA waits when any of its rows is covered by a tile row outside the own bands.
+ * wait_flags[0 .. wait_count) may run past the world size (mirrored flag slots), never past TD_MAX_PEERS entries.  Same
+ * arithmetic and tile order as the whole-canvas wrap blend: every row gets its bits.  Needs the vector path (tile_dtype ==
+ * acc_dtype, W and tile_w multiples of the vector, 16-byte aligned buffers), else TD_ERR_UNSUPPORTED; a bounded plan
+ * (wrap == 0) returns TD_ERR_UNSUPPORTED (it takes the rows entries above).  An empty window launches nothing. */
+int td_blend_multidiffusion_wrap_rows(const td_grid* g, const void* const* batch_ptrs, int num_batches, int tile_bs, int N, int C,
+                                      int tile_dtype, int acc_dtype, const float* weights, float* x_out, void* x_buffer,
+                                      int row_begin, int row_end, const uint32_t* wait_flags, int wait_count,
+                                      const uint32_t* wait_value, int own_band_begin, int own_band_end, uint32_t flags, void* stream);
+int td_blend_mixture_wrap_rows(const td_grid* g, const void* const* batch_ptrs, int num_batches, int tile_bs, int N, int C,
+                               int tile_dtype, int acc_dtype, const float* tile_weights, const float* rescale, void* x_buffer,
+                               int row_begin, int row_end, const uint32_t* wait_flags, int wait_count, const uint32_t* wait_value,
+                               int own_band_begin, int own_band_end, uint32_t flags, void* stream);
 /* One warp spins (acquire, system scope, bounded) until flags[i] >= *value for i < count: stream-ordered work after it
  * sees what the signalling ranks wrote before their td_peer_signal. */
 int td_peer_wait(const uint32_t* flags, int count, const uint32_t* value, void* stream);

@@ -33,7 +33,7 @@ TD_MAX_GRID_DIM = 256
 TD_MAX_BATCH_PTRS = 128
 TD_MAX_PEERS = 16
 TD_IPC_HANDLE_BYTES = 64
-ABI_VERSION = 11
+ABI_VERSION = 12
 
 DTYPE_CODE = {torch.float16: TD_F16, torch.bfloat16: TD_BF16, torch.float32: TD_F32}
 
@@ -131,6 +131,12 @@ _SIGNATURES = {
     "td_blend_mixture_rows": (c_int, [POINTER(TdGrid), POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_int,
                                       c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_int,
                                       c_uint32, c_void_p]),
+    "td_blend_multidiffusion_wrap_rows": (c_int, [POINTER(TdGrid), POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_int,
+                                                  c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_int,
+                                                  c_uint32, c_void_p]),
+    "td_blend_mixture_wrap_rows": (c_int, [POINTER(TdGrid), POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_int,
+                                           c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_int,
+                                           c_uint32, c_void_p]),
     "td_peer_wait": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
     "td_push_regions": (c_int, [POINTER(TdPushRegion), c_int, POINTER(c_void_p), c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     "td_region_composite": (c_int, [c_void_p, c_void_p, POINTER(TdRegion), c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),

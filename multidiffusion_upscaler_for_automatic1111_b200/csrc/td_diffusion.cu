@@ -1635,7 +1635,7 @@ extern "C" int td_blend_multidiffusion(const td_grid* g, const void* const* batc
 // launch), or a td_status.
 static int setup_rows_window(const td_grid* g, BlendParams* bp, const char* what, int tile_dtype, int acc_dtype,
                              std::initializer_list<const void*> ptrs, int row_begin, int row_end, const uint32_t* wait_flags,
-                             int wait_count, const uint32_t* wait_value, int own_band_begin, int own_band_end) {
+                             int wait_count, const uint32_t* wait_value, int own_band_begin, int own_band_end, int patch_rows = kAsY) {
     if (row_begin < 0 || row_end > g->H || row_begin > row_end || row_begin % 8 != 0 || (row_end % 8 != 0 && row_end != g->H)) {
         td_set_error("%s: rows [%d,%d) must lie in [0,%d) on multiples of 8", what, row_begin, row_end, g->H);
         return TD_ERR_INVALID_ARG;
@@ -1649,9 +1649,9 @@ static int setup_rows_window(const td_grid* g, BlendParams* bp, const char* what
         td_set_error("%s: needs the vector path (same tile / canvas dtype, W and tile_w multiples of the vector, 16-byte aligned buffers)", what);
         return TD_ERR_UNSUPPORTED;
     }
-    // the window is cut into whole patch rows of the cp.async kernel (kAsY rows, a build-time knob; 8 by default)
-    if (row_begin % kAsY != 0 || (row_end % kAsY != 0 && row_end != g->H)) {
-        td_set_error("%s: rows [%d,%d) are not aligned to the %d-row patches of this build", what, row_begin, row_end, kAsY);
+    // the window is cut into whole patch rows of the kernel (cp.async: kAsY rows, a build-time knob; 8 by default)
+    if (row_begin % patch_rows != 0 || (row_end % patch_rows != 0 && row_end != g->H)) {
+        td_set_error("%s: rows [%d,%d) are not aligned to the %d-row patches of this build", what, row_begin, row_end, patch_rows);
         return TD_ERR_UNSUPPORTED;
     }
     bp->py0 = row_begin / kAsY;
@@ -1807,4 +1807,52 @@ extern "C" int td_blend_mixture_rows(const td_grid* g, const void* const* batch_
     }
     if (rc == 1) { td_set_error("td_blend_mixture_rows: geometry outside the cp.async kernel's limits"); return TD_ERR_UNSUPPORTED; }
     return rc;
+}
+
+// Row-strip shard on a periodic canvas (td_wrap.cu): the windowed wrap blends, validated as the rows entries above.  A bounded
+// plan keeps td_blend_*_rows.
+static int wrap_rows_entry(const td_grid* g, const void* const* batch_ptrs, int num_batches, int tile_bs, int N, int C, int tile_dtype,
+                           int acc_dtype, int mixture, const float* weights, const float* tile_weights, const float* rescale, float* x_out,
+                           void* x_buffer, int row_begin, int row_end, const uint32_t* wait_flags, int wait_count,
+                           const uint32_t* wait_value, int own_band_begin, int own_band_end, uint32_t flags, void* stream, const char* what) {
+    BlendParams bp;
+    tl_pdl = !(flags & TD_FLAG_NO_PDL);
+    int st = fill_blend(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, &bp);
+    if (st != TD_OK) return st;
+    if (g->wrap == 0) {
+        td_set_error("%s: a bounded plan (wrap=0) takes td_blend_%s_rows", what, mixture ? "mixture" : "multidiffusion");
+        return TD_ERR_UNSUPPORTED;
+    }
+    if (mixture ? (tile_weights == nullptr || rescale == nullptr || x_buffer == nullptr) : (weights == nullptr || x_out == nullptr)) {
+        td_set_error("%s: null %s", what, mixture ? "tile_weights / rescale / x_buffer" : "weights / x_out");
+        return TD_ERR_INVALID_ARG;
+    }
+    // the wrap blend's CTAs cover 4 canvas rows: any window on multiples of 8 is whole CTA rows
+    st = mixture ? setup_rows_window(g, &bp, what, tile_dtype, acc_dtype, {rescale, x_buffer}, row_begin, row_end, wait_flags, wait_count,
+                                     wait_value, own_band_begin, own_band_end, 8)
+                 : setup_rows_window(g, &bp, what, tile_dtype, acc_dtype, {weights, x_out, x_buffer}, row_begin, row_end, wait_flags,
+                                     wait_count, wait_value, own_band_begin, own_band_end, 8);
+    if (st != TD_OK) return st == 1 ? TD_OK : st;
+    return td_wrap_blend_rows(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, mixture, weights, tile_weights, rescale, x_out, x_buffer,
+                              row_begin, row_end, wait_count > 0 ? wait_flags : nullptr, wait_count, wait_value, own_band_begin,
+                              own_band_end, tl_pdl, stream);
+}
+
+extern "C" int td_blend_multidiffusion_wrap_rows(const td_grid* g, const void* const* batch_ptrs, int num_batches, int tile_bs, int N, int C,
+                                                 int tile_dtype, int acc_dtype, const float* weights, float* x_out, void* x_buffer,
+                                                 int row_begin, int row_end, const uint32_t* wait_flags, int wait_count,
+                                                 const uint32_t* wait_value, int own_band_begin, int own_band_end, uint32_t flags,
+                                                 void* stream) {
+    return wrap_rows_entry(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, 0, weights, nullptr, nullptr, x_out, x_buffer,
+                           row_begin, row_end, wait_flags, wait_count, wait_value, own_band_begin, own_band_end, flags, stream,
+                           "td_blend_multidiffusion_wrap_rows");
+}
+
+extern "C" int td_blend_mixture_wrap_rows(const td_grid* g, const void* const* batch_ptrs, int num_batches, int tile_bs, int N, int C,
+                                          int tile_dtype, int acc_dtype, const float* tile_weights, const float* rescale, void* x_buffer,
+                                          int row_begin, int row_end, const uint32_t* wait_flags, int wait_count, const uint32_t* wait_value,
+                                          int own_band_begin, int own_band_end, uint32_t flags, void* stream) {
+    return wrap_rows_entry(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, 1, nullptr, tile_weights, rescale, nullptr,
+                           x_buffer, row_begin, row_end, wait_flags, wait_count, wait_value, own_band_begin, own_band_end, flags, stream,
+                           "td_blend_mixture_wrap_rows");
 }

@@ -31,3 +31,9 @@ int td_wrap_scatter(const struct td_grid* g, const void* x, void* tiles, int N, 
 int td_wrap_blend(const struct td_grid* g, const void* const* batch_ptrs, int num_batches, int tile_bs, int N, int C, int tile_dtype,
                   int acc_dtype, int mixture, const float* weights, const float* tile_weights, const float* rescale, float* x_out,
                   void* x_buffer, bool vec, bool pdl, void* stream);
+// Row-strip shard on a periodic canvas (td_blend_*_wrap_rows, vector path only, arguments validated by the caller): the blend
+// of the canvas rows [row_begin, row_end) (non-empty), waiting in-kernel for the halo bands.
+int td_wrap_blend_rows(const struct td_grid* g, const void* const* batch_ptrs, int num_batches, int tile_bs, int N, int C, int tile_dtype,
+                       int mixture, const float* weights, const float* tile_weights, const float* rescale, float* x_out, void* x_buffer,
+                       int row_begin, int row_end, const uint32_t* wait_flags, int wait_count, const uint32_t* wait_value,
+                       int own_band_begin, int own_band_end, bool pdl, void* stream);

@@ -139,6 +139,20 @@ wrap_scatter_generic_kernel(const __grid_constant__ WrapParams p, const T* __res
 // ---------------------------------------------------------------------------
 constexpr int kWrapBX = 32, kWrapBY = 4;
 
+// Row-window form (td_blend_*_wrap_rows, row-strip shard): the grid covers the canvas rows [row_begin, row_end) only, with
+// blockIdx.z = CTA row (slowest, walked from the window's end when `descending`) and blockIdx.y = plane.  A CTA any of whose
+// rows is covered by a tile row outside the own bands [own_lo, own_hi) (every CTA when that range is empty) first waits
+// until wait_flags[i] >= *wait_value for i < wait_count: its tile reads may come from a neighbour's halo push.
+struct WindowParams {
+    int row_begin, row_end, rb_count, descending;
+    int wait_count, own_lo, own_hi;
+    const uint32_t* wait_flags;
+    const uint32_t* wait_value;
+};
+
+// a non-empty index range [s, s + n) of tile rows that is not inside the own bands
+__device__ __forceinline__ bool leaves_own(const WindowParams& w, int s, int n) { return n > 0 && (s < w.own_lo || s + n > w.own_hi); }
+
 template <typename T, int MODE>
 struct VisitAcc {
     static constexpr int VEC = Vec<T>::kElems;
@@ -162,10 +176,11 @@ struct VisitAcc {
     }
 };
 
-template <typename T, int MODE, bool WRITE_BUF>
+template <typename T, int MODE, bool WRITE_BUF, bool WINDOW>
 __global__ void __launch_bounds__(kWrapBX * kWrapBY)
 wrap_blend_vec_kernel(const __grid_constant__ WrapParams p, const float* __restrict__ weights, const float* __restrict__ tile_weights,
-                      const float* __restrict__ rescale, float* __restrict__ out_f32, T* __restrict__ out_buf) {
+                      const float* __restrict__ rescale, float* __restrict__ out_f32, T* __restrict__ out_buf,
+                      const __grid_constant__ WindowParams w) {
     constexpr int VEC = Vec<T>::kElems;
     constexpr int L2V = Vec<T>::kLog2;
     __shared__ short s_ys[TD_MAX_GRID_DIM];
@@ -173,16 +188,33 @@ wrap_blend_vec_kernel(const __grid_constant__ WrapParams p, const float* __restr
     load_origins(p, s_ys, s_xs);
     pdl_launch_dependents();
     const int xv = blockIdx.x * kWrapBX + threadIdx.x;
-    const int y = blockIdx.y * kWrapBY + threadIdx.y;
-    const int plane = blockIdx.z;
+    const int y = WINDOW ? w.row_begin + (w.descending ? w.rb_count - 1 - (int)blockIdx.z : (int)blockIdx.z) * kWrapBY + (int)threadIdx.y
+                         : (int)(blockIdx.y * kWrapBY + threadIdx.y);
+    const int plane = WINDOW ? blockIdx.y : blockIdx.z;
     const int x = xv * VEC;
-    const bool live = x < p.W && y < p.H;
+    const bool live = x < p.W && y < (WINDOW ? w.row_end : p.H);
     Cover cy{0, 0, 0, 0}, cx{0, 0, 0, 0};
     if (live) {
         cy = cover(s_ys, p.rows, y, y, p.th, p.H, p.wrap_y, p.inv_dy);
         cx = cover(s_xs, p.cols, x, x + VEC - 1, p.tw, p.W, p.wrap_x, p.inv_dx);
     }
     pdl_wait();
+    if constexpr (WINDOW) {
+        // both index ranges of the row cover: under wrap_y a row near the top is covered by band 0 AND by the last band(s)
+        const bool foreign = live && (leaves_own(w, cy.a0, cy.na) || leaves_own(w, cy.b0, cy.n - cy.na));
+        if (w.wait_count > 0 && __syncthreads_or(foreign)) {
+            if (threadIdx.y == 0 && (int)threadIdx.x < w.wait_count) {
+                const uint32_t want = *w.wait_value;
+                uint32_t v;
+                unsigned long long spins = 0;
+                do {   // bounded: a peer that never signals becomes a launch error, not a hung GPU
+                    asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(w.wait_flags + threadIdx.x) : "memory");
+                    if (++spins > (1ull << 31)) __trap();
+                } while ((int32_t)(v - want) < 0);
+            }
+            __syncthreads();   // publishes the acquire to the CTA before any tile read
+        }
+    }
     if (!live) return;
     const long long pix = (long long)y * p.W + x;
     float acc[VEC];
@@ -345,17 +377,51 @@ int scatter_impl(const WrapParams& p, const void* x, void* tiles, int tile_begin
     return check("td_scatter_tiles (wrap)");
 }
 
+// `win` null: the whole canvas; else its row window (rb_count > 0)
 template <typename T, int MODE>
 int blend_vec_impl(const WrapParams& p, const float* weights, const float* tile_weights, const float* rescale, float* out_f32,
-                   void* out_buf, bool pdl, cudaStream_t st) {
+                   void* out_buf, const WindowParams* win, bool pdl, cudaStream_t st) {
     const int wv = p.W / Vec<T>::kElems;
-    dim3 grid((unsigned)((wv + kWrapBX - 1) / kWrapBX), (unsigned)((p.H + kWrapBY - 1) / kWrapBY), (unsigned)(p.N * p.C));
+    const unsigned gx = (unsigned)((wv + kWrapBX - 1) / kWrapBX), planes = (unsigned)(p.N * p.C);
+    const dim3 grid = win ? dim3(gx, planes, (unsigned)win->rb_count) : dim3(gx, (unsigned)((p.H + kWrapBY - 1) / kWrapBY), planes);
     if (grid.y > 65535u || grid.z > 65535u) { td_set_error("canvas too large for the wrap blend grid"); return TD_ERR_UNSUPPORTED; }
-    if (MODE == MODE_MOD || out_buf != nullptr)
-        launch(pdl, wrap_blend_vec_kernel<T, MODE, true>, grid, dim3(kWrapBX, kWrapBY), st, p, weights, tile_weights, rescale, out_f32, (T*)out_buf);
-    else
-        launch(pdl, wrap_blend_vec_kernel<T, MODE, false>, grid, dim3(kWrapBX, kWrapBY), st, p, weights, tile_weights, rescale, out_f32, (T*)out_buf);
+    const dim3 block(kWrapBX, kWrapBY);
+    const bool buf = MODE == MODE_MOD || out_buf != nullptr;
+    if (win) {
+        if (buf) launch(pdl, wrap_blend_vec_kernel<T, MODE, true, true>, grid, block, st, p, weights, tile_weights, rescale, out_f32, (T*)out_buf, *win);
+        else launch(pdl, wrap_blend_vec_kernel<T, MODE, false, true>, grid, block, st, p, weights, tile_weights, rescale, out_f32, (T*)out_buf, *win);
+        return check("td_blend (wrap, rows)");
+    }
+    const WindowParams whole = {};
+    if (buf) launch(pdl, wrap_blend_vec_kernel<T, MODE, true, false>, grid, block, st, p, weights, tile_weights, rescale, out_f32, (T*)out_buf, whole);
+    else launch(pdl, wrap_blend_vec_kernel<T, MODE, false, false>, grid, block, st, p, weights, tile_weights, rescale, out_f32, (T*)out_buf, whole);
     return check("td_blend (wrap)");
+}
+
+// Does canvas row y lie in a tile row outside the own bands?  (host twin of the kernel's per-CTA wait test)
+bool row_leaves_own(const WrapParams& p, int y, int own_lo, int own_hi) {
+    for (int i = 0; i < p.rows; ++i) {
+        if (i >= own_lo && i < own_hi) continue;
+        int v = y - p.ys[i];
+        if (v < 0 && p.wrap_y) v += p.H;
+        if (v >= 0 && v < p.th) return true;
+    }
+    return false;
+}
+
+// Row-strip shard: the waiting CTAs run last.  The halo enters a strip from its top (a lower rank's bands, or across the
+// seam the last bands of a wrapped canvas), so the window is normally walked from its end; the other way round when the
+// waiting rows sit at its end.
+int window_descending(const WrapParams& p, const WindowParams& w) {
+    if (w.wait_count == 0 || w.own_hi <= w.own_lo) return 0;
+    int first = -1, last = -1;
+    for (int b = 0; b < w.rb_count; ++b) {
+        const int y0 = w.row_begin + b * kWrapBY, y1 = std::min(y0 + kWrapBY, w.row_end);
+        bool waits = false;
+        for (int y = y0; y < y1 && !waits; ++y) waits = row_leaves_own(p, y, w.own_lo, w.own_hi);
+        if (waits) { if (first < 0) first = b; last = b; }
+    }
+    return (first >= 0 && first + last <= w.rb_count - 1) ? 1 : 0;
 }
 
 template <int MODE>
@@ -382,6 +448,22 @@ int blend_generic_impl(int tile_dtype, int acc_dtype, const WrapParams& p, const
     return TD_ERR_INVALID_ARG;
 }
 
+int blend_vec_dispatch(const WrapParams& p, int tile_dtype, int mixture, const float* weights, const float* tile_weights, const float* rescale,
+                       float* x_out, void* x_buffer, const WindowParams* win, bool pdl, cudaStream_t st) {
+    if (mixture) {
+        switch (tile_dtype) {
+            case TD_F16: return blend_vec_impl<__half, MODE_MOD>(p, nullptr, tile_weights, rescale, nullptr, x_buffer, win, pdl, st);
+            case TD_BF16: return blend_vec_impl<__nv_bfloat16, MODE_MOD>(p, nullptr, tile_weights, rescale, nullptr, x_buffer, win, pdl, st);
+            default: return blend_vec_impl<float, MODE_MOD>(p, nullptr, tile_weights, rescale, nullptr, x_buffer, win, pdl, st);
+        }
+    }
+    switch (tile_dtype) {
+        case TD_F16: return blend_vec_impl<__half, MODE_MD>(p, weights, nullptr, nullptr, x_out, x_buffer, win, pdl, st);
+        case TD_BF16: return blend_vec_impl<__nv_bfloat16, MODE_MD>(p, weights, nullptr, nullptr, x_out, x_buffer, win, pdl, st);
+        default: return blend_vec_impl<float, MODE_MD>(p, weights, nullptr, nullptr, x_out, x_buffer, win, pdl, st);
+    }
+}
+
 }  // namespace
 
 int td_wrap_scatter(const td_grid* g, const void* x, void* tiles, int N, int C, int dtype, int tile_begin, int tile_end, bool vec, bool pdl,
@@ -401,20 +483,28 @@ int td_wrap_blend(const td_grid* g, const void* const* batch_ptrs, int num_batch
     p.tile_bs = tile_bs;
     for (int b = 0; b < num_batches; ++b) p.batch_ptrs[b] = batch_ptrs[b];
     cudaStream_t st = (cudaStream_t)stream;
-    if (vec) {
-        if (mixture) {
-            switch (tile_dtype) {
-                case TD_F16: return blend_vec_impl<__half, MODE_MOD>(p, nullptr, tile_weights, rescale, nullptr, x_buffer, pdl, st);
-                case TD_BF16: return blend_vec_impl<__nv_bfloat16, MODE_MOD>(p, nullptr, tile_weights, rescale, nullptr, x_buffer, pdl, st);
-                default: return blend_vec_impl<float, MODE_MOD>(p, nullptr, tile_weights, rescale, nullptr, x_buffer, pdl, st);
-            }
-        }
-        switch (tile_dtype) {
-            case TD_F16: return blend_vec_impl<__half, MODE_MD>(p, weights, nullptr, nullptr, x_out, x_buffer, pdl, st);
-            case TD_BF16: return blend_vec_impl<__nv_bfloat16, MODE_MD>(p, weights, nullptr, nullptr, x_out, x_buffer, pdl, st);
-            default: return blend_vec_impl<float, MODE_MD>(p, weights, nullptr, nullptr, x_out, x_buffer, pdl, st);
-        }
-    }
+    if (vec) return blend_vec_dispatch(p, tile_dtype, mixture, weights, tile_weights, rescale, x_out, x_buffer, nullptr, pdl, st);
     if (mixture) return blend_generic_impl<MODE_MOD>(tile_dtype, acc_dtype, p, nullptr, tile_weights, rescale, nullptr, x_buffer, pdl, st);
     return blend_generic_impl<MODE_MD>(tile_dtype, acc_dtype, p, weights, nullptr, nullptr, x_out, x_buffer, pdl, st);
+}
+
+int td_wrap_blend_rows(const td_grid* g, const void* const* batch_ptrs, int num_batches, int tile_bs, int N, int C, int tile_dtype,
+                       int mixture, const float* weights, const float* tile_weights, const float* rescale, float* x_out, void* x_buffer,
+                       int row_begin, int row_end, const uint32_t* wait_flags, int wait_count, const uint32_t* wait_value,
+                       int own_band_begin, int own_band_end, bool pdl, void* stream) {
+    WrapParams p;
+    fill_params(g, N, C, &p);
+    p.tile_bs = tile_bs;
+    for (int b = 0; b < num_batches; ++b) p.batch_ptrs[b] = batch_ptrs[b];
+    WindowParams w;
+    w.row_begin = row_begin;
+    w.row_end = row_end;
+    w.rb_count = (row_end - row_begin + kWrapBY - 1) / kWrapBY;
+    w.wait_count = wait_flags != nullptr ? wait_count : 0;
+    w.wait_flags = wait_flags;
+    w.wait_value = wait_value;
+    w.own_lo = w.wait_count > 0 ? own_band_begin : 0;   // no wait: the own-band test is never made
+    w.own_hi = w.wait_count > 0 ? own_band_end : 0;
+    w.descending = window_descending(p, w);
+    return blend_vec_dispatch(p, tile_dtype, mixture, weights, tile_weights, rescale, x_out, x_buffer, &w, pdl, (cudaStream_t)stream);
 }

@@ -187,6 +187,40 @@ def blend_mixture_rows(g: TdGrid, band_ptrs: Sequence[int], N: int, C: int, tile
     return x_buffer
 
 
+def blend_multidiffusion_wrap_rows(g: TdGrid, band_ptrs: Sequence[int], N: int, C: int, tile_dtype: torch.dtype, weights: torch.Tensor,
+                                   x_out: torch.Tensor, row_begin: int, row_end: int, x_buffer: Optional[torch.Tensor] = None,
+                                   wait=None, own_bands=(0, 0), flags: int = 0, tile_bs: Optional[int] = None) -> torch.Tensor:
+    """`blend_multidiffusion` of the canvas rows [row_begin, row_end) of a periodic plan (g.wrap != 0) into those rows of the
+    fp32 x_out (and of x_buffer, the tile dtype, when given); returns x_out.  band_ptrs / wait / own_bands as in
+    `blend_mixture_rows`; `tile_bs` (default g.cols: one pointer per tile row) for another pointer table
+    (td_blend_multidiffusion_wrap_rows)."""
+    _require_cuda(x_out, "x_out")
+    fptr, count, vptr = wait if wait is not None else (None, 0, None)
+    ptrs = (ctypes.c_void_p * len(band_ptrs))(*band_ptrs)
+    with torch.cuda.device(x_out.device):
+        check(lib.td_blend_multidiffusion_wrap_rows(ctypes.byref(g), ptrs, len(band_ptrs), int(g.cols if tile_bs is None else tile_bs), N, C,
+                                                    dtype_code(tile_dtype), dtype_code(tile_dtype), weights.data_ptr(), x_out.data_ptr(),
+                                                    x_buffer.data_ptr() if x_buffer is not None else None, int(row_begin), int(row_end),
+                                                    fptr if count else None, int(count), vptr if count else None, int(own_bands[0]),
+                                                    int(own_bands[1]), int(flags), current_stream_ptr(x_out.device)))
+    return x_out
+
+
+def blend_mixture_wrap_rows(g: TdGrid, band_ptrs: Sequence[int], N: int, C: int, tile_dtype: torch.dtype, tile_weights: torch.Tensor,
+                            rescale: torch.Tensor, x_buffer: torch.Tensor, row_begin: int, row_end: int, wait=None,
+                            own_bands=(0, 0), flags: int = 0) -> torch.Tensor:
+    """`blend_mixture_rows` on a periodic plan (g.wrap != 0): td_blend_mixture_wrap_rows."""
+    _require_cuda(x_buffer, "x_buffer")
+    fptr, count, vptr = wait if wait is not None else (None, 0, None)
+    ptrs = (ctypes.c_void_p * len(band_ptrs))(*band_ptrs)
+    with torch.cuda.device(x_buffer.device):
+        check(lib.td_blend_mixture_wrap_rows(ctypes.byref(g), ptrs, len(band_ptrs), int(g.cols), N, C, dtype_code(tile_dtype),
+                                             dtype_code(x_buffer.dtype), tile_weights.data_ptr(), rescale.data_ptr(), x_buffer.data_ptr(),
+                                             int(row_begin), int(row_end), fptr if count else None, int(count), vptr if count else None,
+                                             int(own_bands[0]), int(own_bands[1]), int(flags), current_stream_ptr(x_buffer.device)))
+    return x_buffer
+
+
 # ---------------------------------------------------------------------------------------------------------
 # DemoFusion (tile_methods/demofusion.py): thin wrappers over the C-ABI, one launch each
 # ---------------------------------------------------------------------------------------------------------

@@ -260,6 +260,10 @@ def blend_multidiffusion_peer(g, exchange: PeerExchange, parity: int, shard: Til
     nb = shard.num_chunks
     ptrs = (ctypes.c_void_p * nb)(*exchange.buf_ptrs[parity][:nb])
     x_out = out if out is not None else torch.empty((N, C, g.H, g.W), dtype=torch.float32, device=dev)
+    if g.wrap:   # a periodic plan: the windowed wrap blend over the whole canvas, waiting for every rank, no own bands
+        wait = (ctypes.c_void_p(exchange.flag_ptrs[exchange.rank]), exchange.world, ctypes.c_void_p(exchange.counter_ptr))
+        return engine.blend_multidiffusion_wrap_rows(g, list(exchange.buf_ptrs[parity][:nb]), N, C, dtype, weights, x_out, 0, g.H,
+                                                     x_buffer=x_buffer, wait=wait, tile_bs=shard.chunk)
     with torch.cuda.device(dev):
         check(lib.td_blend_multidiffusion_peer(ctypes.byref(g), ptrs, nb, shard.chunk, N, C, _cabi.dtype_code(dtype),
                                                _cabi.dtype_code(dtype), weights.data_ptr(), x_out.data_ptr(),
@@ -286,13 +290,20 @@ class StripShard:
       * latent halo, up the ranks: rank r scatters from canvas rows `[ys[first band], ys[last band] + th)`, which
         reach into the strips of higher ranks; they send those rows of the blended latent back (`x_out` / `x_in`).
     Every pixel is blended by exactly one rank, with the covering tiles in the same ascending order as on one GPU:
-    the union of the strips is bit-identical to the single-GPU latent."""
+    the union of the strips is bit-identical to the single-GPU latent.
 
-    def __init__(self, ys: Sequence[int], cols: int, tile_h: int, H: int, rank: int, world: int):
+    `wrap_y` (a plan periodic in y, seamless tiling): band i covers the canvas rows (ys[i] + v) mod H, v < tile_h, so the
+    last band(s) run past H into the top rows of rank 0's strip (on a pitch-4 plan also of further strips) -- the strips
+    close into a ring.  Tile halo then also goes "down" across the seam (rank W-1 -> rank 0), a rank whose bands wrap
+    scatters from the rows [ys[first], H) and [0, e) and receives the top ones from their owners, and a waiter's senders
+    may be a cyclic run of ranks, e.g. {W-1, 0} (see the flag bookkeeping below).  Rows keep their canvas position."""
+
+    def __init__(self, ys: Sequence[int], cols: int, tile_h: int, H: int, rank: int, world: int, wrap_y: bool = False):
         if not (0 <= rank < world):
             raise ValueError(f"rank {rank} outside world {world}")
         rows = len(ys)
         self.rank, self.world, self.rows, self.cols, self.tile_h, self.H = rank, world, rows, cols, tile_h, H
+        self.wrap_y = bool(wrap_y)
         self.ys = [int(v) for v in ys]
         base, extra = divmod(rows, world)
         counts = [base + (1 if r < extra else 0) for r in range(world)]
@@ -339,6 +350,12 @@ class StripShard:
             if self.band_begin[r] <= i < self.band_end[r]:
                 continue
             v0, v1 = max(0, lo - self.ys[i]), min(self.tile_h, hi - self.ys[i])
+            if self.wrap_y:           # the band's rows past H, at v = row - ys[i] + H
+                w0, w1 = max(0, lo - self.ys[i] + self.H), min(self.tile_h, hi - self.ys[i] + self.H)
+                if w1 > w0:
+                    # one contiguous run of tile rows per (band, target): the pushes and the halo slots rely on it
+                    assert v1 <= v0 or v1 == w0, f"band {i} reaches rank {r}'s strip in two separate runs of tile rows"
+                    v0, v1 = (v0, w1) if v1 > v0 else (w0, w1)
             if v1 > v0:
                 out.append((i, self.owner_of_band(i), v0, v1))
         return out
@@ -349,23 +366,33 @@ class StripShard:
         return [(i, q, v0, v1) for q in range(self.world) if q != r for (i, p, v0, v1) in self.halo_in(q) if p == r]
 
     def scatter_rows(self, r: Optional[int] = None):
-        """Canvas rows rank r reads when it scatters its tiles."""
+        """Canvas rows rank r reads when it scatters its tiles (under wrap_y the end may lie past H: rows mod H)."""
         r = self.rank if r is None else r
         if self.band_end[r] == self.band_begin[r]:
             return 0, 0
         return self.ys[self.band_begin[r]], self.ys[self.band_end[r] - 1] + self.tile_h
 
+    def scatter_spans(self, r: Optional[int] = None) -> List[tuple]:
+        """scatter_rows as canvas row ranges [a, b) inside [0, H): one, or under wrap_y two ([ys_first, H) and [0, e))."""
+        lo, hi = self.scatter_rows(r)
+        if hi <= self.H:
+            return [(lo, hi)] if hi > lo else []
+        if hi - self.H >= lo:
+            return [(0, self.H)]
+        return [(0, hi - self.H), (lo, self.H)]
+
     def x_in(self, r: Optional[int] = None):
         """[(owner rank q, y0, y1)]: blended-latent rows outside r's strip that r needs for its next scatter."""
         r = self.rank if r is None else r
-        lo, hi = self.scatter_rows(r)
+        spans = self.scatter_spans(r)
         out = []
         for q in range(self.world):
             if q == r:
                 continue
-            a, b = max(lo, self.B[q]), min(hi, self.B[q + 1])
-            if b > a:
-                out.append((q, a, b))
+            for lo, hi in spans:
+                a, b = max(lo, self.B[q]), min(hi, self.B[q + 1])
+                if b > a:
+                    out.append((q, a, b))
         return out
 
     def x_out(self, r: Optional[int] = None):
@@ -376,18 +403,41 @@ class StripShard:
     # A waiter polls ONE contiguous run of flag slots, the span of the ranks that send it rows.  The span may hold a rank
     # that has no rows for it (the latent-halo senders of a pitch-4 plan can skip a rank whose strip is empty), and such a
     # rank must still bump its slot every step or the wait never ends: every rank inside a waiter's span pushes to it once
-    # per step, a signal-only push (no regions) when it has nothing to send.  The tile-halo span runs over lower ranks,
-    # the latent-halo span over higher ones, so no wait cycle can form.
+    # per step, a signal-only push (no regions) when it has nothing to send.
+    #
+    # On a ring (wrap_y) a waiter's senders may be a CYCLIC run, e.g. {W-1, 0}: the span is then the shortest cyclic run from
+    # the first sender above the waiter to the last one below it (it never holds the waiter), and it is polled as the
+    # contiguous slots [first, first + count) with first + count up to 2 * world: flag slot r + world stands for rank r.  A sender
+    # whose rank lies in the wrapped part of a target's run publishes into its mirrored slot r + world there instead of slot r,
+    # so td_push_regions and the in-kernel waits stay those of a bounded plan (the flag arrays hold 32 slots, 2 * TD_MAX_PEERS)
+    # and a push still publishes into one slot per target (at most world - 1).
+    #
+    # No wait cycle can stall a step: every wait of step s is satisfied by pushes of step s only, and those pushes are ordered
+    # after nothing but the waits of step s - 1 (tile-halo push -> blend -> latent-halo push + wait on each rank).  Nor can a
+    # halo be overwritten while it is read: a rank that sends tile halo to q reads latent rows of q (its band covers rows of
+    # q's strip, so it scatters from them) and therefore waits, at the end of step s, for q's latent push -- which q makes
+    # only after its step-s blend has read that halo.  (Bounded plans: the tile-halo span runs over lower ranks, the
+    # latent-halo span over higher ones.)
     def _flag_plan(self):
         if not hasattr(self, "_flag_plan_cache"):
             plan = {}
+            W = self.world
             for kind in ("tiles", "x"):
                 spans = []
-                for r in range(self.world):
+                for r in range(W):
                     s = sorted({p for (_, p, _, _) in self.halo_in(r)}) if kind == "tiles" else sorted({q for (q, _, _) in self.x_in(r)})
-                    spans.append((s[0], s[-1] - s[0] + 1) if s else (0, 0))
-                targets = [[q for q in range(self.world) if spans[q][0] <= r < spans[q][0] + spans[q][1]] for r in range(self.world)]
-                plan[kind] = (spans, targets)
+                    if not s:
+                        spans.append((0, 0))
+                    elif not self.wrap_y:
+                        spans.append((s[0], s[-1] - s[0] + 1))
+                    else:
+                        first = next((r + k) % W for k in range(1, W) if (r + k) % W in s)
+                        last = next((r - k) % W for k in range(1, W) if (r - k) % W in s)
+                        spans.append((first, (last - first) % W + 1))
+                holds = lambda q, k: spans[q][0] <= k < spans[q][0] + spans[q][1]
+                targets = [[q for q in range(W) if holds(q, r) or holds(q, r + W)] for r in range(W)]
+                mirrored = [[q for q in targets[r] if not holds(q, r)] for r in range(W)]
+                plan[kind] = (spans, targets, mirrored)
             self._flag_plan_cache = plan
         return self._flag_plan_cache
 
@@ -405,6 +455,18 @@ class StripShard:
         """The ranks rank r pushes to in set `kind` every step (with rows, or signal-only), ascending."""
         r = self.rank if r is None else r
         return list(self._flag_plan()[kind][1][r])
+
+    def mirrored_targets(self, kind: str, r: Optional[int] = None) -> List[int]:
+        """The push targets that poll rank r in the wrapped part of their wait run in set `kind`: rank r publishes into its
+        mirrored slot r + world there instead of slot r (none under a bounded plan)."""
+        r = self.rank if r is None else r
+        return list(self._flag_plan()[kind][2][r])
+
+    def push_slots(self, kind: str, r: Optional[int] = None) -> List[tuple]:
+        """[(target rank, flag slot)] rank r bumps in set `kind` every step, one per target, ascending by target."""
+        r = self.rank if r is None else r
+        mirrored = set(self.mirrored_targets(kind, r))
+        return [(q, r + self.world if q in mirrored else r) for q in self.push_targets(kind, r)]
 
 
 # measurement switches (defaults = the shipped path): TD_STRIP_LATE_WAIT=0 -> every blend CTA waits for the halos (no own-band
@@ -452,15 +514,16 @@ class _PeerFlags:
         torch.cuda.synchronize(self.device)
 
     def push(self, regions: Sequence[tuple], targets: Sequence[int], wait_first: int = 0, wait_count: int = 0, bump_own: bool = True,
-             bump_next: Optional[int] = None):
+             bump_next: Optional[int] = None, mirrored: Sequence[int] = ()):
         """Copy `regions` [(src, dst, planes, rows, row_bytes, src_plane_bytes, src_pitch_bytes, dst_plane_bytes,
         dst_pitch_bytes)] (16-byte aligned) into peer memory and publish them in slot `rank` of the `targets`' flag arrays;
         optionally advance this set's expect counter and wait for ranks [wait_first, wait_first + wait_count); optionally
-        advance another set's expect counter (device pointer) when done -- ONE launch (td_push_regions)."""
+        advance another set's expect counter (device pointer) when done -- ONE launch (td_push_regions).  `mirrored`: the
+        targets that poll this rank in its mirrored slot rank + world (a wrapped strip plan, StripShard.mirrored_targets)."""
         regions = list(regions)
         if len(regions) > _cabi.TD_MAX_PUSH_REGIONS:
             raise ValueError(f"{len(regions)} halo regions in one push (TD_MAX_PUSH_REGIONS = {_cabi.TD_MAX_PUSH_REGIONS})")
-        slots = [self.ptrs[q] + 4 * self.rank for q in targets if q != self.rank]
+        slots = [self.ptrs[q] + 4 * (self.rank + (self.world if q in mirrored else 0)) for q in targets if q != self.rank]
         table = (ctypes.c_void_p * max(1, len(slots)))(*slots)
         arr = (_cabi.TdPushRegion * max(1, len(regions)))()
         for k, (src, dst, planes, rows, rb, sp, spi, dp, dpi) in enumerate(regions):
@@ -500,6 +563,11 @@ class StripExchange:
         self.xes = torch.empty((), dtype=latent_dtype).element_size()
         if (W * self.xes) % 16 != 0:      # the latent-halo rows are pushed as 16-byte vectors
             raise ValueError(f"row-strip shard: a {latent_dtype} latent needs W % {16 // self.xes} == 0 (W = {W})")
+        for kind in ("tiles", "x"):       # one td_push_regions publishes into at most TD_MAX_PEERS flag slots
+            n = len(sh.push_slots(kind))
+            if n > _cabi.TD_MAX_PEERS:
+                raise ValueError(f"row-strip shard: rank {sh.rank} would publish into {n} {kind} flag slots per push "
+                                 f"(TD_MAX_PEERS = {_cabi.TD_MAX_PEERS})")
         self.band_elems = sh.cols * N * C * sh.tile_h * tile_w                 # one band of tiles [cols*N, C, th, tw]
         self.halo_bands = [i for (i, _, _, _) in sh.halo_in()]
         n_own = len(sh.bands())
@@ -531,6 +599,7 @@ class StripExchange:
         self.flags_tiles.set_expect(_cabi.TD_PUSH_CTAS)      # the first step's blend waits for ONE push of each sender
         self._tile_wait, self._x_wait = sh.wait_range("tiles"), sh.wait_range("x")
         self._tile_targets, self._x_targets = sh.push_targets("tiles"), sh.push_targets("x")
+        self._tile_mirrored, self._x_mirrored = sh.mirrored_targets("tiles"), sh.mirrored_targets("x")
         dist.barrier(group=group)
 
     # ---- this rank's tile outputs -----------------------------------------------------------------------------
@@ -558,7 +627,7 @@ class StripExchange:
         # the blend's expect counter of this set is advanced by the latent-halo push that closed the PREVIOUS step (bump_next):
         # nothing this launch writes is read by this rank's own blend, so it may ride a side stream
         if not _OVERLAP_PUSH:
-            self.flags_tiles.push(regions, self._tile_targets, bump_own=False)
+            self.flags_tiles.push(regions, self._tile_targets, bump_own=False, mirrored=self._tile_mirrored)
             return
         # side stream: this rank's blend waits (in-kernel, only in the CTAs that read a halo) for the NEIGHBOUR's push, not
         # for this one -- the NVLink copy overlaps the blend of the interior rows; push_x_halos_and_wait joins the side
@@ -570,7 +639,7 @@ class StripExchange:
         fork.record(main)
         self._side.wait_event(fork)
         with torch.cuda.stream(self._side):
-            self.flags_tiles.push(regions, self._tile_targets, bump_own=False)
+            self.flags_tiles.push(regions, self._tile_targets, bump_own=False, mirrored=self._tile_mirrored)
             self._join = torch.cuda.Event()
             self._join.record(self._side)
 
@@ -603,6 +672,11 @@ class StripExchange:
             return self.x_out
         if not hasattr(self, "_ptr_table"):
             self._ptr_table = self.band_pointer_table()
+        own = (sh.band_begin[sh.rank], sh.band_end[sh.rank]) if _LATE_WAIT else (0, 0)
+        if g.wrap:                         # a periodic plan: the windowed wrap blend (no reciprocal weights)
+            engine.blend_multidiffusion_wrap_rows(g, list(self._ptr_table), self.N, self.C, self.dtype, weights, self.x_out, lo, hi,
+                                                  x_buffer=x_buffer, wait=(f, count, v), own_bands=own, flags=flags)
+            return self.x_out
         with torch.cuda.device(self.device):
             check(lib.td_blend_multidiffusion_rows(ctypes.byref(g), self._ptr_table, sh.rows, sh.cols, self.N, self.C, _cabi.dtype_code(self.dtype),
                                                    _cabi.dtype_code(self.dtype), weights.data_ptr(),
@@ -626,8 +700,9 @@ class StripExchange:
         if not hasattr(self, "_ptr_table"):
             self._ptr_table = self.band_pointer_table()
         own = (sh.band_begin[sh.rank], sh.band_end[sh.rank]) if _LATE_WAIT else (0, 0)
-        return engine.blend_mixture_rows(g, list(self._ptr_table), self.N, self.C, self.dtype, tile_weights, rescale, out, lo, hi,
-                                         wait=self.flags_tiles.wait_args(*self._tile_wait), own_bands=own, flags=flags)
+        rows_blend = engine.blend_mixture_wrap_rows if g.wrap else engine.blend_mixture_rows
+        return rows_blend(g, list(self._ptr_table), self.N, self.C, self.dtype, tile_weights, rescale, out, lo, hi,
+                          wait=self.flags_tiles.wait_args(*self._tile_wait), own_bands=own, flags=flags)
 
     def join_side(self):
         """The caller's stream waits for the side-stream tile-halo push of this step (no-op when there is none)."""
@@ -647,7 +722,8 @@ class StripExchange:
             regions.append((self._xout.ptr + a * row, self.peer_xout[p] + a * row, self.N * self.C, 1, (b - a) * row, plane, plane, plane, plane))
         first, count = self._x_wait
         self.join_side()
-        self.flags_x.push(regions, self._x_targets, first, count, bump_own=True, bump_next=self.flags_tiles.counter_ptr)
+        self.flags_x.push(regions, self._x_targets, first, count, bump_own=True, bump_next=self.flags_tiles.counter_ptr,
+                          mirrored=self._x_mirrored)
 
     def gather_latent(self, x: torch.Tensor) -> torch.Tensor:
         """All ranks' strips of `x` (any tensor laid out like the latent) -> the full latent on every rank."""

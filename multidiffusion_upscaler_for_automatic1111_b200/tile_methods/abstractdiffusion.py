@@ -268,14 +268,17 @@ class AbstractDiffusion:
         Custom regions (init_custom_bbox) are shared out as well: region j is denoised by rank j % world and its output
         all-gathered (parallel.RegionShard); in strip mode its input rows are gathered from the strips' owners first.  Every
         rank composites the regions over the rows it returns.  Without a background layer (draw_background=False, no
-        init_grid_bbox) only the regions are sharded, in replicate mode."""
+        init_grid_bbox) only the regions are sharded, in replicate mode.
+
+        A wrapped grid (init_grid_bbox(..., wrap_x / wrap_y), seamless tiling) needs an explicit mode: under "strip" with
+        wrap_y the strips close into a ring (StripShard(wrap_y=True)); both modes stay bit-identical to one GPU."""
         import torch.distributed as dist
         from .. import parallel
         if self._grid is None and not self.enable_custom_bbox:
             raise RuntimeError("init_tile_shard() must follow init_grid_bbox() or init_custom_bbox()")
-        if self._grid is not None and self._grid.wrap:
-            raise NotImplementedError("init_tile_shard() does not support a wrapped grid (wrap_x / wrap_y): the strip plan and the "
-                                      "peer-memory blends assume a bounded canvas")
+        if self._grid is not None and self._grid.wrap and mode is None:
+            raise NotImplementedError("init_tile_shard() on a wrapped grid (wrap_x / wrap_y, a periodic canvas) needs an explicit "
+                                      "mode='strip' or mode='replicate'")
         if mode is None:
             mode = "strip" if (fused and self.method == "MultiDiffusion" and self._grid is not None) else "replicate"
         if mode not in ("strip", "replicate"):
@@ -291,7 +294,8 @@ class AbstractDiffusion:
             self._strip = None
             self._shard = parallel.TileShard(0, rank, world)
         elif mode == "strip":
-            self._strip = parallel.StripShard(list(g.ys[:g.rows]), g.cols, g.tile_h, g.H, rank, world)
+            self._strip = parallel.StripShard(list(g.ys[:g.rows]), g.cols, g.tile_h, g.H, rank, world,
+                                              wrap_y=bool(g.wrap & engine.WRAP_Y))
             t0, t1 = self._strip.tile_range()
             self._shard = parallel.TileShard(self.num_tiles, rank, world)     # kept for callers that read .begin / .end
             self._shard.begin, self._shard.end = t0, t1
