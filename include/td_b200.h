@@ -353,7 +353,9 @@ int td_region_composite_rows(const void* x_buffer, const float* weights, const t
  * ------------------------------------------------------------------------- */
 
 /* Dilated global views -- demofusion.py:283-308: out[(v*N+n), c, i, j] = src_v[n, c, by_v + i*s, bx_v + j*s],
- * src_v = x1 where view_second[v] (mixture mode: the blurred latent) else x0.  Host int arrays of n_views. */
+ * src_v = x1 where view_second[v] (mixture mode: the blurred latent) else x0.  Host int arrays of n_views,
+ * 1 <= n_views <= 64 per launch.  Any offsets with 0 <= bx, bx + (out_w - 1) * s < W and 0 <= by,
+ * by + (out_h - 1) * s < H are gathered; others are refused with TD_ERR_INVALID_ARG. */
 int td_dilated_gather(const void* x0, const void* x1, void* out, int N, int C, int H, int W, int s,
                       int out_h, int out_w, const int32_t* view_bx, const int32_t* view_by,
                       const int32_t* view_second, int n_views, int dtype, void* stream);
@@ -362,7 +364,9 @@ int td_dilated_gather(const void* x0, const void* x1, void* out, int N, int C, i
  * rounded through dtype), `/ 2` in mixture mode, and out = x_local*(1-c2) + x_global*c2 (each product and
  * the sum rounded through dtype).  view_batch_ptrs: HOST array of DEVICE pointers, batch b holding
  * views [b*views_per_batch, ...) as [.*N, C, out_h, out_w].  Pixels with y >= end_y or x >= end_x get
- * x_global = 0 (the reference's `end = W - jitter_range` slice bound, demofusion.py:280). */
+ * x_global = 0 (the reference's `end = W - jitter_range` slice bound, demofusion.py:280).  Refused with
+ * TD_ERR_INVALID_ARG before any launch: s <= 0, a non-positive size, end_y > H, end_x > W, and views that
+ * do not cover [0, end_y) x [0, end_x), i.e. (end_y - 1) / s >= out_h or (end_x - 1) / s >= out_w. */
 int td_demofusion_combine(const void* x_local, const void* const* view_batch_ptrs, int num_batches,
                           int views_per_batch, int n_views, void* out, int N, int C, int H, int W, int s,
                           int out_h, int out_w, int end_y, int end_x, int mixture, float c2,

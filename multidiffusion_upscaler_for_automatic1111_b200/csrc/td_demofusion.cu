@@ -22,12 +22,12 @@ namespace {
 
 using namespace td;
 
-constexpr int kMaxViews = 64;     // 2 * s * s, s <= 5
+constexpr int kMaxViews = 64;     // views per launch (the caller batches 2 * s * s views, s <= 8)
 constexpr int kMaxKernel = 15;
 
 struct ViewTable {
     int n_views;                        // views in this launch
-    unsigned char bx[kMaxViews], by[kMaxViews];
+    int32_t bx[kMaxViews], by[kMaxViews];   // any offset the host check accepts (8 bits wrapped offsets >= 256)
     unsigned char second[kMaxViews];    // 1: read from the second (blurred) source
 };
 
@@ -145,7 +145,7 @@ extern "C" int td_dilated_gather(const void* x0, const void* x1, void* out, int 
             td_set_error("td_dilated_gather: view %d out of range", v);
             return TD_ERR_INVALID_ARG;
         }
-        vt.bx[v] = (unsigned char)view_bx[v]; vt.by[v] = (unsigned char)view_by[v]; vt.second[v] = (unsigned char)sec;
+        vt.bx[v] = view_bx[v]; vt.by[v] = view_by[v]; vt.second[v] = (unsigned char)sec;
     }
     const int es = td_dtype_size(dtype);
     if (es == 0) { td_set_error("td_dilated_gather: unknown dtype"); return TD_ERR_INVALID_ARG; }
@@ -161,8 +161,14 @@ extern "C" int td_demofusion_combine(const void* x_local, const void* const* vie
                                      int n_views, void* out, int N, int C, int H, int W, int s, int out_h, int out_w, int end_y,
                                      int end_x, int mixture, float c2, float one_minus_c2, int dtype, void* stream) {
     if (x_local == nullptr || out == nullptr || view_batch_ptrs == nullptr || num_batches <= 0 || num_batches > TD_MAX_BATCH_PTRS ||
-        views_per_batch <= 0 || n_views != (mixture ? 2 : 1) * s * s || (long long)num_batches * views_per_batch < n_views) {
+        views_per_batch <= 0 || s <= 0 || n_views != (mixture ? 2 : 1) * s * s || (long long)num_batches * views_per_batch < n_views ||
+        N <= 0 || C <= 0 || H <= 0 || W <= 0 || out_h <= 0 || out_w <= 0 || end_y > H || end_x > W) {
         td_set_error("td_demofusion_combine: bad arguments");
+        return TD_ERR_INVALID_ARG;
+    }
+    // every pixel of [0, end) must map inside a view: i = y / s < out_h
+    if ((end_y > 0 && (end_y - 1) / s >= out_h) || (end_x > 0 && (end_x - 1) / s >= out_w)) {
+        td_set_error("td_demofusion_combine: views %dx%d do not cover [0, %d) x [0, %d) at scale %d", out_h, out_w, end_y, end_x, s);
         return TD_ERR_INVALID_ARG;
     }
     CombineParams p;

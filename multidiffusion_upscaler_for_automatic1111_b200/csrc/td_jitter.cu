@@ -243,7 +243,7 @@ extern "C" int td_demofusion_combine_offset(const void* x_local, const void* con
                                             float one_minus_c2, int dtype, void* stream) {
     if (x_local == nullptr || out == nullptr || view_batch_ptrs == nullptr || num_batches <= 0 || num_batches > TD_MAX_BATCH_PTRS ||
         views_per_batch <= 0 || s <= 0 || n_views != (mixture ? 2 : 1) * s * s || (long long)num_batches * views_per_batch < n_views ||
-        offset < 0 || end_y > H || end_x > W || out_h <= 0 || out_w <= 0) {
+        offset < 0 || N <= 0 || C <= 0 || H <= 0 || W <= 0 || end_y > H || end_x > W || out_h <= 0 || out_w <= 0) {
         td_set_error("td_demofusion_combine_offset: bad arguments");
         return TD_ERR_INVALID_ARG;
     }

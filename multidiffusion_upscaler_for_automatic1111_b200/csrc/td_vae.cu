@@ -242,12 +242,13 @@ affine_clamp_kernel(T* __restrict__ x, int C, long long HW, const float* __restr
     const float l = lo[0], h = hi[0];
     T* p = x + (long long)plane * HW;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < HW; i += (long long)gridDim.x * blockDim.x) {
-        // torch evaluates each op in the tensor dtype: round through T after every step
+        // torch evaluates each op in the tensor dtype: round through T after every step.  The _rn intrinsics keep
+        // `* so + mo` from being contracted into one FMA where round_through is the identity (fp32).
         float v = Elem<T>::to_f32(p[i]);
-        v = round_through<T>(v - mn);
+        v = round_through<T>(__fsub_rn(v, mn));
         v = round_through<T>(__fdiv_rn(v, sn));
-        v = round_through<T>(v * so);
-        v = round_through<T>(v + mo);
+        v = round_through<T>(__fmul_rn(v, so));
+        v = round_through<T>(__fadd_rn(v, mo));
         p[i] = Elem<T>::from_f32(fminf(fmaxf(v, l), h));
     }
 }
