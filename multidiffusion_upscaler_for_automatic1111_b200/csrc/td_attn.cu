@@ -33,6 +33,7 @@
 
 #include "td_b200.h"
 #include "td_internal.h"
+#include "td_launch.h"
 #include "td_tma.cuh"
 #include "td_wgmma.cuh"
 
@@ -269,27 +270,23 @@ int encode_operand(CUtensorMap* m, const void* base, int is_bf16, int T, int C, 
     return td_encode_map(m, base, is_bf16, 2, dims, str, box, es, true, what);
 }
 
-// one launch of the <BF16, NC> form: shared-memory opt-in (per call: the call is one per VAE tile) and the ring depth
+// one launch of the <BF16, NC> form: shared-memory opt-in and the ring depth
 template <bool BF16, int NC, int NO>
 int attn_launch(const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv, AttnParams p, uint16_t* o, cudaStream_t st) {
-    int dev = 0, optin = 0;
+    const DeviceProps dev = device_props();
     cudaFuncAttributes fa;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess ||
-        cudaFuncGetAttributes(&fa, attn_kernel<BF16, NC, NO>) != cudaSuccess) {
+    if (!dev.ok || cudaFuncGetAttributes(&fa, attn_kernel<BF16, NC, NO>) != cudaSuccess) {
         cudaGetLastError();
         td_set_error("td_attention: device / kernel query failed");
         return TD_ERR_CUDA;
     }
-    optin -= (int)fa.sharedSizeBytes;        // the opt-in limit covers static + dynamic shared memory
+    const int optin = dev.smem_optin - (int)fa.sharedSizeBytes;   // the opt-in limit covers static + dynamic shared memory
     constexpr int stage_bytes = 2 * NC * kAttnChunkBytes;
     p.stages = std::min(kAttnMaxStages, (optin - 1024 - stage_bytes - kAttnXchgBytes) / stage_bytes);
     if (p.stages < 2) { td_set_error("td_attention: not enough shared memory"); return TD_ERR_UNSUPPORTED; }
     const int smem = 1024 + (1 + p.stages) * stage_bytes + kAttnXchgBytes;
-    if (cudaFuncSetAttribute(attn_kernel<BF16, NC, NO>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) {
-        cudaGetLastError();
-        td_set_error("td_attention: shared-memory opt-in (%d bytes) failed", smem);
-        return TD_ERR_CUDA;
-    }
+    const int rc = smem_optin(attn_kernel<BF16, NC, NO>, smem, "td_attention");
+    if (rc != TD_OK) return rc;
     int per_sm = 0;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, attn_kernel<BF16, NC, NO>, kAttnThreads, smem) != cudaSuccess || per_sm < 1) {
         cudaGetLastError();
@@ -297,9 +294,7 @@ int attn_launch(const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap&
         return TD_ERR_UNSUPPORTED;
     }
     attn_kernel<BF16, NC, NO><<<dim3(p.key_blocks, NC / NO), kAttnThreads, smem, st>>>(mq, mk, mv, p, o);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { td_set_error("td_attention: launch failed: %s", cudaGetErrorString(e)); return TD_ERR_CUDA; }
-    return TD_OK;
+    return launch_status("td_attention");
 }
 
 template <bool BF16>
@@ -324,7 +319,7 @@ extern "C" int td_attention(const void* q, const void* k, const void* v, void* o
     for (int64_t pitch : {q_pitch, k_pitch, v_pitch, o_pitch})
         if (pitch < C || pitch % 8 != 0) { td_set_error("td_attention: pitches must cover C and be multiples of 8 elements (16 bytes)"); return TD_ERR_INVALID_ARG; }
     for (const void* ptr : {q, k, v, (const void*)o})
-        if ((reinterpret_cast<uintptr_t>(ptr) & 15u) != 0) { td_set_error("td_attention: tensors must be 16-byte aligned"); return TD_ERR_INVALID_ARG; }
+        if (!aligned16(ptr)) { td_set_error("td_attention: tensors must be 16-byte aligned"); return TD_ERR_INVALID_ARG; }
 
     AttnParams p;
     std::memset(&p, 0, sizeof(p));

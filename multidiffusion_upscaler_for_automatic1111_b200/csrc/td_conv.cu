@@ -29,10 +29,10 @@
 #include <cstdint>
 #include <cstdlib>
 #include <cstring>
-#include <mutex>
 
 #include "td_b200.h"
 #include "td_internal.h"
+#include "td_launch.h"
 #include "td_tma.cuh"
 #include "td_wgmma.cuh"
 
@@ -243,61 +243,24 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
 }
 
 // ------------------------------------------------------------------------------------------------- host
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn conv_encode_fn() {
-    static EncodeTiledFn fn = [] {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess)
-            return (EncodeTiledFn) nullptr;
-        return (EncodeTiledFn)p;
+// Dynamic shared memory the conv kernels may use: the device's opt-in limit covers static + dynamic shared memory, so the
+// kernels' static part is left out.  -1 when a query failed.
+int conv_dyn_smem_limit(const DeviceProps& dev) {
+    if (!dev.ok) return -1;
+    static const int static_bytes = [] {
+        cudaFuncAttributes fa;
+        if (cudaFuncGetAttributes(&fa, conv_gemm_kernel<256, false>) != cudaSuccess) { cudaGetLastError(); return -1; }
+        return (int)fa.sharedSizeBytes;
     }();
-    return fn;
-}
-
-template <int BN> bool conv_smem_optin(int bytes) {
-    return cudaFuncSetAttribute(conv_gemm_kernel<BN, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) == cudaSuccess &&
-           cudaFuncSetAttribute(conv_gemm_kernel<BN, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) == cudaSuccess;
-}
-
-struct ConvDev { int sms; int smem_optin; bool ok; };
-ConvDev conv_dev() {
-    static std::mutex mu;
-    static ConvDev cache[64];
-    static bool have[64] = {};
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return {0, 0, false};
-    std::lock_guard<std::mutex> lk(mu);
-    if (!have[dev]) {
-        ConvDev d{0, 0, false};
-        d.ok = cudaDeviceGetAttribute(&d.sms, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess &&
-               cudaDeviceGetAttribute(&d.smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) == cudaSuccess;
-        if (d.ok) {   // the opt-in limit covers static + dynamic shared memory: leave room for the kernel's static part
-            cudaFuncAttributes fa;
-            if (cudaFuncGetAttributes(&fa, conv_gemm_kernel<256, false>) != cudaSuccess) { cudaGetLastError(); d.ok = false; }
-            else {
-                d.smem_optin -= (int)fa.sharedSizeBytes;
-                if (!conv_smem_optin<16>(d.smem_optin) || !conv_smem_optin<32>(d.smem_optin) || !conv_smem_optin<64>(d.smem_optin) ||
-                    !conv_smem_optin<128>(d.smem_optin) || !conv_smem_optin<256>(d.smem_optin)) {
-                    cudaGetLastError();
-                    d.ok = false;
-                }
-            }
-        }
-        cache[dev] = d;
-        have[dev] = true;
-    }
-    return cache[dev];
+    return static_bytes < 0 ? -1 : dev.smem_optin - static_bytes;
 }
 
 }  // namespace
 
 int td_encode_map(CUtensorMap* out, const void* base, int is_bf16, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                   const uint32_t* box, const uint32_t* estr, bool swizzle128, const char* what) {
-    EncodeTiledFn fn = conv_encode_fn();
-    if (fn == nullptr) { td_set_error("cuTensorMapEncodeTiled is not available from this driver"); return TD_ERR_CUDA; }
+    const td::EncodeTiledFn fn = td::tensor_map_encoder();
+    if (fn == nullptr) return TD_ERR_CUDA;
     cuuint64_t d[5]; cuuint64_t s[4]; cuuint32_t b[5]; cuuint32_t e[5];
     for (int i = 0; i < rank; ++i) { d[i] = dims[i]; b[i] = box[i]; e[i] = estr[i]; }
     for (int i = 0; i + 1 < rank; ++i) s[i] = strides_bytes[i];
@@ -306,7 +269,7 @@ int td_encode_map(CUtensorMap* out, const void* base, int is_bf16, int rank, con
                           swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) {
-        td_set_error("cuTensorMapEncodeTiled failed (%d) for %s: dims [%llu,%llu,%llu,%llu] box [%u,%u,%u,%u]", (int)r, what,
+        td_set_error("tensor-map encoding failed (%d) for %s: dims [%llu,%llu,%llu,%llu] box [%u,%u,%u,%u]", (int)r, what,
                      (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)(rank > 2 ? dims[2] : 0),
                      (unsigned long long)(rank > 3 ? dims[3] : 0), box[0], box[1], rank > 2 ? box[2] : 0, rank > 3 ? box[3] : 0);
         return TD_ERR_CUDA;
@@ -336,15 +299,16 @@ int conv_run(const td_conv_desc* d, const void* x, const void* w, const float* b
         return TD_ERR_INVALID_ARG;
     }
     for (const void* ptr : {x, w, (const void*)y, residual, (const void*)(d->bias_per_row ? nullptr : bias), (const void*)d->post_scale, (const void*)d->post_shift})
-        if (ptr != nullptr && (reinterpret_cast<uintptr_t>(ptr) & 15u) != 0) { td_set_error("td_conv2d_nhwc: tensors (and per-channel vectors) must be 16-byte aligned"); return TD_ERR_INVALID_ARG; }
+        if (ptr != nullptr && !aligned16(ptr)) { td_set_error("td_conv2d_nhwc: tensors (and per-channel vectors) must be 16-byte aligned"); return TD_ERR_INVALID_ARG; }
     if (d->y2 != nullptr && (d->post_scale == nullptr || d->post_shift == nullptr || d->y2_pitch < d->Cout || d->y2_pitch % 8 != 0 ||
-                             (reinterpret_cast<uintptr_t>(d->y2) & 15u) != 0)) {
+                             !aligned16(d->y2))) {
         td_set_error("td_conv2d_nhwc: y2 needs post_scale / post_shift, a 16-byte aligned pointer and a pitch >= Cout in multiples of 8");
         return TD_ERR_INVALID_ARG;
     }
     if ((d->post_scale == nullptr) != (d->post_shift == nullptr)) { td_set_error("td_conv2d_nhwc: post_scale and post_shift come together"); return TD_ERR_INVALID_ARG; }
-    const ConvDev dev = conv_dev();
-    if (!dev.ok) { td_set_error("td_conv2d_nhwc: device query / shared-memory opt-in failed"); return TD_ERR_CUDA; }
+    const DeviceProps dev = device_props();
+    const int smem_limit = conv_dyn_smem_limit(dev);
+    if (smem_limit < 0) { td_set_error("td_conv2d_nhwc: device query failed"); return TD_ERR_CUDA; }
 
     ConvParams p;
     std::memset(&p, 0, sizeof(p));
@@ -372,7 +336,7 @@ int conv_run(const td_conv_desc* d, const void* x, const void* w, const float* b
     p.y2_pitch = d->y2 != nullptr ? d->y2_pitch : 0;
     p.res_pitch = residual != nullptr ? d->res_pitch : 0;
     const int stage_bytes = kConvStageA + bn * 128;
-    p.stages = std::min(kConvMaxStages, (dev.smem_optin - 1024) / stage_bytes);
+    p.stages = std::min(kConvMaxStages, (smem_limit - 1024) / stage_bytes);
     if (p.stages < 2) { td_set_error("td_conv2d_nhwc: not enough shared memory"); return TD_ERR_UNSUPPORTED; }
     const size_t smem = (size_t)p.stages * stage_bytes + 1024;
 
@@ -398,20 +362,24 @@ int conv_run(const td_conv_desc* d, const void* x, const void* w, const float* b
     const int grid = std::min(p.num_tiles, dev.sms);
     const uint16_t* res = static_cast<const uint16_t*>(residual);
     cudaStream_t st = (cudaStream_t)stream;
-#define TD_CONV_LAUNCH(BN)                                                                                                          \
-    (p.is_bf16 ? conv_gemm_kernel<BN, true><<<grid, kConvThreads, smem, st>>>(ma, mb, p, bias, res, d->post_scale, d->post_shift, yo, y2o) \
-               : conv_gemm_kernel<BN, false><<<grid, kConvThreads, smem, st>>>(ma, mb, p, bias, res, d->post_scale, d->post_shift, yo, y2o))
+    // every form is opted in to the whole limit (once per device: smem_optin remembers it), whatever its stage count
+#define TD_CONV_LAUNCH(BN, BF16)                                                                                                    \
+    do {                                                                                                                            \
+        const int rc = smem_optin(conv_gemm_kernel<BN, BF16>, smem_limit, "td_conv2d_nhwc");                                        \
+        if (rc != TD_OK) return rc;                                                                                                 \
+        conv_gemm_kernel<BN, BF16><<<grid, kConvThreads, smem, st>>>(ma, mb, p, bias, res, d->post_scale, d->post_shift, yo, y2o);  \
+    } while (0)
+#define TD_CONV_CASE(BN) if (p.is_bf16) TD_CONV_LAUNCH(BN, true); else TD_CONV_LAUNCH(BN, false)
     switch (bn) {
-        case 16: TD_CONV_LAUNCH(16); break;
-        case 32: TD_CONV_LAUNCH(32); break;
-        case 64: TD_CONV_LAUNCH(64); break;
-        case 128: TD_CONV_LAUNCH(128); break;
-        default: TD_CONV_LAUNCH(256); break;
+        case 16: TD_CONV_CASE(16); break;
+        case 32: TD_CONV_CASE(32); break;
+        case 64: TD_CONV_CASE(64); break;
+        case 128: TD_CONV_CASE(128); break;
+        default: TD_CONV_CASE(256); break;
     }
+#undef TD_CONV_CASE
 #undef TD_CONV_LAUNCH
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { td_set_error("td_conv2d_nhwc: launch failed: %s", cudaGetErrorString(e)); return TD_ERR_CUDA; }
-    return TD_OK;
+    return launch_status("td_conv2d_nhwc");
 }
 }  // namespace
 

@@ -17,6 +17,7 @@
 #include "td_b200.h"
 #include "td_device.cuh"
 #include "td_internal.h"
+#include "td_launch.h"
 
 namespace {
 
@@ -121,11 +122,6 @@ depthwise_conv_kernel(const T* __restrict__ in, T* __restrict__ out, const __gri
     }
 }
 
-int launch_ok(const char* what) {
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { td_set_error("%s: CUDA launch failed: %s", what, cudaGetErrorString(e)); return TD_ERR_CUDA; }
-    return TD_OK;
-}
 
 }  // namespace
 
@@ -154,7 +150,7 @@ extern "C" int td_dilated_gather(const void* x0, const void* x1, void* out, int 
     cudaStream_t st = (cudaStream_t)stream;
     if (es == 2) dilated_gather_kernel<__half><<<grid, 256, 0, st>>>((const __half*)x0, (const __half*)x1, (__half*)out, vt, NC, H, W, s, out_h, out_w);
     else dilated_gather_kernel<float><<<grid, 256, 0, st>>>((const float*)x0, (const float*)x1, (float*)out, vt, NC, H, W, s, out_h, out_w);
-    return launch_ok("td_dilated_gather");
+    return launch_status("td_dilated_gather");
 }
 
 extern "C" int td_demofusion_combine(const void* x_local, const void* const* view_batch_ptrs, int num_batches, int views_per_batch,
@@ -185,7 +181,7 @@ extern "C" int td_demofusion_combine(const void* x_local, const void* const* vie
     else if (dtype == TD_BF16) demofusion_combine_kernel<__nv_bfloat16><<<blocks, 256, 0, st>>>(p, (const __nv_bfloat16*)x_local, (__nv_bfloat16*)out);
     else if (dtype == TD_F32) demofusion_combine_kernel<float><<<blocks, 256, 0, st>>>(p, (const float*)x_local, (float*)out);
     else { td_set_error("td_demofusion_combine: unknown dtype"); return TD_ERR_INVALID_ARG; }
-    return launch_ok("td_demofusion_combine");
+    return launch_status("td_demofusion_combine");
 }
 
 extern "C" int td_depthwise_conv2d(const void* in, void* out, int planes, int H, int W, const float* kernel_host, int k, int dtype,
@@ -204,5 +200,5 @@ extern "C" int td_depthwise_conv2d(const void* in, void* out, int planes, int H,
     else if (dtype == TD_BF16) depthwise_conv_kernel<__nv_bfloat16><<<blocks, 256, 0, st>>>((const __nv_bfloat16*)in, (__nv_bfloat16*)out, ck, planes, H, W);
     else if (dtype == TD_F32) depthwise_conv_kernel<float><<<blocks, 256, 0, st>>>((const float*)in, (float*)out, ck, planes, H, W);
     else { td_set_error("td_depthwise_conv2d: unknown dtype"); return TD_ERR_INVALID_ARG; }
-    return launch_ok("td_depthwise_conv2d");
+    return launch_status("td_depthwise_conv2d");
 }

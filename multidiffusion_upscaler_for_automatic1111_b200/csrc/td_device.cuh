@@ -1,5 +1,6 @@
 // Device-side helpers: element traits with explicit IEEE roundings, 128-bit
-// read-only loads, unaligned-vector extraction by funnel shift.
+// read-only loads, unaligned-vector extraction by funnel shift, packed adds and
+// exact divides, programmatic dependent launch and the cross-GPU flag wait.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -110,6 +111,63 @@ __device__ __forceinline__ int upper_bound16(const short* a, int n, int val) {
         if ((int)a[mid] <= val) lo = mid + 1; else hi = mid;
     }
     return lo;
+}
+
+// largest i with a[i] <= val (or -1); `a` non-decreasing.  The estimate `inv_d` only affects speed, never the result.
+__device__ __forceinline__ int last_le(const short* a, int n, int val, float inv_d) {
+    int i = min(n - 1, max(0, (int)((float)val * inv_d)));
+    while (i + 1 < n && (int)a[i + 1] <= val) ++i;
+    while (i >= 0 && (int)a[i] > val) --i;
+    return i;
+}
+
+// floor(n / d) for n, d < 2^16 with magic = ceil(2^32 / d) (magic_u16, td_launch.h); d == 1 is passed as magic 0.
+__device__ __forceinline__ unsigned fastdiv(unsigned n, unsigned magic) { return magic ? __umulhi(n, magic) : n; }
+
+// ---- packed 16-byte arithmetic -----------------------------------------------
+// acc (+)= e on one 32-bit word of packed T, rounded through T: round_half(a + b) of the exact sum equals torch's
+// half(float(a) + float(b)) (fp32 has >= 2p+2 bits: double rounding is innocuous)
+template <typename T> __device__ __forceinline__ uint32_t packed_add(uint32_t a, uint32_t b);
+template <> __device__ __forceinline__ uint32_t packed_add<__half>(uint32_t a, uint32_t b) {
+    __half2 r = __hadd2(*reinterpret_cast<__half2*>(&a), *reinterpret_cast<__half2*>(&b));
+    return *reinterpret_cast<uint32_t*>(&r);
+}
+template <> __device__ __forceinline__ uint32_t packed_add<__nv_bfloat16>(uint32_t a, uint32_t b) {
+    __nv_bfloat162 r = __hadd2(*reinterpret_cast<__nv_bfloat162*>(&a), *reinterpret_cast<__nv_bfloat162*>(&b));
+    return *reinterpret_cast<uint32_t*>(&r);
+}
+template <> __device__ __forceinline__ uint32_t packed_add<float>(uint32_t a, uint32_t b) {
+    return __float_as_uint(__fadd_rn(__uint_as_float(a), __uint_as_float(b)));
+}
+
+// a / w correctly rounded, for w a positive integer <= 4096 with rcp = its correctly rounded reciprocal and a any 16-bit
+// float value (checked exhaustively by td_debug_check_fast_div)
+__device__ __forceinline__ float div_exact_small_int(float a, float w, float rcp) {
+    const float q = __fmul_rn(a, rcp);
+    const float r = __fmaf_rn(-q, w, a);
+    const float q2 = __fmaf_rn(r, rcp, q);
+    // w > 0: the quotient carries a's sign (this also keeps -0 / w = -0, which the fma chain turns into +0)
+    return __uint_as_float((__float_as_uint(q2) & 0x7fffffffu) | (__float_as_uint(a) & 0x80000000u));
+}
+
+// ---- launch and cross-GPU ordering -------------------------------------------
+// Programmatic dependent launch (sm_90+): a kernel launched with the stream-serialisation attribute (launch(), td_launch.h)
+// may become resident while its predecessor in the stream drains.  pdl_wait() blocks until the predecessor has completed
+// and its memory is visible -- it precedes every global read or write of the kernels, so stream order is kept; what
+// overlaps is the launch itself, the parameter fetch and the index arithmetic.  Both are no-ops for an ordinary launch.
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+
+// Spin until *flag >= want (modulo 2^32), loading with acquire semantics at system scope: what the GPU that released the
+// flag wrote before it is then visible to this thread (and, after a barrier, to its CTA).  Bounded: a peer that never
+// signals (crashed / interrupted rank) becomes a launch error, not a hung GPU.
+__device__ __forceinline__ void spin_until_ge(const uint32_t* flag, uint32_t want) {
+    uint32_t v;
+    unsigned long long spins = 0;
+    do {
+        asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(flag) : "memory");
+        if (++spins > (1ull << 31)) __trap();
+    } while ((int32_t)(v - want) < 0);
 }
 
 }  // namespace td

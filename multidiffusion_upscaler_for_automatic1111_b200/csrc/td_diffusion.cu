@@ -23,12 +23,12 @@
 
 #include <algorithm>
 #include <cstdint>
-#include <atomic>
 #include <mutex>
 
 #include "td_b200.h"
 #include "td_device.cuh"
 #include "td_internal.h"
+#include "td_launch.h"
 #include "td_tma.cuh"
 
 namespace {
@@ -65,30 +65,11 @@ struct BlendParams {
 
 enum { MODE_MD = 0, MODE_MOD = 1 };
 
-// largest i with a[i] <= val (or -1); `a` non-decreasing.  The estimate only
-// affects speed, never the result.
-__device__ __forceinline__ int last_le(const short* a, int n, int val, float inv_d) {
-    int i = min(n - 1, max(0, (int)((float)val * inv_d)));
-    while (i + 1 < n && (int)a[i + 1] <= val) ++i;
-    while (i >= 0 && (int)a[i] > val) --i;
-    return i;
-}
-
 __device__ __forceinline__ void load_origins(const GeomParams& g, short* s_ys, short* s_xs) {
     for (int i = threadIdx.x; i < g.rows; i += blockDim.x) s_ys[i] = g.ys[i];
     for (int i = threadIdx.x; i < g.cols; i += blockDim.x) s_xs[i] = g.xs[i];
     __syncthreads();
 }
-
-// floor(n / d) for n, d < 2^16 with magic = ceil(2^32 / d); d == 1 is passed as magic 0.
-__device__ __forceinline__ unsigned fastdiv(unsigned n, unsigned magic) { return magic ? __umulhi(n, magic) : n; }
-
-// Programmatic dependent launch (sm_90+): a kernel launched with the stream-serialisation attribute may become
-// resident while its predecessor in the stream drains.  pdl_wait() blocks until the predecessor has completed and
-// its memory is visible -- it precedes every global read or write below, so stream order is kept; what overlaps
-// is the launch itself, the parameter fetch and the index arithmetic.  Both are no-ops for an ordinary launch.
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
 // ---------------------------------------------------------------------------
 // Scatter, vector path (the default).  One block = `rows_per_block` rows of one (tile, n, c)
@@ -173,24 +154,6 @@ scatter_generic_kernel(const __grid_constant__ GeomParams g, const T* __restrict
 // accumulates with packed HADD2: round_half(a + b) of the exact sum, which equals
 // torch's half(float(a) + float(b)) (fp32 has >= 2p+2 bits: double rounding is innocuous).
 // ---------------------------------------------------------------------------
-template <typename T> struct PackedAdd;  // acc (+)= e on one 32-bit word of packed T
-template <> struct PackedAdd<__half> {
-    __device__ static __forceinline__ uint32_t add(uint32_t a, uint32_t b) {
-        __half2 r = __hadd2(*reinterpret_cast<__half2*>(&a), *reinterpret_cast<__half2*>(&b));
-        return *reinterpret_cast<uint32_t*>(&r);
-    }
-};
-template <> struct PackedAdd<__nv_bfloat16> {
-    __device__ static __forceinline__ uint32_t add(uint32_t a, uint32_t b) {
-        __nv_bfloat162 r = __hadd2(*reinterpret_cast<__nv_bfloat162*>(&a), *reinterpret_cast<__nv_bfloat162*>(&b));
-        return *reinterpret_cast<uint32_t*>(&r);
-    }
-};
-template <> struct PackedAdd<float> {
-    __device__ static __forceinline__ uint32_t add(uint32_t a, uint32_t b) {
-        return __float_as_uint(__fadd_rn(__uint_as_float(a), __uint_as_float(b)));
-    }
-};
 
 constexpr int kBlendWarps = 2;       // warps per block, stacked in y
 constexpr int kWarpVecs = 8;         // vectors per warp row (lane = 8 vectors x 4 rows)
@@ -212,15 +175,7 @@ blend_grid_vec_kernel(const __grid_constant__ BlendParams p, const float* __rest
     __shared__ short s_xs[TD_MAX_GRID_DIM];
     const GeomParams& g = p.g;
     if (p.wait_flags != nullptr) {   // tile shard: peers' tile outputs must be complete before they are read
-        if ((int)threadIdx.x < p.wait_world) {
-            const uint32_t want = *p.wait_value;
-            uint32_t v;
-            unsigned long long spins = 0;
-            do {   // bounded: a peer that never signals (crashed / interrupted rank) becomes a launch error, not a hung GPU
-                asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p.wait_flags + threadIdx.x) : "memory");
-                if (++spins > (1ull << 31)) __trap();
-            } while ((int32_t)(v - want) < 0);
-        }
+        if ((int)threadIdx.x < p.wait_world) spin_until_ge(p.wait_flags + threadIdx.x, *p.wait_value);
     }
     load_origins(g, s_ys, s_xs);   // (contains the __syncthreads that publishes the wait)
 
@@ -312,10 +267,10 @@ blend_grid_vec_kernel(const __grid_constant__ BlendParams p, const float* __rest
             for (int q = 0; q < RPT; ++q) {
                 const uint4 e = Vec<T>::window(A[gi][q], B[gi][q], sft[gi]);
                 if constexpr (kPacked) {
-                    pacc[q].x = PackedAdd<T>::add(pacc[q].x, e.x);
-                    pacc[q].y = PackedAdd<T>::add(pacc[q].y, e.y);
-                    pacc[q].z = PackedAdd<T>::add(pacc[q].z, e.z);
-                    pacc[q].w = PackedAdd<T>::add(pacc[q].w, e.w);
+                    pacc[q].x = packed_add<T>(pacc[q].x, e.x);
+                    pacc[q].y = packed_add<T>(pacc[q].y, e.y);
+                    pacc[q].z = packed_add<T>(pacc[q].z, e.z);
+                    pacc[q].w = packed_add<T>(pacc[q].w, e.w);
                 } else {
 #pragma unroll
                     for (int j = 0; j < VEC; ++j) {
@@ -407,9 +362,6 @@ constexpr int kAsSlots = kAsY * kAsChunks;       // 72 copy slots per tile visit
 constexpr int kAsThreads = (kAsSlots + 31) / 32 * 32;   // 96 = 3 warps: 72 copy threads
 constexpr int kAsStage = kAsSlots * 16;          // 1152 bytes per tile visit
 
-__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src, int src_bytes) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(smem_dst)), "l"(gmem_src), "r"(src_bytes) : "memory");
-}
 // 16-byte copy that writes zeros instead (no global access) when `neg_if_skip` is negative
 __device__ __forceinline__ void cp_async16_zfill(uint32_t smem_dst, long long gmem_src, int neg_if_skip) {
     asm volatile(
@@ -433,18 +385,10 @@ __device__ __forceinline__ void consume_shifted(uint4& acc, const unsigned char*
         const uint4 B = lds128(p + 16);
         e = Vec<T>::window(A, B, S);    // S is a compile-time constant: register selection / immediate shifts only
     }
-    acc.x = PackedAdd<T>::add(acc.x, e.x);
-    acc.y = PackedAdd<T>::add(acc.y, e.y);
-    acc.z = PackedAdd<T>::add(acc.z, e.z);
-    acc.w = PackedAdd<T>::add(acc.w, e.w);
-}
-
-__device__ __forceinline__ float div_exact_small_int(float a, float w, float rcp) {
-    const float q = __fmul_rn(a, rcp);
-    const float r = __fmaf_rn(-q, w, a);
-    const float q2 = __fmaf_rn(r, rcp, q);
-    // w > 0: the quotient carries a's sign (this also keeps -0 / w = -0, which the fma chain turns into +0)
-    return __uint_as_float((__float_as_uint(q2) & 0x7fffffffu) | (__float_as_uint(a) & 0x80000000u));
+    acc.x = packed_add<T>(acc.x, e.x);
+    acc.y = packed_add<T>(acc.y, e.y);
+    acc.z = packed_add<T>(acc.z, e.z);
+    acc.w = packed_add<T>(acc.w, e.w);
 }
 
 struct __align__(16) VisitEntry {   // per tile visit of a CTA, computed once by one thread
@@ -458,15 +402,8 @@ constexpr int kAsMaxVisits = 64;
 // and the CTA's next barrier publishes the wait to the other threads.
 __device__ __forceinline__ void halo_wait(const BlendParams& p, int by, int r_lo, int tid) {
     const bool reads_halo = r_lo < p.own_r_lo || r_lo + (int)p.prow_n[by] > p.own_r_hi;   // always true when own_r_lo == own_r_hi
-    if (p.wait_flags != nullptr && reads_halo && tid >= kAsThreads - 32 && tid - (kAsThreads - 32) < p.wait_world) {
-        const uint32_t want = *p.wait_value;
-        uint32_t v;
-        unsigned long long spins = 0;
-        do {   // bounded: a peer that never signals becomes a launch error, not a hung GPU
-            asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p.wait_flags + (tid - (kAsThreads - 32))) : "memory");
-            if (++spins > (1ull << 31)) __trap();
-        } while ((int32_t)(v - want) < 0);
-    }
+    if (p.wait_flags != nullptr && reads_halo && tid >= kAsThreads - 32 && tid - (kAsThreads - 32) < p.wait_world)
+        spin_until_ge(p.wait_flags + (tid - (kAsThreads - 32)), *p.wait_value);
 }
 
 // Patch row and plane group of a cp.async blend CTA: sched 0 walks blockIdx.y = patch row, .z = plane group; sched 1 / 2 put
@@ -520,18 +457,12 @@ blend_md_async_kernel(const __grid_constant__ BlendParams p, const float* __rest
         if constexpr (FASTDIV) rv[h] = inside ? __ldg(reinterpret_cast<const float4*>(rcp_weights + wo) + h) : make_float4(1.f, 1.f, 1.f, 1.f);
     }
 
-    // halo_wait, written out: through the helper the compiler schedules this kernel's prologue differently (cfg2 blend
-    // measured about 0.5% slower on an H100 80GB HBM3 at 700 W)
+    // halo_wait's test, written out here: calling halo_wait itself changes how the compiler schedules this kernel's prologue
+    // (cfg2 blend measured about 0.5% slower on an H100 80GB HBM3 at 700 W).  The spin alone through spin_until_ge leaves the
+    // instruction stream as it was with the loop written out (only register numbers differ).
     const bool reads_halo = r_lo < p.own_r_lo || r_lo + (int)p.prow_n[by] > p.own_r_hi;   // always true when own_r_lo == own_r_hi
-    if (p.wait_flags != nullptr && reads_halo && tid >= kAsThreads - 32 && tid - (kAsThreads - 32) < p.wait_world) {
-        const uint32_t want = *p.wait_value;
-        uint32_t v;
-        unsigned long long spins = 0;
-        do {   // bounded: a peer that never signals becomes a launch error, not a hung GPU
-            asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p.wait_flags + (tid - (kAsThreads - 32))) : "memory");
-            if (++spins > (1ull << 31)) __trap();
-        } while ((int32_t)(v - want) < 0);
-    }
+    if (p.wait_flags != nullptr && reads_halo && tid >= kAsThreads - 32 && tid - (kAsThreads - 32) < p.wait_world)
+        spin_until_ge(p.wait_flags + (tid - (kAsThreads - 32)), *p.wait_value);
 
     // ---- per-visit constants: thread i prepares visit i -------------------------------------------------
     const long long plane_bytes = (long long)g.th * g.tw * (long long)sizeof(T);
@@ -1042,10 +973,10 @@ blend_md_tma_kernel(const __grid_constant__ TmaBlendParams<NB> p, const float* _
             const uint4 B = lds128(mine + (size_t)i * STAGE + 16);
             e = Vec<T>::window(A, B, s);
         }
-        acc.x = PackedAdd<T>::add(acc.x, e.x);
-        acc.y = PackedAdd<T>::add(acc.y, e.y);
-        acc.z = PackedAdd<T>::add(acc.z, e.z);
-        acc.w = PackedAdd<T>::add(acc.w, e.w);
+        acc.x = packed_add<T>(acc.x, e.x);
+        acc.y = packed_add<T>(acc.y, e.y);
+        acc.z = packed_add<T>(acc.z, e.z);
+        acc.w = packed_add<T>(acc.w, e.w);
     }
 
     const int x0 = x_lo + tx * VEC, y = y_lo + ty;
@@ -1115,9 +1046,6 @@ blend_grid_generic_kernel(const __grid_constant__ BlendParams p, const float* __
 // ---------------------------------------------------------------------------
 // Host-side dispatch
 // ---------------------------------------------------------------------------
-// magic = ceil(2^32 / d) for fastdiv(); 0 encodes d == 1
-unsigned magic_u16(unsigned d) { return d <= 1 ? 0u : (unsigned)(((1ull << 32) + d - 1) / d); }
-
 constexpr uint32_t kOptInForms = TD_FLAG_ROWS | TD_FLAG_STRIP | TD_FLAG_TMA | TD_FLAG_PIPELINE;
 
 // On an axis whose g->wrap bit is clear every tile must lie inside the canvas (the kernels of this file index the canvas
@@ -1159,44 +1087,10 @@ int fill_geom(const td_grid* g, int N, int C, GeomParams* o) {
     return TD_OK;
 }
 
-inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
-
-// Launch with the programmatic-stream-serialisation attribute (see pdl_wait): inside a stream or a captured graph
-// the kernel may start while its predecessor drains.  tl_pdl is set per C-ABI call from TD_FLAG_NO_PDL.
-thread_local bool tl_pdl = true;
-thread_local cudaError_t tl_launch_err = cudaSuccess;
-
-template <typename... KArgs, typename... Args>
-void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = grid;
-    cfg.blockDim = block;
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr = {};
-    attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr.val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = &attr;
-    cfg.numAttrs = tl_pdl ? 1 : 0;
-    const cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
-    if (e != cudaSuccess) tl_launch_err = e;   // reported by check_launch
-}
-
-int check_launch(const char* what) {
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = tl_launch_err;
-    tl_launch_err = cudaSuccess;
-    if (e != cudaSuccess) {
-        td_set_error("%s: CUDA launch failed: %s", what, cudaGetErrorString(e));
-        return TD_ERR_CUDA;
-    }
-    return TD_OK;
-}
-
 inline unsigned blocks_for(long long total, int threads) { return (unsigned)((total + threads - 1) / threads); }
 
 template <typename T>
-int launch_scatter(GeomParams gp, const void* x, void* tiles, int tile_begin, int n_tiles, bool vec, cudaStream_t st) {
+int launch_scatter(GeomParams gp, const void* x, void* tiles, int tile_begin, int n_tiles, bool vec, bool pdl, cudaStream_t st) {
     const long long elems = (long long)n_tiles * gp.N * gp.C * gp.th * gp.tw;
     if (elems == 0) return TD_OK;
     if (vec) {
@@ -1205,11 +1099,11 @@ int launch_scatter(GeomParams gp, const void* x, void* tiles, int tile_begin, in
         const int rows_per_block = std::max(1, std::min(gp.th, (128 * 4 + twv - 1) / twv));  // ~4 vectors per thread
         if ((long long)rows_per_block * twv >= 65536) { td_set_error("tile row too wide for the vector scatter"); return TD_ERR_UNSUPPORTED; }
         dim3 grid((unsigned)(n_tiles * gp.N * gp.C), (unsigned)((gp.th + rows_per_block - 1) / rows_per_block));
-        launch_pdl(scatter_vec_kernel<T>, grid, dim3(128), 0, st, gp, (const T*)x, (T*)tiles, tile_begin, rows_per_block);
-    } else {
-        scatter_generic_kernel<T><<<blocks_for(elems, 256), 256, 0, st>>>(gp, (const T*)x, (T*)tiles, tile_begin, elems);
+        return launch("td_scatter_tiles", scatter_vec_kernel<T>, grid, dim3(128), 0, st, pdl, gp, (const T*)x, (T*)tiles, tile_begin,
+                      rows_per_block);
     }
-    return check_launch("td_scatter_tiles");
+    scatter_generic_kernel<T><<<blocks_for(elems, 256), 256, 0, st>>>(gp, (const T*)x, (T*)tiles, tile_begin, elems);
+    return launch_status("td_scatter_tiles");
 }
 
 template <typename T, int MODE>
@@ -1225,7 +1119,7 @@ int launch_blend_vec(const BlendParams& bp, const float* weights, const float* t
         blend_grid_vec_kernel<T, MODE, true><<<grid, kBlendWarps * 32, 0, st>>>(bp, weights, tile_weights, rescale, out_f32, (T*)out_buf);
     else
         blend_grid_vec_kernel<T, MODE, false><<<grid, kBlendWarps * 32, 0, st>>>(bp, weights, tile_weights, rescale, out_f32, (T*)out_buf);
-    return check_launch("td_blend (vec)");
+    return launch_status("td_blend (vec)");
 }
 
 // max number of tile rows (cols) touching any BY-row (BX-px) patch: bounds the TMA stage count
@@ -1239,32 +1133,6 @@ int max_union(const int32_t* org, int n, int extent, int size, int patch) {
         best = std::max(best, cnt);
     }
     return best;
-}
-
-// dynamic shared memory a kernel may request without opting in (48 KB minus its static allocation, with margin)
-constexpr int kNoOptInSmem = 40 * 1024;
-
-// The opt-in above 48 KB of dynamic shared memory is a per-device function attribute: remember the size configured
-// for each device ordinal (a host may drive several GPUs from one process), set it under a lock.
-constexpr int kMaxDevices = 64;
-struct SmemOptIn {
-    std::atomic<int> bytes[kMaxDevices];
-    SmemOptIn() { for (auto& b : bytes) b.store(kNoOptInSmem, std::memory_order_relaxed); }
-};
-
-template <typename KernelT>
-int ensure_dyn_smem(KernelT kernel, int bytes, SmemOptIn* configured) {
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0) { td_set_error("cudaGetDevice failed"); return TD_ERR_CUDA; }
-    std::atomic<int>* slot = dev < kMaxDevices ? &configured->bytes[dev] : nullptr;
-    if (slot != nullptr && bytes <= slot->load(std::memory_order_acquire)) return TD_OK;
-    static std::mutex mu;
-    std::lock_guard<std::mutex> lk(mu);
-    if (slot != nullptr && bytes <= slot->load(std::memory_order_relaxed)) return TD_OK;
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-    if (e != cudaSuccess) { td_set_error("cudaFuncSetAttribute(%d B smem): %s", bytes, cudaGetErrorString(e)); return TD_ERR_CUDA; }
-    if (slot != nullptr) slot->store(bytes, std::memory_order_release);
-    return TD_OK;
 }
 
 template <typename T, bool WRITE_BUF, int NB>
@@ -1285,12 +1153,11 @@ int launch_blend_tma_nb(const td_grid* g, const BlendParams& bp, int tile_dtype,
         if (rc != TD_OK) return rc;
     }
     const int smem = nv_cap * (STAGE + 8);
-    static SmemOptIn configured;
-    int rc = ensure_dyn_smem(blend_md_tma_kernel<T, WRITE_BUF, NB>, smem, &configured);
+    int rc = smem_optin(blend_md_tma_kernel<T, WRITE_BUF, NB>, smem, "td_blend_multidiffusion (tma)");
     if (rc != TD_OK) return rc;
     dim3 grid((unsigned)((bp.g.W + BX - 1) / BX), (unsigned)((bp.g.H + kTmaBY - 1) / kTmaBY), (unsigned)NC);
     blend_md_tma_kernel<T, WRITE_BUF, NB><<<grid, kTmaThreads, smem, st>>>(tp, weights, out_f32, (T*)out_buf);
-    return check_launch("td_blend_multidiffusion (tma)");
+    return launch_status("td_blend_multidiffusion (tma)");
 }
 
 // returns TD_OK if launched, 1 if the TMA path does not apply (caller falls back), <0 on error
@@ -1324,65 +1191,53 @@ void fill_patch_table(const int32_t* org, int n, int extent, int size, int patch
     }
 }
 
-int sm_count() {
-    static int n = [] {
-        int dev = 0, v = 0;
-        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;
-        return v;
-    }();
-    return n;
-}
-
 template <typename T, bool WRITE_BUF, bool FASTDIV, int PPC>
 int launch_blend_async_ppc(const BlendParams& bp, const float* weights, const float* rcp_weights, float* out_f32, void* out_buf,
-                           int nv_cap, cudaStream_t st) {
+                           int nv_cap, bool pdl, cudaStream_t st) {
     constexpr int VEC = Vec<T>::kElems;
     constexpr int BX = kAsX * VEC;
     const int px = (bp.g.W + BX - 1) / BX, py = (bp.g.H + kAsY - 1) / kAsY, planes = bp.g.N * bp.g.C;
     const int smem = nv_cap * PPC * kAsStage;
-    static SmemOptIn configured;
-    int rc = ensure_dyn_smem(blend_md_async_kernel<T, WRITE_BUF, FASTDIV, PPC>, smem, &configured);
+    const char* what = "td_blend_multidiffusion (cp.async)";
+    int rc = smem_optin(blend_md_async_kernel<T, WRITE_BUF, FASTDIV, PPC>, smem, what);
     if (rc != TD_OK) return rc;
     const unsigned gy = (unsigned)(bp.py_count > 0 ? bp.py_count : py), gz = (unsigned)(planes / PPC);
     dim3 grid((unsigned)px, bp.sched ? gz : gy, bp.sched ? gy : gz);
-    launch_pdl(blend_md_async_kernel<T, WRITE_BUF, FASTDIV, PPC>, grid, dim3(kAsThreads), (size_t)smem, st, bp, weights, rcp_weights,
-               out_f32, (T*)out_buf);
-    return TD_OK;
+    return launch(what, blend_md_async_kernel<T, WRITE_BUF, FASTDIV, PPC>, grid, dim3(kAsThreads), (size_t)smem, st, pdl, bp, weights,
+                  rcp_weights, out_f32, (T*)out_buf);
 }
 
-// planes per CTA (tl_ppc_max is set per C-ABI call: TD_FLAG_ONE_PLANE forces 1)
+// planes per CTA: at most TD_AS_PPC, 1 under TD_FLAG_ONE_PLANE (ppc_max)
 #ifndef TD_AS_PPC
 #define TD_AS_PPC 1   // tuning knob (-DTD_AS_PPC=): 1 / 2 / 4; cfg2 blend 12.5 us at 1 vs 13.35 us at 2 (H100 80GB HBM3, 700 W)
 #endif
-thread_local int tl_ppc_max = TD_AS_PPC;
+int ppc_max(uint32_t flags) { return (flags & TD_FLAG_ONE_PLANE) ? 1 : TD_AS_PPC; }
 
 template <typename T, bool WRITE_BUF, bool FASTDIV>
 int launch_blend_async_impl(const BlendParams& bp, const float* weights, const float* rcp_weights, float* out_f32, void* out_buf,
-                            int nv_cap, bool pipelined, cudaStream_t st) {
+                            int nv_cap, bool pipelined, bool pdl, int max_ppc, cudaStream_t st) {
     constexpr int VEC = Vec<T>::kElems;
     constexpr int BX = kAsX * VEC;
     const int px = (bp.g.W + BX - 1) / BX, py = (bp.g.H + kAsY - 1) / kAsY, planes = bp.g.N * bp.g.C;
     if (pipelined) {
         const int smem = 2 * nv_cap * kAsStage;
-        static SmemOptIn configured;
-        int rc = ensure_dyn_smem(blend_md_pipe_kernel<T, WRITE_BUF, FASTDIV>, smem, &configured);
+        const char* what = "td_blend_multidiffusion (cp.async)";
+        int rc = smem_optin(blend_md_pipe_kernel<T, WRITE_BUF, FASTDIV>, smem, what);
         if (rc != TD_OK) return rc;
         const long long total = (long long)px * py * planes;
         const int per_sm = std::max(1, std::min(8, (220 * 1024) / (smem + 3 * 1024)));   // CTAs that fit one SM's shared memory
-        const int grid = (int)std::min<long long>(total, (long long)sm_count() * per_sm);
+        const DeviceProps dev = device_props();
+        const int sms = dev.ok ? dev.sms : 132;                                            // an H100's count when the query fails
+        const int grid = (int)std::min<long long>(total, (long long)sms * per_sm);
         blend_md_pipe_kernel<T, WRITE_BUF, FASTDIV><<<grid, kAsThreads, smem, st>>>(bp, weights, rcp_weights, out_f32, (T*)out_buf, nv_cap,
                                                                                    px, py, (int)total);
-    } else {
-        int rc;
-        if (tl_ppc_max >= 4 && planes % 4 == 0 && 4 * nv_cap * kAsStage <= 64 * 1024)
-            rc = launch_blend_async_ppc<T, WRITE_BUF, FASTDIV, 4>(bp, weights, rcp_weights, out_f32, out_buf, nv_cap, st);
-        else if (tl_ppc_max >= 2 && planes % 2 == 0 && 2 * nv_cap * kAsStage <= 64 * 1024)
-            rc = launch_blend_async_ppc<T, WRITE_BUF, FASTDIV, 2>(bp, weights, rcp_weights, out_f32, out_buf, nv_cap, st);
-        else
-            rc = launch_blend_async_ppc<T, WRITE_BUF, FASTDIV, 1>(bp, weights, rcp_weights, out_f32, out_buf, nv_cap, st);
-        if (rc != TD_OK) return rc;
+        return launch_status(what);
     }
-    return check_launch("td_blend_multidiffusion (cp.async)");
+    if (max_ppc >= 4 && planes % 4 == 0 && 4 * nv_cap * kAsStage <= 64 * 1024)
+        return launch_blend_async_ppc<T, WRITE_BUF, FASTDIV, 4>(bp, weights, rcp_weights, out_f32, out_buf, nv_cap, pdl, st);
+    if (max_ppc >= 2 && planes % 2 == 0 && 2 * nv_cap * kAsStage <= 64 * 1024)
+        return launch_blend_async_ppc<T, WRITE_BUF, FASTDIV, 2>(bp, weights, rcp_weights, out_f32, out_buf, nv_cap, pdl, st);
+    return launch_blend_async_ppc<T, WRITE_BUF, FASTDIV, 1>(bp, weights, rcp_weights, out_f32, out_buf, nv_cap, pdl, st);
 }
 
 // Row-strip shard (patch tables filled): only the CTAs that read a neighbour's band wait; they sit at the end of the row range
@@ -1400,7 +1255,7 @@ void schedule_halo_waits_last(BlendParams& bp) {
 
 template <typename T, bool WRITE_BUF>
 int launch_blend_async(const td_grid* g, const BlendParams& bp_in, const float* weights, const float* rcp_weights, float* out_f32,
-                       void* out_buf, int nv_cap, bool pipelined, cudaStream_t st) {
+                       void* out_buf, int nv_cap, bool pipelined, bool pdl, int max_ppc, cudaStream_t st) {
     constexpr int VEC = Vec<T>::kElems;
     constexpr int BX = kAsX * VEC;
     BlendParams bp = bp_in;
@@ -1408,47 +1263,46 @@ int launch_blend_async(const td_grid* g, const BlendParams& bp_in, const float* 
     fill_patch_table(g->xs, g->cols, g->tile_w, g->W, BX, bp.pcol_lo, bp.pcol_n);
     if (!pipelined) schedule_halo_waits_last(bp);
     if (rcp_weights != nullptr && sizeof(T) == 2)
-        return launch_blend_async_impl<T, WRITE_BUF, true>(bp, weights, rcp_weights, out_f32, out_buf, nv_cap, pipelined, st);
-    return launch_blend_async_impl<T, WRITE_BUF, false>(bp, weights, nullptr, out_f32, out_buf, nv_cap, pipelined, st);
+        return launch_blend_async_impl<T, WRITE_BUF, true>(bp, weights, rcp_weights, out_f32, out_buf, nv_cap, pipelined, pdl, max_ppc, st);
+    return launch_blend_async_impl<T, WRITE_BUF, false>(bp, weights, nullptr, out_f32, out_buf, nv_cap, pipelined, pdl, max_ppc, st);
 }
 
 template <typename T, bool WINDOW>
-int launch_blend_mod_async(const BlendParams& bp, int smem, const float* tile_weights, const float* rescale, void* out_buf, cudaStream_t st) {
+int launch_blend_mod_async(const BlendParams& bp, int smem, const float* tile_weights, const float* rescale, void* out_buf, bool pdl,
+                           cudaStream_t st) {
     constexpr int BX = kAsX * Vec<T>::kElems;
-    static SmemOptIn configured;
-    int rc = ensure_dyn_smem(blend_mod_async_kernel<T, WINDOW>, smem, &configured);
+    const char* what = "td_blend_mixture (cp.async)";
+    int rc = smem_optin(blend_mod_async_kernel<T, WINDOW>, smem, what);
     if (rc != TD_OK) return rc;
     const unsigned gy = (unsigned)(WINDOW ? bp.py_count : (bp.g.H + kAsY - 1) / kAsY), gz = (unsigned)(bp.g.N * bp.g.C);
     dim3 grid((unsigned)((bp.g.W + BX - 1) / BX), bp.sched ? gz : gy, bp.sched ? gy : gz);
-    launch_pdl(blend_mod_async_kernel<T, WINDOW>, grid, dim3(kAsThreads), (size_t)smem, st, bp, tile_weights, rescale, (T*)out_buf);
-    return TD_OK;
+    return launch(what, blend_mod_async_kernel<T, WINDOW>, grid, dim3(kAsThreads), (size_t)smem, st, pdl, bp, tile_weights, rescale,
+                  (T*)out_buf);
 }
 
 // Mixture of Diffusers on the cp.async kernel; 0 launched, 1 not applicable, <0 error
 template <typename T>
 int try_launch_blend_mod_async(const td_grid* g, const BlendParams& bp_in, const float* tile_weights, const float* rescale, void* out_buf,
-                               cudaStream_t st) {
+                               bool pdl, cudaStream_t st) {
     constexpr int VEC = Vec<T>::kElems;
     constexpr int BX = kAsX * VEC;
     if (bp_in.g.N * bp_in.g.C > 65535 || (bp_in.g.H + kAsY - 1) / kAsY > 65535 || bp_in.tile_stride >= (1ll << 31)) return 1;
     if ((bp_in.g.H + kAsY - 1) / kAsY > TD_MAX_GRID_DIM || (bp_in.g.W + BX - 1) / BX > TD_MAX_GRID_DIM) return 1;
-    if ((reinterpret_cast<uintptr_t>(tile_weights) & 15u) != 0 || (bp_in.g.tw & 7) != 0) return 1;
+    if (!aligned16(tile_weights) || (bp_in.g.tw & 7) != 0) return 1;
     const int nv_cap = max_union(g->ys, g->rows, g->tile_h, g->H, kAsY) * max_union(g->xs, g->cols, g->tile_w, g->W, BX);
     if (nv_cap <= 0 || nv_cap > kAsMaxVisits || nv_cap > kAsThreads || nv_cap * kAsStage > 200 * 1024) return 1;
     BlendParams bp = bp_in;
     fill_patch_table(g->ys, g->rows, g->tile_h, g->H, kAsY, bp.prow_lo, bp.prow_n);
     fill_patch_table(g->xs, g->cols, g->tile_w, g->W, BX, bp.pcol_lo, bp.pcol_n);
     schedule_halo_waits_last(bp);
-    const int rc = bp.py_count > 0 ? launch_blend_mod_async<T, true>(bp, nv_cap * kAsStage, tile_weights, rescale, out_buf, st)
-                                   : launch_blend_mod_async<T, false>(bp, nv_cap * kAsStage, tile_weights, rescale, out_buf, st);
-    if (rc != TD_OK) return rc;
-    return check_launch("td_blend_mixture (cp.async)");
+    return bp.py_count > 0 ? launch_blend_mod_async<T, true>(bp, nv_cap * kAsStage, tile_weights, rescale, out_buf, pdl, st)
+                           : launch_blend_mod_async<T, false>(bp, nv_cap * kAsStage, tile_weights, rescale, out_buf, pdl, st);
 }
 
 // returns TD_OK if launched, 1 if the path does not apply (caller falls back), <0 on error
 template <typename T>
 int try_launch_blend_async(const td_grid* g, const BlendParams& bp, const float* weights, const float* rcp_weights, float* out_f32,
-                           void* out_buf, bool pipelined, cudaStream_t st) {
+                           void* out_buf, bool pipelined, bool pdl, int max_ppc, cudaStream_t st) {
     constexpr int VEC = Vec<T>::kElems;
     constexpr int BX = kAsX * VEC;
     if (bp.g.N * bp.g.C > 65535 || (bp.g.H + kAsY - 1) / kAsY > 65535) return 1;
@@ -1457,8 +1311,8 @@ int try_launch_blend_async(const td_grid* g, const BlendParams& bp, const float*
     if (nv_cap <= 0 || nv_cap > kAsMaxVisits || nv_cap > kAsThreads || nv_cap * kAsStage > 200 * 1024) return 1;
     if ((bp.g.H + kAsY - 1) / kAsY > TD_MAX_GRID_DIM || (bp.g.W + BX - 1) / BX > TD_MAX_GRID_DIM) return 1;   // patch tables
     if (pipelined && 2 * nv_cap * kAsStage > 200 * 1024) pipelined = false;
-    return out_buf != nullptr ? launch_blend_async<T, true>(g, bp, weights, rcp_weights, out_f32, out_buf, nv_cap, pipelined, st)
-                              : launch_blend_async<T, false>(g, bp, weights, rcp_weights, out_f32, out_buf, nv_cap, pipelined, st);
+    return out_buf != nullptr ? launch_blend_async<T, true>(g, bp, weights, rcp_weights, out_f32, out_buf, nv_cap, pipelined, pdl, max_ppc, st)
+                              : launch_blend_async<T, false>(g, bp, weights, rcp_weights, out_f32, out_buf, nv_cap, pipelined, pdl, max_ppc, st);
 }
 
 template <typename TIn, typename TAcc, int MODE>
@@ -1468,7 +1322,7 @@ int launch_blend_generic(const BlendParams& bp, const float* weights, const floa
     const long long total = (long long)g.N * g.C * g.H * g.W;
     blend_grid_generic_kernel<TIn, TAcc, MODE><<<blocks_for(total, 256), 256, 0, st>>>(bp, weights, tile_weights, rescale,
                                                                                        out_f32, (TAcc*)out_buf, total);
-    return check_launch("td_blend (generic)");
+    return launch_status("td_blend (generic)");
 }
 
 template <int MODE>
@@ -1547,7 +1401,7 @@ __global__ void empty_kernel() {}
 extern "C" int td_debug_launch_empty(int blocks, int threads, void* stream) {
     if (blocks <= 0 || threads <= 0 || threads > 1024) { td_set_error("td_debug_launch_empty: bad launch shape"); return TD_ERR_INVALID_ARG; }
     empty_kernel<<<blocks, threads, 0, (cudaStream_t)stream>>>();
-    return check_launch("td_debug_launch_empty");
+    return launch_status("td_debug_launch_empty");
 }
 
 extern "C" int td_scatter_tiles(const td_grid* g, const void* x, void* tiles, int N, int C, int dtype, int tile_begin,
@@ -1564,25 +1418,24 @@ extern "C" int td_scatter_tiles(const td_grid* g, const void* x, void* tiles, in
     const int es = td_dtype_size(dtype);
     if (es == 0) { td_set_error("td_scatter_tiles: unknown dtype %d", dtype); return TD_ERR_INVALID_ARG; }
     const int vec = 16 / es;
-    tl_pdl = !(flags & TD_FLAG_NO_PDL);
+    const bool pdl = !(flags & TD_FLAG_NO_PDL);
     const bool vec_ok = !(flags & TD_FLAG_FORCE_GENERIC) && gp.W % vec == 0 && gp.tw % vec == 0 && aligned16(x) && aligned16(tiles);
-    if (g->wrap) return td_wrap_scatter(g, x, tiles, N, C, dtype, tile_begin, tile_end, vec_ok, tl_pdl, stream);
+    if (g->wrap) return td_wrap_scatter(g, x, tiles, N, C, dtype, tile_begin, tile_end, vec_ok, pdl, stream);
     cudaStream_t s = (cudaStream_t)stream;
     if (vec_ok && !(flags & TD_FLAG_NO_TMA)) {   // default: row-block form (td_rows.cu); falls through when not applicable
         const int rc = td_rows_try_launch_scatter(g, x, tiles, N, C, dtype, tile_begin, tile_end, (flags & TD_FLAG_NO_PDL) ? 0 : 1, stream);
         if (rc <= 0) return rc;
     }
     // fp16 and bf16 are both moved as opaque 16-bit words
-    if (es == 2) return launch_scatter<__half>(gp, x, tiles, tile_begin, tile_end - tile_begin, vec_ok, s);
-    return launch_scatter<float>(gp, x, tiles, tile_begin, tile_end - tile_begin, vec_ok, s);
+    if (es == 2) return launch_scatter<__half>(gp, x, tiles, tile_begin, tile_end - tile_begin, vec_ok, pdl, s);
+    return launch_scatter<float>(gp, x, tiles, tile_begin, tile_end - tile_begin, vec_ok, pdl, s);
 }
 
 extern "C" int td_blend_multidiffusion(const td_grid* g, const void* const* batch_ptrs, int num_batches, int tile_bs, int N,
                                        int C, int tile_dtype, int acc_dtype, const float* weights, const float* rcp_weights,
                                        float* x_out, void* x_buffer, uint32_t flags, void* stream) {
     BlendParams bp;
-    tl_pdl = !(flags & TD_FLAG_NO_PDL);
-    tl_ppc_max = (flags & TD_FLAG_ONE_PLANE) ? 1 : TD_AS_PPC;
+    const bool pdl = !(flags & TD_FLAG_NO_PDL);
     int st = fill_blend(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, &bp);
     if (st != TD_OK) return st;
     if (weights == nullptr || x_out == nullptr) { td_set_error("td_blend_multidiffusion: null weights / x_out"); return TD_ERR_INVALID_ARG; }
@@ -1590,7 +1443,7 @@ extern "C" int td_blend_multidiffusion(const td_grid* g, const void* const* batc
     const bool vec_ok = !(flags & TD_FLAG_FORCE_GENERIC) && blend_vec_ok(bp, tile_dtype, acc_dtype, {weights, rcp_weights, x_out, x_buffer});
     if (g->wrap)
         return td_wrap_blend(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, 0, weights, nullptr, nullptr, x_out, x_buffer,
-                             vec_ok, tl_pdl, stream);
+                             vec_ok, pdl, stream);
     bp.g.dbg_no_tiles = (flags & TD_FLAG_DBG_NO_TILES) ? 1 : 0;
     cudaStream_t s = (cudaStream_t)stream;
     if (vec_ok) {
@@ -1615,9 +1468,9 @@ extern "C" int td_blend_multidiffusion(const td_grid* g, const void* const* batc
         } else if (!(flags & TD_FLAG_NO_TMA)) {
             const bool pipe = (flags & TD_FLAG_PIPELINE) != 0;   // opt-in (see the comment above the kernel)
             switch (tile_dtype) {
-                case TD_F16: rc = try_launch_blend_async<__half>(g, bp, weights, rcp_weights, x_out, x_buffer, pipe, s); break;
-                case TD_BF16: rc = try_launch_blend_async<__nv_bfloat16>(g, bp, weights, rcp_weights, x_out, x_buffer, pipe, s); break;
-                default: rc = try_launch_blend_async<float>(g, bp, weights, nullptr, x_out, x_buffer, pipe, s); break;
+                case TD_F16: rc = try_launch_blend_async<__half>(g, bp, weights, rcp_weights, x_out, x_buffer, pipe, pdl, ppc_max(flags), s); break;
+                case TD_BF16: rc = try_launch_blend_async<__nv_bfloat16>(g, bp, weights, rcp_weights, x_out, x_buffer, pipe, pdl, ppc_max(flags), s); break;
+                default: rc = try_launch_blend_async<float>(g, bp, weights, nullptr, x_out, x_buffer, pipe, pdl, ppc_max(flags), s); break;
             }
         }
         if (rc <= 0) return rc;   // launched or hard error; 1 = not applicable -> register-staged kernel
@@ -1671,8 +1524,7 @@ extern "C" int td_blend_multidiffusion_rows(const td_grid* g, const void* const*
                                             int wait_count, const uint32_t* wait_value, int own_band_begin, int own_band_end,
                                             uint32_t flags, void* stream) {
     BlendParams bp;
-    tl_pdl = !(flags & TD_FLAG_NO_PDL);
-    tl_ppc_max = (flags & TD_FLAG_ONE_PLANE) ? 1 : TD_AS_PPC;
+    const bool pdl = !(flags & TD_FLAG_NO_PDL);
     int st = fill_blend(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, &bp);
     if (st != TD_OK) return st;
     if ((st = refuse_wrapped(g, "td_blend_multidiffusion_rows")) != TD_OK) return st;
@@ -1683,9 +1535,9 @@ extern "C" int td_blend_multidiffusion_rows(const td_grid* g, const void* const*
     cudaStream_t s = (cudaStream_t)stream;
     int rc;
     switch (tile_dtype) {
-        case TD_F16: rc = try_launch_blend_async<__half>(g, bp, weights, rcp_weights, x_out, x_buffer, false, s); break;
-        case TD_BF16: rc = try_launch_blend_async<__nv_bfloat16>(g, bp, weights, rcp_weights, x_out, x_buffer, false, s); break;
-        default: rc = try_launch_blend_async<float>(g, bp, weights, nullptr, x_out, x_buffer, false, s); break;
+        case TD_F16: rc = try_launch_blend_async<__half>(g, bp, weights, rcp_weights, x_out, x_buffer, false, pdl, ppc_max(flags), s); break;
+        case TD_BF16: rc = try_launch_blend_async<__nv_bfloat16>(g, bp, weights, rcp_weights, x_out, x_buffer, false, pdl, ppc_max(flags), s); break;
+        default: rc = try_launch_blend_async<float>(g, bp, weights, nullptr, x_out, x_buffer, false, pdl, ppc_max(flags), s); break;
     }
     if (rc == 1) { td_set_error("td_blend_multidiffusion_rows: geometry outside the cp.async kernel's limits"); return TD_ERR_UNSUPPORTED; }
     return rc;
@@ -1698,7 +1550,7 @@ extern "C" int td_debug_check_fast_div(int dtype, int max_w, unsigned long long*
     }
     if (dtype == TD_F16) check_fast_div_kernel<__half><<<256, 256, 0, (cudaStream_t)stream>>>(max_w, mismatches_dev);
     else check_fast_div_kernel<__nv_bfloat16><<<256, 256, 0, (cudaStream_t)stream>>>(max_w, mismatches_dev);
-    return check_launch("td_debug_check_fast_div");
+    return launch_status("td_debug_check_fast_div");
 }
 
 extern "C" int td_blend_multidiffusion_peer(const td_grid* g, const void* const* batch_ptrs, int num_batches, int tile_bs, int N,
@@ -1706,8 +1558,7 @@ extern "C" int td_blend_multidiffusion_peer(const td_grid* g, const void* const*
                                             void* x_buffer, const uint32_t* wait_flags, int world, const uint32_t* wait_value,
                                             uint32_t flags, void* stream) {
     BlendParams bp;
-    tl_pdl = !(flags & TD_FLAG_NO_PDL);
-    tl_ppc_max = (flags & TD_FLAG_ONE_PLANE) ? 1 : TD_AS_PPC;
+    const bool pdl = !(flags & TD_FLAG_NO_PDL);
     int st = fill_blend(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, &bp);
     if (st != TD_OK) return st;
     if ((st = refuse_wrapped(g, "td_blend_multidiffusion_peer")) != TD_OK) return st;
@@ -1722,9 +1573,9 @@ extern "C" int td_blend_multidiffusion_peer(const td_grid* g, const void* const*
     if (flags & TD_FLAG_PEER_ASYNC) {   // cp.async-staged kernel over peer pointers: measured slower over NVLink than direct loads (opt-in)
         int rc;
         switch (tile_dtype) {
-            case TD_F16: rc = try_launch_blend_async<__half>(g, bp, weights, nullptr, x_out, x_buffer, false, s); break;
-            case TD_BF16: rc = try_launch_blend_async<__nv_bfloat16>(g, bp, weights, nullptr, x_out, x_buffer, false, s); break;
-            default: rc = try_launch_blend_async<float>(g, bp, weights, nullptr, x_out, x_buffer, false, s); break;
+            case TD_F16: rc = try_launch_blend_async<__half>(g, bp, weights, nullptr, x_out, x_buffer, false, pdl, ppc_max(flags), s); break;
+            case TD_BF16: rc = try_launch_blend_async<__nv_bfloat16>(g, bp, weights, nullptr, x_out, x_buffer, false, pdl, ppc_max(flags), s); break;
+            default: rc = try_launch_blend_async<float>(g, bp, weights, nullptr, x_out, x_buffer, false, pdl, ppc_max(flags), s); break;
         }
         if (rc <= 0) return rc;
     }
@@ -1739,8 +1590,7 @@ extern "C" int td_blend_mixture(const td_grid* g, const void* const* batch_ptrs,
                                 int tile_dtype, int acc_dtype, const float* tile_weights, const float* rescale,
                                 void* x_buffer, uint32_t flags, void* stream) {
     BlendParams bp;
-    tl_pdl = !(flags & TD_FLAG_NO_PDL);
-    tl_ppc_max = (flags & TD_FLAG_ONE_PLANE) ? 1 : TD_AS_PPC;
+    const bool pdl = !(flags & TD_FLAG_NO_PDL);
     int st = fill_blend(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, &bp);
     if (st != TD_OK) return st;
     if (tile_weights == nullptr || rescale == nullptr || x_buffer == nullptr) {
@@ -1751,7 +1601,7 @@ extern "C" int td_blend_mixture(const td_grid* g, const void* const* batch_ptrs,
     const bool vec_ok = !(flags & TD_FLAG_FORCE_GENERIC) && blend_vec_ok(bp, tile_dtype, acc_dtype, {rescale, x_buffer});
     if (g->wrap)
         return td_wrap_blend(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, 1, nullptr, tile_weights, rescale, nullptr,
-                             x_buffer, vec_ok, tl_pdl, stream);
+                             x_buffer, vec_ok, pdl, stream);
     cudaStream_t s = (cudaStream_t)stream;
     if (vec_ok) {
         if (flags & TD_FLAG_ROWS) {   // opt-in: row-block form (td_rows.cu)
@@ -1767,9 +1617,9 @@ extern "C" int td_blend_mixture(const td_grid* g, const void* const* batch_ptrs,
         if (!(flags & TD_FLAG_NO_TMA)) {
             int rc;
             switch (tile_dtype) {
-                case TD_F16: rc = try_launch_blend_mod_async<__half>(g, bp, tile_weights, rescale, x_buffer, s); break;
-                case TD_BF16: rc = try_launch_blend_mod_async<__nv_bfloat16>(g, bp, tile_weights, rescale, x_buffer, s); break;
-                default: rc = try_launch_blend_mod_async<float>(g, bp, tile_weights, rescale, x_buffer, s); break;
+                case TD_F16: rc = try_launch_blend_mod_async<__half>(g, bp, tile_weights, rescale, x_buffer, pdl, s); break;
+                case TD_BF16: rc = try_launch_blend_mod_async<__nv_bfloat16>(g, bp, tile_weights, rescale, x_buffer, pdl, s); break;
+                default: rc = try_launch_blend_mod_async<float>(g, bp, tile_weights, rescale, x_buffer, pdl, s); break;
             }
             if (rc <= 0) return rc;   // launched or hard error; 1 = not applicable -> register-staged kernel
         }
@@ -1787,7 +1637,7 @@ extern "C" int td_blend_mixture_rows(const td_grid* g, const void* const* batch_
                                      int row_begin, int row_end, const uint32_t* wait_flags, int wait_count, const uint32_t* wait_value,
                                      int own_band_begin, int own_band_end, uint32_t flags, void* stream) {
     BlendParams bp;
-    tl_pdl = !(flags & TD_FLAG_NO_PDL);
+    const bool pdl = !(flags & TD_FLAG_NO_PDL);
     int st = fill_blend(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, &bp);
     if (st != TD_OK) return st;
     if ((st = refuse_wrapped(g, "td_blend_mixture_rows")) != TD_OK) return st;
@@ -1801,9 +1651,9 @@ extern "C" int td_blend_mixture_rows(const td_grid* g, const void* const* batch_
     cudaStream_t s = (cudaStream_t)stream;
     int rc;
     switch (tile_dtype) {
-        case TD_F16: rc = try_launch_blend_mod_async<__half>(g, bp, tile_weights, rescale, x_buffer, s); break;
-        case TD_BF16: rc = try_launch_blend_mod_async<__nv_bfloat16>(g, bp, tile_weights, rescale, x_buffer, s); break;
-        default: rc = try_launch_blend_mod_async<float>(g, bp, tile_weights, rescale, x_buffer, s); break;
+        case TD_F16: rc = try_launch_blend_mod_async<__half>(g, bp, tile_weights, rescale, x_buffer, pdl, s); break;
+        case TD_BF16: rc = try_launch_blend_mod_async<__nv_bfloat16>(g, bp, tile_weights, rescale, x_buffer, pdl, s); break;
+        default: rc = try_launch_blend_mod_async<float>(g, bp, tile_weights, rescale, x_buffer, pdl, s); break;
     }
     if (rc == 1) { td_set_error("td_blend_mixture_rows: geometry outside the cp.async kernel's limits"); return TD_ERR_UNSUPPORTED; }
     return rc;
@@ -1816,7 +1666,7 @@ static int wrap_rows_entry(const td_grid* g, const void* const* batch_ptrs, int 
                            void* x_buffer, int row_begin, int row_end, const uint32_t* wait_flags, int wait_count,
                            const uint32_t* wait_value, int own_band_begin, int own_band_end, uint32_t flags, void* stream, const char* what) {
     BlendParams bp;
-    tl_pdl = !(flags & TD_FLAG_NO_PDL);
+    const bool pdl = !(flags & TD_FLAG_NO_PDL);
     int st = fill_blend(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, &bp);
     if (st != TD_OK) return st;
     if (g->wrap == 0) {
@@ -1835,7 +1685,7 @@ static int wrap_rows_entry(const td_grid* g, const void* const* batch_ptrs, int 
     if (st != TD_OK) return st == 1 ? TD_OK : st;
     return td_wrap_blend_rows(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, mixture, weights, tile_weights, rescale, x_out, x_buffer,
                               row_begin, row_end, wait_count > 0 ? wait_flags : nullptr, wait_count, wait_value, own_band_begin,
-                              own_band_end, tl_pdl, stream);
+                              own_band_end, pdl, stream);
 }
 
 extern "C" int td_blend_multidiffusion_wrap_rows(const td_grid* g, const void* const* batch_ptrs, int num_batches, int tile_bs, int N, int C,

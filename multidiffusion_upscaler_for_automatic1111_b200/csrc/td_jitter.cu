@@ -19,6 +19,7 @@
 #include "td_b200.h"
 #include "td_device.cuh"
 #include "td_internal.h"
+#include "td_launch.h"
 
 namespace {
 
@@ -171,11 +172,6 @@ combine_offset_kernel(const __grid_constant__ CombineOffsetParams p, const T* __
         out[e] = combine_offset_elem<T>(p, x_local, e);
 }
 
-int launched(const char* what) {
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { td_set_error("%s: CUDA launch failed: %s", what, cudaGetErrorString(e)); return TD_ERR_CUDA; }
-    return TD_OK;
-}
 
 unsigned blocks_for(long long total) { return (unsigned)std::max(1LL, std::min((total + 255) / 256, 148LL * 32)); }
 
@@ -208,7 +204,7 @@ extern "C" int td_scatter_bboxes(const void* x, void* tiles, const int32_t* orig
     if (es == 2) scatter_bboxes_kernel<uint16_t><<<blocks_for(total), 256, 0, st>>>((const uint16_t*)x, (uint16_t*)tiles, origins_dev, N * C, H, W, tile_h, tile_w, total);
     else if (es == 4) scatter_bboxes_kernel<uint32_t><<<blocks_for(total), 256, 0, st>>>((const uint32_t*)x, (uint32_t*)tiles, origins_dev, N * C, H, W, tile_h, tile_w, total);
     else { td_set_error("td_scatter_bboxes: unknown dtype"); return TD_ERR_INVALID_ARG; }
-    return launched("td_scatter_bboxes");
+    return launch_status("td_scatter_bboxes");
 }
 
 extern "C" int td_blend_bboxes(const void* const* batch_ptrs, int num_batches, int tile_bs, const int32_t* origins_dev,
@@ -234,7 +230,7 @@ extern "C" int td_blend_bboxes(const void* const* batch_ptrs, int num_batches, i
     else if (dtype == TD_BF16) blend_bboxes_kernel<__nv_bfloat16><<<blocks_for(total), 256, 0, st>>>(p, origins_dev, out);
     else if (dtype == TD_F32) blend_bboxes_kernel<float><<<blocks_for(total), 256, 0, st>>>(p, origins_dev, out);
     else { td_set_error("td_blend_bboxes: unknown dtype"); return TD_ERR_INVALID_ARG; }
-    return launched("td_blend_bboxes");
+    return launch_status("td_blend_bboxes");
 }
 
 extern "C" int td_demofusion_combine_offset(const void* x_local, const void* const* view_batch_ptrs, int num_batches,
@@ -266,7 +262,7 @@ extern "C" int td_demofusion_combine_offset(const void* x_local, const void* con
     else if (dtype == TD_BF16) combine_offset_kernel<__nv_bfloat16><<<blocks_for(total), 256, 0, st>>>(p, (const __nv_bfloat16*)x_local, (__nv_bfloat16*)out);
     else if (dtype == TD_F32) combine_offset_kernel<float><<<blocks_for(total), 256, 0, st>>>(p, (const float*)x_local, (float*)out);
     else { td_set_error("td_demofusion_combine_offset: unknown dtype"); return TD_ERR_INVALID_ARG; }
-    return launched("td_demofusion_combine_offset");
+    return launch_status("td_demofusion_combine_offset");
 }
 
 #ifdef TD_JITTER_HOST_EMULATION

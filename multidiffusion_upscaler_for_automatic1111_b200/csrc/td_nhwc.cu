@@ -22,6 +22,7 @@
 #include "td_b200.h"
 #include "td_device.cuh"
 #include "td_internal.h"
+#include "td_launch.h"
 
 namespace {
 
@@ -29,23 +30,9 @@ using namespace td;
 
 constexpr int kNhwcThreads = 256;
 
-int nhwc_check(const char* what) {
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) {
-        td_set_error("%s: CUDA launch failed: %s", what, cudaGetErrorString(e));
-        return TD_ERR_CUDA;
-    }
-    return TD_OK;
-}
-
-int nhwc_sms() {
-    static int sms = 0;
-    if (sms == 0) {
-        int dev = 0, n = 0;
-        if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess) sms = n;
-        else sms = 132;
-    }
-    return sms;
+int nhwc_sms() {   // grid sizing only: an H100's count when the query fails
+    const DeviceProps d = device_props();
+    return d.ok ? d.sms : 132;
 }
 
 template <typename T> __device__ __forceinline__ float vget(const uint4& v, int j) { return Vec<T>::get(v, j); }
@@ -336,7 +323,7 @@ extern "C" int td_nchw_to_nhwc(const void* x, void* y, int N, int C, int rows, i
         nchw_to_nhwc_kernel<__half><<<grid, kNhwcThreads, 0, (cudaStream_t)stream>>>((const __half*)x, (__half*)y, C, x_plane_stride, x_pitch, x_img_stride, rows, cols, Cpad, total);
     else
         nchw_to_nhwc_kernel<__nv_bfloat16><<<grid, kNhwcThreads, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)y, C, x_plane_stride, x_pitch, x_img_stride, rows, cols, Cpad, total);
-    return nhwc_check("td_nchw_to_nhwc");
+    return launch_status("td_nchw_to_nhwc");
 }
 
 extern "C" int td_nchw_to_nhwc_wrap(const void* x, void* y, int N, int C, int rows, int cols, int row0, int col0, int H, int W,
@@ -355,7 +342,7 @@ extern "C" int td_nchw_to_nhwc_wrap(const void* x, void* y, int N, int C, int ro
         nchw_to_nhwc_wrap_kernel<__nv_bfloat16><<<grid, kNhwcThreads, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)y, C,
                                                                                                x_plane_stride, x_pitch, x_img_stride, rows, cols,
                                                                                                row0, col0, H, W, Cpad, total);
-    return nhwc_check("td_nchw_to_nhwc_wrap");
+    return launch_status("td_nchw_to_nhwc_wrap");
 }
 
 extern "C" int td_nhwc_to_nchw_region(const void* x, void* y, int N, int C, int rows, int cols, int64_t x_img_stride, int x_width,
@@ -369,7 +356,7 @@ extern "C" int td_nhwc_to_nchw_region(const void* x, void* y, int N, int C, int 
     // fp16 and bf16 move as opaque 16-bit words
     nhwc_to_nchw_region_kernel<__half><<<grid, kNhwcThreads, 0, (cudaStream_t)stream>>>((const __half*)x, (__half*)y, C, x_pitch, x_width, x_img_stride,
                                                                                           y_plane_stride, y_pitch, y_img_stride, rows, cols, total);
-    return nhwc_check("td_nhwc_to_nchw_region");
+    return launch_status("td_nhwc_to_nchw_region");
 }
 
 extern "C" int td_upsample2x_nhwc(const void* x, void* y, int N, int H, int W, int C, int dtype, void* stream) {
@@ -379,7 +366,7 @@ extern "C" int td_upsample2x_nhwc(const void* x, void* y, int N, int H, int W, i
     }
     const long long total = (long long)N * H * W * (C / 8);
     upsample2x_nhwc_kernel<__half><<<grid_for(total, kNhwcThreads), kNhwcThreads, 0, (cudaStream_t)stream>>>((const __half*)x, (__half*)y, H, W, C / 8, total);
-    return nhwc_check("td_upsample2x_nhwc");
+    return launch_status("td_upsample2x_nhwc");
 }
 
 extern "C" int64_t td_gn_stats_nhwc_workspace_bytes(int64_t pixels, int C, int groups) {
@@ -404,7 +391,7 @@ extern "C" int td_gn_stats_nhwc(const void* x, int64_t pixels, int C, int groups
     if (dtype == TD_F16) gn_stats_nhwc_partial_kernel<__half><<<grid, kNhwcThreads, 0, st>>>((const __half*)x, pixels, C, groups, (float*)workspace);
     else gn_stats_nhwc_partial_kernel<__nv_bfloat16><<<grid, kNhwcThreads, 0, st>>>((const __nv_bfloat16*)x, pixels, C, groups, (float*)workspace);
     gn_stats_nhwc_final_kernel<<<(groups * 32 + 255) / 256, 256, 0, st>>>((const float*)workspace, grid, groups, mean, var);
-    return nhwc_check("td_gn_stats_nhwc");
+    return launch_status("td_gn_stats_nhwc");
 }
 
 extern "C" int td_gn_apply_nhwc(const void* x, void* y, int64_t pixels, int C, int groups, int dtype, const float* mean, const float* var,
@@ -422,7 +409,7 @@ extern "C" int td_gn_apply_nhwc(const void* x, void* y, int64_t pixels, int C, i
     cudaStream_t st = (cudaStream_t)stream;
     if (dtype == TD_F16) gn_apply_nhwc_kernel<__half><<<grid, kNhwcThreads, 0, st>>>((const __half*)x, (__half*)y, pixels, C, groups, mean, var, gamma, beta, eps, act);
     else gn_apply_nhwc_kernel<__nv_bfloat16><<<grid, kNhwcThreads, 0, st>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)y, pixels, C, groups, mean, var, gamma, beta, eps, act);
-    return nhwc_check("td_gn_apply_nhwc");
+    return launch_status("td_gn_apply_nhwc");
 }
 
 extern "C" int td_softmax_rows(const void* x, void* y, int rows, int cols, int64_t pitch, int dtype, void* stream) {
@@ -433,5 +420,5 @@ extern "C" int td_softmax_rows(const void* x, void* y, int rows, int cols, int64
     cudaStream_t st = (cudaStream_t)stream;
     if (dtype == TD_F16) softmax_rows_kernel<__half><<<rows, kNhwcThreads, 0, st>>>((const __half*)x, (__half*)y, cols, pitch);
     else softmax_rows_kernel<__nv_bfloat16><<<rows, kNhwcThreads, 0, st>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)y, cols, pitch);
-    return nhwc_check("td_softmax_rows");
+    return launch_status("td_softmax_rows");
 }

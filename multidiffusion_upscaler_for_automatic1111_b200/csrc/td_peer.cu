@@ -11,7 +11,9 @@
 #include <cstring>
 
 #include "td_b200.h"
+#include "td_device.cuh"
 #include "td_internal.h"
+#include "td_launch.h"
 
 namespace {
 
@@ -40,13 +42,7 @@ __global__ void peer_signal_kernel(const __grid_constant__ SignalTable tbl, int 
 __global__ void peer_wait_kernel(const uint32_t* flags, int count, const uint32_t* value) {
     const int t = threadIdx.x;
     if (t >= count) return;
-    const uint32_t want = *value;
-    uint32_t v;
-    unsigned long long spins = 0;
-    do {
-        asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(flags + t) : "memory");
-        if (++spins > (1ull << 31)) __trap();
-    } while ((int32_t)(v - want) < 0);
+    td::spin_until_ge(flags + t, *value);
 }
 
 
@@ -109,15 +105,7 @@ push_regions_kernel(const __grid_constant__ PushTable t) {
     if ((int)threadIdx.x < t.n_targets)
         asm volatile("red.release.sys.global.add.u32 [%0], %1;" ::"l"(t.targets[threadIdx.x]), "r"(1u) : "memory");
     if (blockIdx.x != 0 || threadIdx.x >= 32) return;
-    if ((int)threadIdx.x < t.wait_count) {
-        const uint32_t want = s_want;
-        uint32_t f;
-        unsigned long long spins = 0;
-        do {   // bounded: a peer that never signals becomes a launch error, not a hung GPU
-            asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(f) : "l"(t.wait_flags + threadIdx.x) : "memory");
-            if (++spins > (1ull << 31)) __trap();
-        } while ((int32_t)(f - want) < 0);
-    }
+    if ((int)threadIdx.x < t.wait_count) td::spin_until_ge(t.wait_flags + threadIdx.x, s_want);
     __syncwarp();
     if (threadIdx.x == 0 && t.bump_next != nullptr) *t.bump_next += (uint32_t)TD_PUSH_CTAS;
 }
@@ -179,8 +167,7 @@ extern "C" int td_peer_signal(void* const* flag_ptrs, int world, int rank, uint3
         tbl.ptrs[i] = (uint32_t*)flag_ptrs[i];
     }
     peer_signal_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(tbl, world, rank, step_counter);
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? TD_OK : cuda_fail("td_peer_signal", e);
+    return td::launch_status("td_peer_signal");
 }
 
 extern "C" int td_peer_wait(const uint32_t* flags, int count, const uint32_t* value, void* stream) {
@@ -190,8 +177,7 @@ extern "C" int td_peer_wait(const uint32_t* flags, int count, const uint32_t* va
     }
     if (count == 0) return TD_OK;
     peer_wait_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(flags, count, value);
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? TD_OK : cuda_fail("td_peer_wait", e);
+    return td::launch_status("td_peer_wait");
 }
 
 extern "C" int td_push_regions(const td_push_region* regions, int n_regions, void* const* target_slots, int n_targets,
@@ -224,6 +210,5 @@ extern "C" int td_push_regions(const td_push_region* regions, int n_regions, voi
     }
     t.n_targets = n_targets; t.expect_own = expect_own; t.wait_flags = wait_flags; t.wait_count = wait_count; t.bump_next = bump_next;
     push_regions_kernel<<<TD_PUSH_CTAS, 256, 0, (cudaStream_t)stream>>>(t);
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? TD_OK : cuda_fail("td_push_regions", e);
+    return td::launch_status("td_push_regions");
 }

@@ -22,6 +22,7 @@
 #include "td_b200.h"
 #include "td_device.cuh"
 #include "td_internal.h"
+#include "td_launch.h"
 
 namespace {
 
@@ -113,9 +114,7 @@ int region_composite_launch(const char* fn, const void* x_buffer, const float* w
         case TD_F32: region_composite_kernel<float><<<grid, 256, 0, st>>>(p, (const float*)x_buffer, weights, out); break;
         default: td_set_error("%s: unknown dtype %d", fn, dtype); return TD_ERR_INVALID_ARG;
     }
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { td_set_error("%s: launch failed: %s", fn, cudaGetErrorString(e)); return TD_ERR_CUDA; }
-    return TD_OK;
+    return launch_status(fn);
 }
 
 }  // namespace

@@ -34,11 +34,11 @@
 #include <algorithm>
 #include <cstdint>
 #include <cstring>
-#include <mutex>
 
 #include "td_b200.h"
 #include "td_device.cuh"
 #include "td_internal.h"
+#include "td_launch.h"
 #include "td_tma.cuh"
 
 namespace {
@@ -71,9 +71,6 @@ struct SegTable {                        // geometry of the unit staged in one s
     int band[kRowsMaxSegs], yy0[kRowsMaxSegs], nr[kRowsMaxSegs], off[kRowsMaxSegs];
 };
 
-__device__ __forceinline__ void rows_pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void rows_pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-
 // global -> shared bulk copy (1-D TMA): src, dst 16-byte aligned, bytes % 16 == 0; completes on `bar` (complete_tx)
 __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uint32_t bytes, uint64_t* bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
@@ -89,26 +86,6 @@ __device__ __forceinline__ void stg256(float* p, const float (&f)[8]) {
 __device__ __forceinline__ void ldg256(const float* p, float (&f)[8]) {
     asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(f[0]), "=f"(f[1]), "=f"(f[2]), "=f"(f[3]) : "l"(p));
     asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(f[4]), "=f"(f[5]), "=f"(f[6]), "=f"(f[7]) : "l"(p + 4));
-}
-
-template <typename T> __device__ __forceinline__ uint32_t rows_packed_add(uint32_t a, uint32_t b);
-template <> __device__ __forceinline__ uint32_t rows_packed_add<__half>(uint32_t a, uint32_t b) {
-    __half2 r = __hadd2(*reinterpret_cast<__half2*>(&a), *reinterpret_cast<__half2*>(&b));
-    return *reinterpret_cast<uint32_t*>(&r);
-}
-template <> __device__ __forceinline__ uint32_t rows_packed_add<__nv_bfloat16>(uint32_t a, uint32_t b) {
-    __nv_bfloat162 r = __hadd2(*reinterpret_cast<__nv_bfloat162*>(&a), *reinterpret_cast<__nv_bfloat162*>(&b));
-    return *reinterpret_cast<uint32_t*>(&r);
-}
-template <> __device__ __forceinline__ uint32_t rows_packed_add<float>(uint32_t a, uint32_t b) {
-    return __float_as_uint(__fadd_rn(__uint_as_float(a), __uint_as_float(b)));
-}
-
-__device__ __forceinline__ float rows_div_exact_small_int(float a, float w, float rcp) {
-    const float q = __fmul_rn(a, rcp);
-    const float r = __fmaf_rn(-q, w, a);
-    const float q2 = __fmaf_rn(r, rcp, q);
-    return __uint_as_float((__float_as_uint(q2) & 0x7fffffffu) | (__float_as_uint(a) & 0x80000000u));
 }
 
 // ---- producer: stage unit `u` into slot `slot` (called by all 32 lanes of warp 0) -----------------------------
@@ -265,8 +242,8 @@ blend_rows_md_kernel(const __grid_constant__ RowsParams p, const float* __restri
     const bool worker = r < p.RC;
     if (worker) rows_col_refs<T>(p, xv, cr, jn);
     __syncthreads();
-    rows_pdl_launch_dependents();
-    rows_pdl_wait();
+    pdl_launch_dependents();
+    pdl_wait();
     if (tid < 32)
         for (int k = 0; k < min(n, p.nslots); ++k) rows_issue<T, false>(p, c.u_begin + k, k, rows_smem, segs, full, (const T*)nullptr);
 
@@ -307,10 +284,10 @@ blend_rows_md_kernel(const __grid_constant__ RowsParams p, const float* __restri
                 for (int cc = 0; cc < kRowsMaxCols; ++cc) {
                     if (cc < jn) {
                         const uint4 e = rows_visit<T>(rowbase + (uint32_t)cr[cc].j * colstride, cr[cc]);
-                        acc.x = rows_packed_add<T>(acc.x, e.x);
-                        acc.y = rows_packed_add<T>(acc.y, e.y);
-                        acc.z = rows_packed_add<T>(acc.z, e.z);
-                        acc.w = rows_packed_add<T>(acc.w, e.w);
+                        acc.x = packed_add<T>(acc.x, e.x);
+                        acc.y = packed_add<T>(acc.y, e.y);
+                        acc.z = packed_add<T>(acc.z, e.z);
+                        acc.w = packed_add<T>(acc.w, e.w);
                     }
                 }
             }
@@ -320,7 +297,7 @@ blend_rows_md_kernel(const __grid_constant__ RowsParams p, const float* __restri
 #pragma unroll
             for (int j = 0; j < VEC; ++j) {
                 const float a = Vec<T>::get(acc, j);
-                if constexpr (FASTDIV) f[j] = wv[j] > 1.0f ? rows_div_exact_small_int(a, wv[j], rv[j]) : a;
+                if constexpr (FASTDIV) f[j] = wv[j] > 1.0f ? div_exact_small_int(a, wv[j], rv[j]) : a;
                 else f[j] = wv[j] > 1.0f ? __fdiv_rn(a, wv[j]) : a;
             }
             if constexpr (VEC == 8) stg256(out_f32 + o, f);
@@ -366,8 +343,8 @@ blend_rows_mod_kernel(const __grid_constant__ RowsParams p, const float* __restr
     const bool worker = r < p.RC;
     if (worker) rows_col_refs<T>(p, xv, cr, jn);
     __syncthreads();
-    rows_pdl_launch_dependents();
-    rows_pdl_wait();
+    pdl_launch_dependents();
+    pdl_wait();
     if (tid < 32) {
         if (tid == 0) {
             mbar_arrive_expect_tx(&aux_full, (uint32_t)p.aux_bytes);
@@ -476,8 +453,8 @@ scatter_rows_kernel(const __grid_constant__ RowsParams p, const T* __restrict__ 
     const int ps = tid / p.twv, uv = tid - ps * p.twv;
     const bool worker = ps < slot_rows;
     __syncthreads();
-    rows_pdl_launch_dependents();
-    rows_pdl_wait();
+    pdl_launch_dependents();
+    pdl_wait();
     if (tid < 32)
         for (int k = 0; k < min(n, p.nslots); ++k) rows_issue<T, true>(p, c.u_begin + k, k, rows_smem, segs, full, x);
     const uint32_t crow_bytes = (uint32_t)p.W * (uint32_t)sizeof(T);
@@ -518,44 +495,6 @@ scatter_rows_kernel(const __grid_constant__ RowsParams p, const T* __restrict__ 
 }
 
 // ---- host ---------------------------------------------------------------------------------------------------------
-struct DevInfo { int sms; int smem_optin; bool ok; };
-DevInfo dev_info() {
-    static std::mutex mu;
-    static DevInfo cache[64];
-    static bool have[64] = {};
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return {0, 0, false};
-    std::lock_guard<std::mutex> lk(mu);
-    if (!have[dev]) {
-        DevInfo d{0, 0, false};
-        d.ok = cudaDeviceGetAttribute(&d.sms, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess &&
-               cudaDeviceGetAttribute(&d.smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) == cudaSuccess;
-        cache[dev] = d;
-        have[dev] = true;
-    }
-    return cache[dev];
-}
-
-// cudaFuncAttributeMaxDynamicSharedMemorySize is per kernel and per device: cache keyed by the kernel's address
-// (several instantiations share one function-pointer TYPE, so a per-template static would alias them).
-bool rows_smem_optin(const void* kernel, int bytes) {
-    static std::mutex mu;
-    struct Entry { const void* fn; int dev; };
-    static Entry done[64];
-    static int ndone = 0;
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return false;
-    std::lock_guard<std::mutex> lk(mu);
-    for (int i = 0; i < ndone; ++i)
-        if (done[i].fn == kernel && done[i].dev == dev) return true;
-    if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) != cudaSuccess) {
-        cudaGetLastError();
-        return false;
-    }
-    if (ndone < 64) done[ndone++] = Entry{kernel, dev};
-    return true;
-}
-
 // Fills geometry, picks RC (canvas rows per unit) and the slot layout.  Returns false when the row-block form does
 // not apply (the caller falls back to the kernels in td_diffusion.cu).  scatter: slots hold canvas rows.
 bool rows_plan(const td_grid* g, int N, int C, int es, int budget_bytes, bool scatter, int sms, RowsParams* p) {
@@ -636,34 +575,10 @@ bool rows_plan(const td_grid* g, int N, int C, int es, int budget_bytes, bool sc
 
 bool rows_aligned(const void* ptr, size_t a) { return (reinterpret_cast<uintptr_t>(ptr) & (a - 1)) == 0; }
 
-template <typename... KArgs, typename... Args>
-cudaError_t rows_launch(void (*kernel)(KArgs...), int grid, size_t smem, bool pdl, cudaStream_t st, Args... args) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)grid);
-    cfg.blockDim = dim3(kRowsThreads);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr = {};
-    attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr.val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = &attr;
-    cfg.numAttrs = pdl ? 1 : 0;
-    return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
-}
-
-int rows_check(cudaError_t e, const char* what) {
-    if (e == cudaSuccess) e = cudaGetLastError();
-    if (e != cudaSuccess) {
-        td_set_error("%s: CUDA launch failed: %s", what, cudaGetErrorString(e));
-        return TD_ERR_CUDA;
-    }
-    return TD_OK;
-}
-
 bool rows_fill_batches(RowsParams* p, const void* const* batch_ptrs, int num_batches, int tile_bs, int es) {
     if (num_batches > TD_MAX_BATCH_PTRS) return false;
     for (int b = 0; b < num_batches; ++b) {
-        if (!rows_aligned(batch_ptrs[b], 16)) return false;
+        if (!aligned16(batch_ptrs[b])) return false;
         p->batch_ptrs[b] = batch_ptrs[b];
     }
     p->num_batches = num_batches;
@@ -672,35 +587,33 @@ bool rows_fill_batches(RowsParams* p, const void* const* batch_ptrs, int num_bat
     return ((long long)p->tw * es) % 16 == 0;
 }
 
+// The row-block form declines (returns 1, the caller falls back) when its shared-memory opt-in fails.
 template <typename T>
 int rows_launch_md(const RowsParams& p, int grid, const float* weights, const float* rcp, float* x_out, void* x_buffer, bool pdl, cudaStream_t st) {
     const size_t smem = (size_t)p.nslots * p.slot_bytes;
-    cudaError_t e;
-#define TD_ROWS_MD(WB, FD)                                                                                                    \
-    do {                                                                                                                      \
-        if (!rows_smem_optin((const void*)blend_rows_md_kernel<T, WB, FD>, kRowsSmemBudget)) return 1;                                     \
-        e = rows_launch(blend_rows_md_kernel<T, WB, FD>, grid, smem, pdl, st, p, weights, rcp, x_out, (T*)x_buffer);         \
-    } while (0)
     const bool fd = rcp != nullptr && sizeof(T) == 2;
-    if (x_buffer != nullptr) { if (fd) TD_ROWS_MD(true, true); else TD_ROWS_MD(true, false); }
-    else { if (fd) TD_ROWS_MD(false, true); else TD_ROWS_MD(false, false); }
-#undef TD_ROWS_MD
-    return rows_check(e, "td_blend_multidiffusion (row-block form)");
+    auto kernel = x_buffer != nullptr ? (fd ? blend_rows_md_kernel<T, true, true> : blend_rows_md_kernel<T, true, false>)
+                                      : (fd ? blend_rows_md_kernel<T, false, true> : blend_rows_md_kernel<T, false, false>);
+    const char* what = "td_blend_multidiffusion (row-block form)";
+    if (smem_optin(kernel, kRowsSmemBudget, what) != TD_OK) return 1;
+    return launch(what, kernel, dim3((unsigned)grid), dim3(kRowsThreads), smem, st, pdl, p, weights, rcp, x_out, (T*)x_buffer);
 }
 
 template <typename T>
 int rows_launch_mod(const RowsParams& p, int grid, const float* tile_weights, const float* rescale, void* x_buffer, bool pdl, cudaStream_t st) {
     const size_t smem = (size_t)p.aux_bytes + (size_t)p.nslots * p.slot_bytes;
-    if (!rows_smem_optin((const void*)blend_rows_mod_kernel<T>, kRowsSmemBudget)) return 1;
-    return rows_check(rows_launch(blend_rows_mod_kernel<T>, grid, smem, pdl, st, p, tile_weights, rescale, (T*)x_buffer),
-                      "td_blend_mixture (row-block form)");
+    const char* what = "td_blend_mixture (row-block form)";
+    if (smem_optin(blend_rows_mod_kernel<T>, kRowsSmemBudget, what) != TD_OK) return 1;
+    return launch(what, blend_rows_mod_kernel<T>, dim3((unsigned)grid), dim3(kRowsThreads), smem, st, pdl, p, tile_weights, rescale,
+                  (T*)x_buffer);
 }
 
 template <typename T>
 int rows_launch_scatter(const RowsParams& p, int grid, const void* x, void* tiles, bool pdl, cudaStream_t st) {
     const size_t smem = (size_t)p.nslots * p.slot_bytes;
-    if (!rows_smem_optin((const void*)scatter_rows_kernel<T>, kRowsSmemBudget)) return 1;
-    return rows_check(rows_launch(scatter_rows_kernel<T>, grid, smem, pdl, st, p, (const T*)x, (T*)tiles), "td_scatter_tiles (row-block form)");
+    const char* what = "td_scatter_tiles (row-block form)";
+    if (smem_optin(scatter_rows_kernel<T>, kRowsSmemBudget, what) != TD_OK) return 1;
+    return launch(what, scatter_rows_kernel<T>, dim3((unsigned)grid), dim3(kRowsThreads), smem, st, pdl, p, (const T*)x, (T*)tiles);
 }
 
 }  // namespace
@@ -709,14 +622,14 @@ int rows_launch_scatter(const RowsParams& p, int grid, const void* x, void* tile
 int td_rows_try_launch_md(const td_grid* g, const void* const* batch_ptrs, int num_batches, int tile_bs, int N, int C, int dtype,
                           const float* weights, const float* rcp_weights, float* x_out, void* x_buffer, int pdl, int dbg_no_tiles,
                           void* stream) {
-    const DevInfo d = dev_info();
+    const DeviceProps d = device_props();
     if (!d.ok || d.smem_optin < kRowsSmemBudget) return 1;
     const int es = td_dtype_size(dtype);
     RowsParams p;
     if (!rows_plan(g, N, C, es, kRowsSmemBudget, false, d.sms, &p)) return 1;
     if (!rows_fill_batches(&p, batch_ptrs, num_batches, tile_bs, es)) return 1;
     if (!rows_aligned(weights, 32) || !rows_aligned(x_out, 32) || (rcp_weights && !rows_aligned(rcp_weights, 32)) ||
-        (x_buffer && !rows_aligned(x_buffer, 16)))
+        (x_buffer && !aligned16(x_buffer)))
         return 1;
     p.dbg_no_tiles = dbg_no_tiles;
     const int grid = std::min(d.sms, p.nunits);
@@ -730,7 +643,7 @@ int td_rows_try_launch_md(const td_grid* g, const void* const* batch_ptrs, int n
 
 int td_rows_try_launch_mod(const td_grid* g, const void* const* batch_ptrs, int num_batches, int tile_bs, int N, int C, int dtype,
                            const float* tile_weights, const float* rescale, void* x_buffer, int pdl, void* stream) {
-    const DevInfo d = dev_info();
+    const DeviceProps d = device_props();
     if (!d.ok || d.smem_optin < kRowsSmemBudget) return 1;
     const int es = td_dtype_size(dtype);
     const int aux = (g->tile_h * g->tile_w * 4 + 127) & ~127;
@@ -738,7 +651,7 @@ int td_rows_try_launch_mod(const td_grid* g, const void* const* batch_ptrs, int 
     RowsParams p;
     if (!rows_plan(g, N, C, es, kRowsSmemBudget - aux, false, d.sms, &p)) return 1;
     if (!rows_fill_batches(&p, batch_ptrs, num_batches, tile_bs, es)) return 1;
-    if (!rows_aligned(tile_weights, 16) || !rows_aligned(rescale, 32) || !rows_aligned(x_buffer, 16)) return 1;
+    if (!aligned16(tile_weights) || !rows_aligned(rescale, 32) || !aligned16(x_buffer)) return 1;
     p.aux_bytes = aux;
     const int grid = std::min(d.sms, p.nunits);
     cudaStream_t st = (cudaStream_t)stream;
@@ -753,12 +666,12 @@ int td_rows_try_launch_mod(const td_grid* g, const void* const* batch_ptrs, int 
 
 int td_rows_try_launch_scatter(const td_grid* g, const void* x, void* tiles, int N, int C, int dtype, int tile_begin, int tile_end,
                                int pdl, void* stream) {
-    const DevInfo d = dev_info();
+    const DeviceProps d = device_props();
     if (!d.ok || d.smem_optin < kRowsSmemBudget) return 1;
     const int es = td_dtype_size(dtype);
     RowsParams p;
     if (!rows_plan(g, N, C, es, kRowsSmemBudget, true, d.sms, &p)) return 1;
-    if (!rows_aligned(x, 16) || !rows_aligned(tiles, 16) || ((long long)g->W * es) % 16 != 0) return 1;
+    if (!aligned16(x) || !aligned16(tiles) || ((long long)g->W * es) % 16 != 0) return 1;
     p.tile_begin = tile_begin;
     p.tile_end = tile_end;
     const int grid = std::min(d.sms, p.nunits);

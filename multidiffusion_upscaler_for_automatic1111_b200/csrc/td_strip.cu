@@ -24,6 +24,7 @@
 #include "td_b200.h"
 #include "td_device.cuh"
 #include "td_internal.h"
+#include "td_launch.h"
 
 namespace {
 
@@ -339,11 +340,11 @@ strip_blend_kernel(const __grid_constant__ StripParams p, const float* __restric
                    float* __restrict__ out_f32, T* __restrict__ out_buf) {
     extern __shared__ __align__(16) unsigned char td_strip_smem[];
     const int strip = blockIdx.x, plane = blockIdx.y * PPC, tid = threadIdx.x;
-    // programmatic dependent launch (as in td_diffusion.cu): the next grid may become resident while this one drains;
-    // every global access of THIS grid waits for its predecessor below.  Both are no-ops for an ordinary launch.
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    // programmatic dependent launch: the next grid may become resident while this one drains; every global access of THIS
+    // grid waits for its predecessor below
+    pdl_launch_dependents();
     strip_phase_table<T>(p, strip, plane, tid, td_strip_smem);     // kernel parameters only
-    asm volatile("griddepcontrol.wait;" ::: "memory");
+    pdl_wait();
     __syncthreads();
     strip_phase_copy<T, PPC>(p, strip, tid, (int)blockDim.x, td_strip_smem);
     asm volatile("cp.async.commit_group;\n\tcp.async.wait_group 0;" ::: "memory");
@@ -417,17 +418,15 @@ strip_blend_mod_kernel(const __grid_constant__ StripParams p, const float* __res
                        T* __restrict__ out_buf) {
     extern __shared__ __align__(16) unsigned char td_strip_smem[];
     const int strip = blockIdx.x, plane = blockIdx.y, tid = threadIdx.x;
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    pdl_launch_dependents();
     strip_phase_table<T>(p, strip, plane, tid, td_strip_smem);
-    asm volatile("griddepcontrol.wait;" ::: "memory");
+    pdl_wait();
     __syncthreads();
     strip_phase_copy<T>(p, strip, tid, (int)blockDim.x, td_strip_smem);
     asm volatile("cp.async.commit_group;\n\tcp.async.wait_group 0;" ::: "memory");
     __syncthreads();
     strip_phase_consume_mod<T>(p, strip, plane, tid, td_strip_smem, tile_weights, rescale, out_buf);
 }
-
-unsigned s_magic(unsigned d) { return d <= 1 ? 0u : (unsigned)(((1ull << 32) + d - 1) / d); }
 
 // fills p and the launch shape; 0 = applicable, 1 = not applicable
 int strip_plan(const td_grid* g, const void* const* batch_ptrs, int num_batches, int tile_bs, int N, int C, int elem_size, StripParams* p,
@@ -460,8 +459,8 @@ int strip_plan(const td_grid* g, const void* const* batch_ptrs, int num_batches,
     if (nv_cap > *nthreads) return 1;                          // phase 1: one thread per visit
     p->tile_stride = (long long)p->NC * g->tile_h * g->tile_w;
     if (p->tile_stride >= (1ll << 31)) return 1;
-    p->bs_magic = s_magic((unsigned)tile_bs); p->cols_magic = s_magic((unsigned)g->cols); p->spv_magic = s_magic((unsigned)p->spv);
-    p->cpr_magic = s_magic((unsigned)p->cpr); p->xv_magic = s_magic((unsigned)p->xv);
+    p->bs_magic = magic_u16((unsigned)tile_bs); p->cols_magic = magic_u16((unsigned)g->cols); p->spv_magic = magic_u16((unsigned)p->spv);
+    p->cpr_magic = magic_u16((unsigned)p->cpr); p->xv_magic = magic_u16((unsigned)p->xv);
     if (g->num_tiles >= 65536 || kStripRows * p->xv >= 65536) return 1;
     for (int i = 0; i < g->rows; ++i) p->ys[i] = (short)g->ys[i];
     for (int i = 0; i < g->cols; ++i) p->xs[i] = (short)g->xs[i];
@@ -469,39 +468,14 @@ int strip_plan(const td_grid* g, const void* const* batch_ptrs, int num_batches,
     return 0;
 }
 
-// opt-in above 48 KB of dynamic shared memory: once per kernel and device (called under g_strip_mu)
-template <typename KernelT>
-int strip_ensure_smem(KernelT kernel, int smem, int* configured /* [64], zero-initialised */) {
-    if (smem <= 40 * 1024) return TD_OK;
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0) { td_set_error("cudaGetDevice failed"); return TD_ERR_CUDA; }
-    if (dev < 64 && smem <= configured[dev]) return TD_OK;
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) { td_set_error("strip blend: cudaFuncSetAttribute(%d B): %s", smem, cudaGetErrorString(e)); return TD_ERR_CUDA; }
-    if (dev < 64) configured[dev] = smem;
-    return TD_OK;
-}
-
 template <typename T, bool WRITE_BUF, bool FASTDIV, int PPC>
 int strip_launch(const StripParams& p, int strips, int nthreads, int smem, const float* weights, const float* rcp, float* out_f32,
                  void* out_buf, bool pdl, cudaStream_t st) {
-    static int configured[64] = {0};
-    const int rc = strip_ensure_smem(strip_blend_kernel<T, WRITE_BUF, FASTDIV, PPC>, smem, configured);
+    const char* what = "td_blend_multidiffusion (strip)";
+    const int rc = smem_optin(strip_blend_kernel<T, WRITE_BUF, FASTDIV, PPC>, smem, what);
     if (rc != TD_OK) return rc;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)strips, (unsigned)(p.NC / PPC));
-    cfg.blockDim = dim3((unsigned)nthreads);
-    cfg.dynamicSmemBytes = (size_t)smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr = {};
-    attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr.val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = &attr;
-    cfg.numAttrs = pdl ? 1 : 0;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, strip_blend_kernel<T, WRITE_BUF, FASTDIV, PPC>, p, weights, rcp, out_f32, (T*)out_buf);
-    if (e == cudaSuccess) e = cudaGetLastError();
-    if (e != cudaSuccess) { td_set_error("td_blend_multidiffusion (strip): CUDA launch failed: %s", cudaGetErrorString(e)); return TD_ERR_CUDA; }
-    return TD_OK;
+    return launch(what, strip_blend_kernel<T, WRITE_BUF, FASTDIV, PPC>, dim3((unsigned)strips, (unsigned)(p.NC / PPC)), dim3((unsigned)nthreads),
+                  (size_t)smem, st, pdl, p, weights, rcp, out_f32, (T*)out_buf);
 }
 
 template <typename T, int PPC>
@@ -527,23 +501,11 @@ int strip_pick_ppc(const StripParams& p, int smem1, int max_ppc, int* smem) {
 template <typename T>
 int strip_launch_mod(const StripParams& p, int strips, int nthreads, int smem, const float* tile_weights, const float* rescale, void* out_buf,
                      bool pdl, cudaStream_t st) {
-    static int configured[64] = {0};
-    const int rc = strip_ensure_smem(strip_blend_mod_kernel<T>, smem, configured);
+    const char* what = "td_blend_mixture (strip)";
+    const int rc = smem_optin(strip_blend_mod_kernel<T>, smem, what);
     if (rc != TD_OK) return rc;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)strips, (unsigned)p.NC);
-    cfg.blockDim = dim3((unsigned)nthreads);
-    cfg.dynamicSmemBytes = (size_t)smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr = {};
-    attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr.val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = &attr;
-    cfg.numAttrs = pdl ? 1 : 0;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, strip_blend_mod_kernel<T>, p, tile_weights, rescale, (T*)out_buf);
-    if (e == cudaSuccess) e = cudaGetLastError();
-    if (e != cudaSuccess) { td_set_error("td_blend_mixture (strip): CUDA launch failed: %s", cudaGetErrorString(e)); return TD_ERR_CUDA; }
-    return TD_OK;
+    return launch(what, strip_blend_mod_kernel<T>, dim3((unsigned)strips, (unsigned)p.NC), dim3((unsigned)nthreads), (size_t)smem, st, pdl, p,
+                  tile_weights, rescale, (T*)out_buf);
 }
 
 std::mutex g_strip_mu;

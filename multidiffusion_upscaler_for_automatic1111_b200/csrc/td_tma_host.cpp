@@ -8,25 +8,10 @@
 
 #include "td_b200.h"
 #include "td_internal.h"
+#include "td_launch.h"
 #include "td_tma.cuh"
 
 namespace {
-
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn encode_fn() {
-    static EncodeTiledFn fn = [] {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess ||
-            q != cudaDriverEntryPointSuccess)
-            return (EncodeTiledFn) nullptr;
-        return (EncodeTiledFn)p;
-    }();
-    return fn;
-}
 
 struct Key {
     const void* base;
@@ -61,11 +46,8 @@ int td_encode_tensor_map_3d(CUtensorMap* out, const void* base, int dtype, uint6
                 return TD_OK;
             }
     }
-    EncodeTiledFn fn = encode_fn();
-    if (fn == nullptr) {
-        td_set_error("cuTensorMapEncodeTiled is not available from this driver");
-        return TD_ERR_CUDA;
-    }
+    const td::EncodeTiledFn fn = td::tensor_map_encoder();
+    if (fn == nullptr) return TD_ERR_CUDA;
     const int es = td_dtype_size(dtype);
     const CUtensorMapDataType dt = dtype == TD_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
                                  : dtype == TD_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
@@ -77,7 +59,7 @@ int td_encode_tensor_map_3d(CUtensorMap* out, const void* base, int dtype, uint6
     CUresult r = fn(&m, dt, 3, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                     CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) {
-        td_set_error("cuTensorMapEncodeTiled failed (%d) for [%llu,%llu,%llu] box [%u,%u]", (int)r,
+        td_set_error("tensor-map encoding failed (%d) for [%llu,%llu,%llu] box [%u,%u]", (int)r,
                      (unsigned long long)planes, (unsigned long long)rows, (unsigned long long)cols, box_rows, box_cols);
         return TD_ERR_CUDA;
     }

@@ -22,6 +22,7 @@
 #include "td_b200.h"
 #include "td_device.cuh"
 #include "td_internal.h"
+#include "td_launch.h"
 
 namespace {
 
@@ -253,16 +254,6 @@ affine_clamp_kernel(T* __restrict__ x, int C, long long HW, const float* __restr
     }
 }
 
-int check_launch_v(const char* what) {
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) {
-        td_set_error("%s: CUDA launch failed: %s", what, cudaGetErrorString(e));
-        return TD_ERR_CUDA;
-    }
-    return TD_OK;
-}
-
-inline bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
 struct StatPlan {
     long long seg_len, chunk;
@@ -274,7 +265,7 @@ StatPlan plan_stats(const void* x, long long nseg, long long seg_len, int dtype)
     StatPlan p;
     const int es = td_dtype_size(dtype), vec = 16 / es;
     p.nseg = (int)nseg; p.seg_len = seg_len;
-    p.vec = al16(x) && (seg_len % vec == 0);
+    p.vec = aligned16(x) && (seg_len % vec == 0);
     // ~64 KB per CTA, at least ~4 CTAs per SM overall, at most 1024 chunks per segment
     long long chunk = 65536 / es;
     long long chunks = (seg_len + chunk - 1) / chunk;
@@ -318,10 +309,10 @@ extern "C" int td_gn_stats(const void* x, int64_t nseg, int64_t seg_len, int dty
     else gn_stats_partial_kernel<T, false, true><<<grid, kStatThreads, 0, s>>>((const T*)x, p.seg_len, p.chunk, p.chunks, ws);
     if (dtype == TD_F16) { TD_LAUNCH(__half) } else if (dtype == TD_BF16) { TD_LAUNCH(__nv_bfloat16) } else { TD_LAUNCH(float) }
 #undef TD_LAUNCH
-    int st = check_launch_v("td_gn_stats (partial)");
+    int st = launch_status("td_gn_stats (partial)");
     if (st != TD_OK) return st;
     gn_stats_final_kernel<<<(unsigned)((p.nseg + 7) / 8), 256, 0, s>>>(ws, p.chunks, p.nseg, mean, var, seg_min, seg_max, unbiased);
-    return check_launch_v("td_gn_stats (final)");
+    return launch_status("td_gn_stats (final)");
 }
 
 extern "C" int td_gn_apply(const void* x, void* y, int B, int C, int64_t HW, int dtype, int groups, const float* mean,
@@ -336,7 +327,7 @@ extern "C" int td_gn_apply(const void* x, void* y, int B, int C, int64_t HW, int
     if (es == 0) { td_set_error("td_gn_apply: unknown dtype %d", dtype); return TD_ERR_INVALID_ARG; }
     if ((long long)B * C > 65535) { td_set_error("td_gn_apply: B*C too large"); return TD_ERR_UNSUPPORTED; }
     const int vec = 16 / es;
-    const bool v = al16(x) && al16(y) && HW % vec == 0;
+    const bool v = aligned16(x) && aligned16(y) && HW % vec == 0;
     const long long per_thread = v ? HW / vec : HW;
     long long bx = (per_thread + 256 * 4 - 1) / (256 * 4);   // ~4 vectors per thread
     bx = std::max(1LL, std::min(bx, 4096LL));
@@ -348,7 +339,7 @@ extern "C" int td_gn_apply(const void* x, void* y, int B, int C, int64_t HW, int
     else gn_apply_kernel<T, false><<<grid, 256, 0, s>>>((const T*)x, (T*)y, C, HW, cpg, groups, mean, var, gamma, beta, eps, act, stats_per_batch);
     if (dtype == TD_F16) { TD_LAUNCH(__half) } else if (dtype == TD_BF16) { TD_LAUNCH(__nv_bfloat16) } else { TD_LAUNCH(float) }
 #undef TD_LAUNCH
-    return check_launch_v("td_gn_apply");
+    return launch_status("td_gn_apply");
 }
 
 extern "C" int td_copy_region(const void* src, void* dst, int planes, int rows, int cols, int64_t src_plane_stride,
@@ -359,7 +350,7 @@ extern "C" int td_copy_region(const void* src, void* dst, int planes, int rows, 
     if (planes == 0 || rows == 0 || cols == 0) return TD_OK;
     if (planes > 65535) { td_set_error("td_copy_region: too many planes"); return TD_ERR_UNSUPPORTED; }
     const int vec = 16 / es;
-    const bool v = al16(src) && al16(dst) && cols % vec == 0 && src_pitch % vec == 0 && dst_pitch % vec == 0 &&
+    const bool v = aligned16(src) && aligned16(dst) && cols % vec == 0 && src_pitch % vec == 0 && dst_pitch % vec == 0 &&
                    src_plane_stride % vec == 0 && dst_plane_stride % vec == 0;
     const int cv = v ? cols / vec : cols;
     dim3 grid((unsigned)std::max(1, std::min((cv + 255) / 256, 64)), (unsigned)std::min(rows, 65535), (unsigned)planes);
@@ -370,7 +361,7 @@ extern "C" int td_copy_region(const void* src, void* dst, int planes, int rows, 
     else copy_region_kernel<T, false><<<grid, 256, 0, s>>>((const T*)src, (T*)dst, rows, cols, src_plane_stride, src_pitch, dst_plane_stride, dst_pitch);
     if (es == 2) { TD_LAUNCH(__half) } else { TD_LAUNCH(float) }
 #undef TD_LAUNCH
-    return check_launch_v("td_copy_region");
+    return launch_status("td_copy_region");
 }
 
 extern "C" int td_resample_nearest(const void* in, void* out, int planes, int H, int W, int oh, int ow, const int32_t* src_y,
@@ -386,7 +377,7 @@ extern "C" int td_resample_nearest(const void* in, void* out, int planes, int H,
     cudaStream_t s = (cudaStream_t)stream;
     if (es == 2) resample_kernel<__half><<<grid, 256, 0, s>>>((const __half*)in, (__half*)out, H, W, oh, ow, src_y, src_x);
     else resample_kernel<float><<<grid, 256, 0, s>>>((const float*)in, (float*)out, H, W, oh, ow, src_y, src_x);
-    return check_launch_v("td_resample_nearest");
+    return launch_status("td_resample_nearest");
 }
 
 extern "C" int td_affine_clamp(void* x, int B, int C, int64_t HW, int dtype, const float* mean_new, const float* std_new,
@@ -403,7 +394,7 @@ extern "C" int td_affine_clamp(void* x, int B, int C, int64_t HW, int dtype, con
     else if (dtype == TD_BF16) affine_clamp_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>((__nv_bfloat16*)x, C, HW, mean_new, std_new, mean_old, std_old, lo, hi);
     else if (dtype == TD_F32) affine_clamp_kernel<float><<<grid, 256, 0, s>>>((float*)x, C, HW, mean_new, std_new, mean_old, std_old, lo, hi);
     else { td_set_error("td_affine_clamp: unknown dtype %d", dtype); return TD_ERR_INVALID_ARG; }
-    return check_launch_v("td_affine_clamp");
+    return launch_status("td_affine_clamp");
 }
 
 // ---- host bookkeeping ----------------------------------------------------------------------

@@ -22,6 +22,7 @@
 #include "td_b200.h"
 #include "td_device.cuh"
 #include "td_internal.h"
+#include "td_launch.h"
 
 namespace {
 
@@ -39,17 +40,6 @@ struct WrapParams {
 };
 
 enum { MODE_MD = 0, MODE_MOD = 1 };
-
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-
-// largest i with a[i] <= val (or -1); `a` non-decreasing
-__device__ __forceinline__ int last_le(const short* a, int n, int val, float inv_d) {
-    int i = min(n - 1, max(0, (int)((float)val * inv_d)));
-    while (i + 1 < n && (int)a[i + 1] <= val) ++i;
-    while (i >= 0 && (int)a[i] > val) --i;
-    return i;
-}
 
 // Tiles of one axis that cover at least one position of [lo, hi]: index range A = [a0, a1] (origins in (lo - t, hi])
 // then, on a periodic axis, B = [b0, n) (origins in (lo - t + L, L)), ascending and disjoint.  `na` = |A|, `n` = |A|+|B|.
@@ -203,15 +193,7 @@ wrap_blend_vec_kernel(const __grid_constant__ WrapParams p, const float* __restr
         // both index ranges of the row cover: under wrap_y a row near the top is covered by band 0 AND by the last band(s)
         const bool foreign = live && (leaves_own(w, cy.a0, cy.na) || leaves_own(w, cy.b0, cy.n - cy.na));
         if (w.wait_count > 0 && __syncthreads_or(foreign)) {
-            if (threadIdx.y == 0 && (int)threadIdx.x < w.wait_count) {
-                const uint32_t want = *w.wait_value;
-                uint32_t v;
-                unsigned long long spins = 0;
-                do {   // bounded: a peer that never signals becomes a launch error, not a hung GPU
-                    asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(w.wait_flags + threadIdx.x) : "memory");
-                    if (++spins > (1ull << 31)) __trap();
-                } while ((int32_t)(v - want) < 0);
-            }
+            if (threadIdx.y == 0 && (int)threadIdx.x < w.wait_count) spin_until_ge(w.wait_flags + threadIdx.x, *w.wait_value);
             __syncthreads();   // publishes the acquire to the CTA before any tile read
         }
     }
@@ -331,35 +313,6 @@ void fill_params(const td_grid* g, int N, int C, WrapParams* p) {
     p->tile_stride = (long long)N * C * g->tile_h * g->tile_w;
 }
 
-thread_local cudaError_t tl_err = cudaSuccess;
-
-template <typename... KArgs, typename... Args>
-void launch(bool pdl, void (*kernel)(KArgs...), dim3 grid, dim3 block, cudaStream_t st, Args... args) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = grid;
-    cfg.blockDim = block;
-    cfg.dynamicSmemBytes = 0;
-    cfg.stream = st;
-    cudaLaunchAttribute attr = {};
-    attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr.val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = &attr;
-    cfg.numAttrs = pdl ? 1 : 0;
-    const cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
-    if (e != cudaSuccess) tl_err = e;
-}
-
-int check(const char* what) {
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = tl_err;
-    tl_err = cudaSuccess;
-    if (e != cudaSuccess) {
-        td_set_error("%s: CUDA launch failed: %s", what, cudaGetErrorString(e));
-        return TD_ERR_CUDA;
-    }
-    return TD_OK;
-}
-
 inline unsigned blocks_for(long long total, int threads) { return (unsigned)((total + threads - 1) / threads); }
 
 template <typename T>
@@ -370,11 +323,11 @@ int scatter_impl(const WrapParams& p, const void* x, void* tiles, int tile_begin
         const int twv = p.tw / Vec<T>::kElems;
         const int rows_per_block = std::max(1, std::min(p.th, (128 * 4 + twv - 1) / twv));   // ~4 vectors per thread
         dim3 grid((unsigned)(n_tiles * p.N * p.C), (unsigned)((p.th + rows_per_block - 1) / rows_per_block));
-        launch(pdl, wrap_scatter_vec_kernel<T>, grid, dim3(128), st, p, (const T*)x, (T*)tiles, tile_begin, rows_per_block);
-    } else {
-        launch(pdl, wrap_scatter_generic_kernel<T>, dim3(blocks_for(elems, 256)), dim3(256), st, p, (const T*)x, (T*)tiles, tile_begin, elems);
+        return launch("td_scatter_tiles (wrap)", wrap_scatter_vec_kernel<T>, grid, dim3(128), 0, st, pdl, p, (const T*)x, (T*)tiles, tile_begin,
+                      rows_per_block);
     }
-    return check("td_scatter_tiles (wrap)");
+    return launch("td_scatter_tiles (wrap)", wrap_scatter_generic_kernel<T>, dim3(blocks_for(elems, 256)), dim3(256), 0, st, pdl, p, (const T*)x,
+                  (T*)tiles, tile_begin, elems);
 }
 
 // `win` null: the whole canvas; else its row window (rb_count > 0)
@@ -388,14 +341,12 @@ int blend_vec_impl(const WrapParams& p, const float* weights, const float* tile_
     const dim3 block(kWrapBX, kWrapBY);
     const bool buf = MODE == MODE_MOD || out_buf != nullptr;
     if (win) {
-        if (buf) launch(pdl, wrap_blend_vec_kernel<T, MODE, true, true>, grid, block, st, p, weights, tile_weights, rescale, out_f32, (T*)out_buf, *win);
-        else launch(pdl, wrap_blend_vec_kernel<T, MODE, false, true>, grid, block, st, p, weights, tile_weights, rescale, out_f32, (T*)out_buf, *win);
-        return check("td_blend (wrap, rows)");
+        auto kernel = buf ? wrap_blend_vec_kernel<T, MODE, true, true> : wrap_blend_vec_kernel<T, MODE, false, true>;
+        return launch("td_blend (wrap, rows)", kernel, grid, block, 0, st, pdl, p, weights, tile_weights, rescale, out_f32, (T*)out_buf, *win);
     }
     const WindowParams whole = {};
-    if (buf) launch(pdl, wrap_blend_vec_kernel<T, MODE, true, false>, grid, block, st, p, weights, tile_weights, rescale, out_f32, (T*)out_buf, whole);
-    else launch(pdl, wrap_blend_vec_kernel<T, MODE, false, false>, grid, block, st, p, weights, tile_weights, rescale, out_f32, (T*)out_buf, whole);
-    return check("td_blend (wrap)");
+    auto kernel = buf ? wrap_blend_vec_kernel<T, MODE, true, false> : wrap_blend_vec_kernel<T, MODE, false, false>;
+    return launch("td_blend (wrap)", kernel, grid, block, 0, st, pdl, p, weights, tile_weights, rescale, out_f32, (T*)out_buf, whole);
 }
 
 // Does canvas row y lie in a tile row outside the own bands?  (host twin of the kernel's per-CTA wait test)
@@ -430,10 +381,9 @@ int blend_generic_impl(int tile_dtype, int acc_dtype, const WrapParams& p, const
     const long long total = (long long)p.N * p.C * p.H * p.W;
     const dim3 grid(blocks_for(total, 256));
 #define TD_CASE(TI, TA, TIn, TAcc)                                                                                         \
-    if (tile_dtype == TI && acc_dtype == TA) {                                                                             \
-        launch(pdl, wrap_blend_generic_kernel<TIn, TAcc, MODE>, grid, dim3(256), st, p, w, tw, rs, out_f32, (TAcc*)out_buf, total); \
-        return check("td_blend (wrap, generic)");                                                                          \
-    }
+    if (tile_dtype == TI && acc_dtype == TA)                                                                               \
+        return launch("td_blend (wrap, generic)", wrap_blend_generic_kernel<TIn, TAcc, MODE>, grid, dim3(256), 0, st, pdl, p, w, tw, rs, \
+                      out_f32, (TAcc*)out_buf, total);
     TD_CASE(TD_F16, TD_F16, __half, __half)
     TD_CASE(TD_F16, TD_BF16, __half, __nv_bfloat16)
     TD_CASE(TD_F16, TD_F32, __half, float)
