@@ -107,6 +107,9 @@ def conv2d_nhwc(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] =
     taps, cout_rows, w_cin = w.shape
     assert taps == ksize * ksize and w_cin == Cin, f"weight {tuple(w.shape)} does not match ksize {ksize} / Cin {Cin}"
     Cout = cout or cout_rows
+    # the kernel steps from one tap's weights to the next by Cout rows (include/td_b200.h: w is [kh*kw][Cout][w_pitch]):
+    # a 3x3 weight packed with more rows than Cout would be read at the wrong tap offsets
+    assert Cout <= cout_rows and (taps == 1 or Cout == cout_rows), f"Cout {Cout} vs {cout_rows} weight rows per tap ({taps} taps)"
     OH, OW = out_hw if out_hw is not None else (H, W)
     if out is None:
         out = torch.empty((N, OH, OW, Cout), dtype=x.dtype, device=x.device)

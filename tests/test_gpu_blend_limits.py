@@ -55,12 +55,16 @@ def eng():
 # ---------------------------------------------------------------------------------------------------------------------
 def launched(fn) -> set:
     """Names of the CUDA kernels `fn` launches (CUPTI activity trace through torch.profiler).  Fails when the trace holds
-    no kernel at all, so that a profiler without CUPTI cannot make the form assertions vacuous.  A session that comes
-    back empty is repeated (up to five runs of `fn`, which must be repeatable): back-to-back short sessions occasionally
-    lose their activity buffer."""
+    no kernel at all, so that a profiler without CUPTI cannot make the form assertions vacuous.
+
+    A single session can come back incomplete: back-to-back short sessions occasionally lose an activity buffer, all of
+    it (an empty trace) or part of it (one kernel of the call missing).  So `fn`, which must be repeatable and launch
+    the same kernels every time, runs in sessions until two non-empty ones in a row record the same names (at most six
+    sessions), and the union of what they recorded is returned: a kernel counts as launched when any session saw it."""
     from torch.profiler import ProfilerActivity, profile
-    for attempt in range(5):
-        time.sleep(0.2 * attempt)
+    seen, prev = set(), None
+    for attempt in range(6):
+        time.sleep(0.1 * attempt)
         torch.cuda.synchronize()
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
             fn()
@@ -73,9 +77,15 @@ def launched(fn) -> set:
                 trace = json.load(f)
         names |= {e.get("name", "") for e in trace.get("traceEvents", []) if e.get("cat") == "kernel"}
         names.discard("")
-        if names:
-            return names
-    raise AssertionError("the profiler recorded no CUDA kernel: the kernel-form assertions would be vacuous")
+        if not names:
+            continue
+        seen |= names
+        if names == prev:
+            break
+        prev = names
+    if not seen:
+        raise AssertionError("the profiler recorded no CUDA kernel: the kernel-form assertions would be vacuous")
+    return seen
 
 
 def forms(names) -> set:
