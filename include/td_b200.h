@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define TD_ABI_VERSION 12
+#define TD_ABI_VERSION 13
 
 typedef enum td_status {
     TD_OK = 0,
@@ -397,6 +397,27 @@ int td_demofusion_combine_offset(const void* x_local, const void* const* view_ba
  * accumulate, result rounded to dtype.  kernel_host: k*k fp32 values (already rounded through dtype). */
 int td_depthwise_conv2d(const void* in, void* out, int planes, int H, int W, const float* kernel_host,
                         int k, int dtype, void* stream);
+
+/* Seamless DemoFusion (new: the reference has no periodic canvas).  `wrap` = TD_WRAP_X | TD_WRAP_Y names the periodic
+ * axes; unknown bits are refused with TD_ERR_INVALID_ARG.
+ *
+ * td_depthwise_conv2d_wrap: td_depthwise_conv2d with circular indexing on the wrapped axes and zero padding on the
+ *   bounded ones; the same taps, tap order and fp32 fmaf accumulation.  Refused: k/2 > L on a wrapped axis of length L.
+ *   wrap = 0 runs the kernel of td_depthwise_conv2d.
+ * td_scatter_bboxes_wrap / td_blend_bboxes_wrap: td_scatter_bboxes / td_blend_bboxes on a window list whose origins
+ *   (canvas coordinates, no padding) may cross the canvas edge.  A window covers rows (y_t + v) mod H on a wrapped y axis
+ *   and y_t + v on a bounded one, where the scatter reads 0 outside [0, H) and the blend drops those pixels (the
+ *   reference's zero pad, slice and crop without materialising the pad); the same in x.  origins_host is REQUIRED.
+ *   Refused before any launch: on a wrapped axis an origin outside [0, L) or tile > L; on a bounded axis an origin
+ *   outside [-(tile - 1), L - 1]. */
+int td_depthwise_conv2d_wrap(const void* in, void* out, int planes, int H, int W, const float* kernel_host,
+                             int k, int wrap, int dtype, void* stream);
+int td_scatter_bboxes_wrap(const void* x, void* tiles, const int32_t* origins_dev, const int32_t* origins_host,
+                           int n_tiles, int N, int C, int H, int W, int tile_h, int tile_w, int wrap, int dtype,
+                           void* stream);
+int td_blend_bboxes_wrap(const void* const* batch_ptrs, int num_batches, int tile_bs, const int32_t* origins_dev,
+                         const int32_t* origins_host, int n_tiles, int N, int C, int H, int W, int tile_h, int tile_w,
+                         int wrap, int dtype, float* out, void* stream);
 
 /* ------------------------------------------------------------------------- *
  *  Tiled-VAE dense contractions on the tensor cores (wgmma, fp32 accumulators in registers).

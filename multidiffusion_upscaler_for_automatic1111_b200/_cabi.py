@@ -33,7 +33,7 @@ TD_MAX_GRID_DIM = 256
 TD_MAX_BATCH_PTRS = 128
 TD_MAX_PEERS = 16
 TD_IPC_HANDLE_BYTES = 64
-ABI_VERSION = 12
+ABI_VERSION = 13
 
 DTYPE_CODE = {torch.float16: TD_F16, torch.bfloat16: TD_BF16, torch.float32: TD_F32}
 
@@ -153,6 +153,11 @@ _SIGNATURES = {
     "td_demofusion_combine_offset": (c_int, [c_void_p, POINTER(c_void_p), c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int,
                                              c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_float, c_int, c_void_p]),
     "td_depthwise_conv2d": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, POINTER(c_float), c_int, c_int, c_void_p]),
+    "td_depthwise_conv2d_wrap": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, POINTER(c_float), c_int, c_int, c_int, c_void_p]),
+    "td_scatter_bboxes_wrap": (c_int, [c_void_p, c_void_p, c_void_p, POINTER(c_int32), c_int, c_int, c_int, c_int, c_int, c_int, c_int,
+                                       c_int, c_int, c_void_p]),
+    "td_blend_bboxes_wrap": (c_int, [POINTER(c_void_p), c_int, c_int, c_void_p, POINTER(c_int32), c_int, c_int, c_int, c_int, c_int,
+                                     c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "td_conv2d_nhwc": (c_int, [POINTER(TdConvDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "td_upconv2x_nhwc": (c_int, [POINTER(TdConvDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "td_attention": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int64, c_int64, c_int64, c_int64, c_float, c_int,

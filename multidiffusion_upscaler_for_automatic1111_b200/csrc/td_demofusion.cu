@@ -4,6 +4,7 @@
 //   td_demofusion_combine  <- strided `x_global[...] += view`, `/2` (mixture), `/weights`,
 //                             and x_local*(1-c2) + x_global*c2                       demofusion.py:296-322
 //   td_depthwise_conv2d    <- gaussian_filter (F.conv2d, groups=C)                   demofusion.py:173-178
+//   td_depthwise_conv2d_wrap  the same stencil with circular indexing on the wrapped axes (seamless DemoFusion, new)
 //
 // The local windows reuse td_scatter_tiles / td_blend_multidiffusion (count-normalised blend) and the
 // mean/std renormalisation reuses td_gn_stats + td_affine_clamp.  Small strided / stencil kernels:
@@ -97,29 +98,75 @@ struct ConvKernel {
     float w[kMaxKernel * kMaxKernel];   // already rounded through the latent dtype by the caller
 };
 
-// out[p, y, x] = T( sum_{dy,dx} x[p, y+dy-k/2, x+dx-k/2] * w[dy][dx] )  (zero padding, fp32 accumulate)
-template <typename T>
+// out[p, y, x] = T( sum_{dy,dx} x[p, y+dy-k/2, x+dx-k/2] * w[dy][dx] )  (fp32 accumulate, taps in (dy, dx) order)
+// Zero padding on a bounded axis; on an axis whose WRAP bit is set the index is taken mod the axis length, with one
+// conditional add or subtract because the host refuses k/2 > L there.  The body is __host__ __device__ so that the
+// test-only harness tests/emul/demofusion_host_emul.cu can run it on a CPU (fmaf is one rounding on both sides).
+template <typename T, int WRAP>
+__host__ __device__ __forceinline__ T depthwise_conv_elem(const T* __restrict__ in, const ConvKernel& ck, int H, int W, long long e) {
+    const int k = ck.k, pad = k / 2;
+    const int x = (int)(e % W);
+    const long long r = e / W;
+    const int y = (int)(r % H);
+    const T* ip = in + (r / H) * (long long)H * W;
+    float acc = 0.0f;
+    for (int dy = 0; dy < k; ++dy) {
+        int yy = y + dy - pad;
+        if constexpr ((WRAP & TD_WRAP_Y) != 0) {
+            if (yy < 0) yy += H;
+            else if (yy >= H) yy -= H;
+        } else if ((unsigned)yy >= (unsigned)H) {
+            continue;
+        }
+        for (int dx = 0; dx < k; ++dx) {
+            int xx = x + dx - pad;
+            if constexpr ((WRAP & TD_WRAP_X) != 0) {
+                if (xx < 0) xx += W;
+                else if (xx >= W) xx -= W;
+            } else if ((unsigned)xx >= (unsigned)W) {
+                continue;
+            }
+            acc = fmaf(Elem<T>::to_f32(ip[(long long)yy * W + xx]), ck.w[dy * k + dx], acc);
+        }
+    }
+    return Elem<T>::from_f32(acc);
+}
+
+template <typename T, int WRAP>
 __global__ void __launch_bounds__(256)
 depthwise_conv_kernel(const T* __restrict__ in, T* __restrict__ out, const __grid_constant__ ConvKernel ck, int planes, int H, int W) {
-    const int k = ck.k, pad = k / 2;
     const long long total = (long long)planes * H * W;
-    for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
-        const int x = (int)(e % W);
-        const long long r = e / W;
-        const int y = (int)(r % H);
-        const T* ip = in + (r / H) * (long long)H * W;
-        float acc = 0.0f;
-        for (int dy = 0; dy < k; ++dy) {
-            const int yy = y + dy - pad;
-            if ((unsigned)yy >= (unsigned)H) continue;
-            for (int dx = 0; dx < k; ++dx) {
-                const int xx = x + dx - pad;
-                if ((unsigned)xx >= (unsigned)W) continue;
-                acc = fmaf(Elem<T>::to_f32(ip[(long long)yy * W + xx]), ck.w[dy * k + dx], acc);
-            }
-        }
-        out[e] = Elem<T>::from_f32(acc);
+    for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x)
+        out[e] = depthwise_conv_elem<T, WRAP>(in, ck, H, W, e);
+}
+
+// validation shared by td_depthwise_conv2d and td_depthwise_conv2d_wrap; fills `ck`
+int conv_args(const char* who, const void* in, const void* out, int planes, int H, int W, const float* kernel_host, int k, int wrap,
+              ConvKernel* ck) {
+    if (in == nullptr || out == nullptr || kernel_host == nullptr || k <= 0 || k > kMaxKernel || (k & 1) == 0 || planes <= 0) {
+        td_set_error("%s: bad arguments (odd k <= %d)", who, kMaxKernel);
+        return TD_ERR_INVALID_ARG;
     }
+    if ((wrap & ~(int)(TD_WRAP_X | TD_WRAP_Y)) != 0 || (wrap != 0 && (H <= 0 || W <= 0))) {
+        td_set_error("%s: bad arguments (wrap=%d, %dx%d canvas)", who, wrap, H, W);
+        return TD_ERR_INVALID_ARG;
+    }
+    if (((wrap & TD_WRAP_X) && k / 2 > W) || ((wrap & TD_WRAP_Y) && k / 2 > H)) {
+        td_set_error("%s: kernel radius %d exceeds a wrapped axis of the %dx%d canvas", who, k / 2, H, W);
+        return TD_ERR_INVALID_ARG;
+    }
+    ck->k = k;
+    for (int i = 0; i < k * k; ++i) ck->w[i] = kernel_host[i];
+    return TD_OK;
+}
+
+template <int WRAP>
+void launch_conv(const void* in, void* out, const ConvKernel& ck, int planes, int H, int W, int dtype, cudaStream_t st) {
+    const long long total = (long long)planes * H * W;
+    const unsigned blocks = (unsigned)std::max(1LL, std::min((total + 255) / 256, 148LL * 32));
+    if (dtype == TD_F16) depthwise_conv_kernel<__half, WRAP><<<blocks, 256, 0, st>>>((const __half*)in, (__half*)out, ck, planes, H, W);
+    else if (dtype == TD_BF16) depthwise_conv_kernel<__nv_bfloat16, WRAP><<<blocks, 256, 0, st>>>((const __nv_bfloat16*)in, (__nv_bfloat16*)out, ck, planes, H, W);
+    else depthwise_conv_kernel<float, WRAP><<<blocks, 256, 0, st>>>((const float*)in, (float*)out, ck, planes, H, W);
 }
 
 
@@ -186,19 +233,47 @@ extern "C" int td_demofusion_combine(const void* x_local, const void* const* vie
 
 extern "C" int td_depthwise_conv2d(const void* in, void* out, int planes, int H, int W, const float* kernel_host, int k, int dtype,
                                    void* stream) {
-    if (in == nullptr || out == nullptr || kernel_host == nullptr || k <= 0 || k > kMaxKernel || (k & 1) == 0 || planes <= 0) {
-        td_set_error("td_depthwise_conv2d: bad arguments (odd k <= %d)", kMaxKernel);
-        return TD_ERR_INVALID_ARG;
-    }
     ConvKernel ck;
-    ck.k = k;
-    for (int i = 0; i < k * k; ++i) ck.w[i] = kernel_host[i];
-    const long long total = (long long)planes * H * W;
-    const unsigned blocks = (unsigned)std::max(1LL, std::min((total + 255) / 256, 148LL * 32));
-    cudaStream_t st = (cudaStream_t)stream;
-    if (dtype == TD_F16) depthwise_conv_kernel<__half><<<blocks, 256, 0, st>>>((const __half*)in, (__half*)out, ck, planes, H, W);
-    else if (dtype == TD_BF16) depthwise_conv_kernel<__nv_bfloat16><<<blocks, 256, 0, st>>>((const __nv_bfloat16*)in, (__nv_bfloat16*)out, ck, planes, H, W);
-    else if (dtype == TD_F32) depthwise_conv_kernel<float><<<blocks, 256, 0, st>>>((const float*)in, (float*)out, ck, planes, H, W);
-    else { td_set_error("td_depthwise_conv2d: unknown dtype"); return TD_ERR_INVALID_ARG; }
+    const int rc = conv_args("td_depthwise_conv2d", in, out, planes, H, W, kernel_host, k, 0, &ck);
+    if (rc != TD_OK) return rc;
+    if (dtype != TD_F16 && dtype != TD_BF16 && dtype != TD_F32) { td_set_error("td_depthwise_conv2d: unknown dtype"); return TD_ERR_INVALID_ARG; }
+    launch_conv<0>(in, out, ck, planes, H, W, dtype, (cudaStream_t)stream);
     return launch_status("td_depthwise_conv2d");
 }
+
+extern "C" int td_depthwise_conv2d_wrap(const void* in, void* out, int planes, int H, int W, const float* kernel_host, int k, int wrap,
+                                        int dtype, void* stream) {
+    ConvKernel ck;
+    const int rc = conv_args("td_depthwise_conv2d_wrap", in, out, planes, H, W, kernel_host, k, wrap, &ck);
+    if (rc != TD_OK) return rc;
+    if (dtype != TD_F16 && dtype != TD_BF16 && dtype != TD_F32) { td_set_error("td_depthwise_conv2d_wrap: unknown dtype"); return TD_ERR_INVALID_ARG; }
+    cudaStream_t st = (cudaStream_t)stream;
+    if (wrap == TD_WRAP_X) launch_conv<TD_WRAP_X>(in, out, ck, planes, H, W, dtype, st);
+    else if (wrap == TD_WRAP_Y) launch_conv<TD_WRAP_Y>(in, out, ck, planes, H, W, dtype, st);
+    else if (wrap == (TD_WRAP_X | TD_WRAP_Y)) launch_conv<TD_WRAP_X | TD_WRAP_Y>(in, out, ck, planes, H, W, dtype, st);
+    else launch_conv<0>(in, out, ck, planes, H, W, dtype, st);
+    return launch_status("td_depthwise_conv2d_wrap");
+}
+
+#ifdef TD_DEMOFUSION_HOST_EMULATION
+// Test-only (tests/emul/demofusion_host_emul.cu includes this file with the macro set): the conv body on the host.
+extern "C" int td_emul_depthwise_conv2d_wrap(const void* in, void* out, int planes, int H, int W, const float* kernel_host, int k, int wrap,
+                                             int dtype) {
+    ConvKernel ck;
+    const int rc = conv_args("td_emul_depthwise_conv2d_wrap", in, out, planes, H, W, kernel_host, k, wrap, &ck);
+    if (rc != TD_OK) return rc;
+    const long long total = (long long)planes * H * W;
+    for (long long e = 0; e < total; ++e) {
+#define TD_CONV_EMUL(T)                                                                                                      \
+    if (wrap == TD_WRAP_X) ((T*)out)[e] = depthwise_conv_elem<T, TD_WRAP_X>((const T*)in, ck, H, W, e);                      \
+    else if (wrap == TD_WRAP_Y) ((T*)out)[e] = depthwise_conv_elem<T, TD_WRAP_Y>((const T*)in, ck, H, W, e);                 \
+    else if (wrap == (TD_WRAP_X | TD_WRAP_Y)) ((T*)out)[e] = depthwise_conv_elem<T, TD_WRAP_X | TD_WRAP_Y>((const T*)in, ck, H, W, e); \
+    else ((T*)out)[e] = depthwise_conv_elem<T, 0>((const T*)in, ck, H, W, e);
+        if (dtype == TD_F16) { TD_CONV_EMUL(__half) }
+        else if (dtype == TD_BF16) { TD_CONV_EMUL(__nv_bfloat16) }
+        else { TD_CONV_EMUL(float) }
+#undef TD_CONV_EMUL
+    }
+    return TD_OK;
+}
+#endif

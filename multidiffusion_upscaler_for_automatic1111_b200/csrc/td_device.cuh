@@ -15,22 +15,22 @@ namespace td {
 template <typename T> struct Elem;
 template <> struct Elem<__half> {
     static constexpr int kDtype = 0;
-    __device__ static __forceinline__ float to_f32(__half v) { return __half2float(v); }
-    __device__ static __forceinline__ __half from_f32(float f) { return __float2half_rn(f); }
+    __host__ __device__ static __forceinline__ float to_f32(__half v) { return __half2float(v); }
+    __host__ __device__ static __forceinline__ __half from_f32(float f) { return __float2half_rn(f); }
     __device__ static __forceinline__ float bits_to_f32(uint16_t b) { return __half2float(__ushort_as_half(b)); }
     __device__ static __forceinline__ uint16_t f32_to_bits(float f) { return __half_as_ushort(__float2half_rn(f)); }
 };
 template <> struct Elem<__nv_bfloat16> {
     static constexpr int kDtype = 1;
-    __device__ static __forceinline__ float to_f32(__nv_bfloat16 v) { return __bfloat162float(v); }
-    __device__ static __forceinline__ __nv_bfloat16 from_f32(float f) { return __float2bfloat16_rn(f); }
+    __host__ __device__ static __forceinline__ float to_f32(__nv_bfloat16 v) { return __bfloat162float(v); }
+    __host__ __device__ static __forceinline__ __nv_bfloat16 from_f32(float f) { return __float2bfloat16_rn(f); }
     __device__ static __forceinline__ float bits_to_f32(uint16_t b) { return __uint_as_float(((uint32_t)b) << 16); }
     __device__ static __forceinline__ uint16_t f32_to_bits(float f) { return __bfloat16_as_ushort(__float2bfloat16_rn(f)); }
 };
 template <> struct Elem<float> {
     static constexpr int kDtype = 2;
-    __device__ static __forceinline__ float to_f32(float v) { return v; }
-    __device__ static __forceinline__ float from_f32(float f) { return f; }
+    __host__ __device__ static __forceinline__ float to_f32(float v) { return v; }
+    __host__ __device__ static __forceinline__ float from_f32(float f) { return f; }
 };
 
 // round an fp32 value through T (the "store to x_buffer, load it back" of the reference)

@@ -8,6 +8,8 @@
 //                                     weights==0 -> 1, x_local = x_buffer / weights               demofusion.py:259-264
 //   td_demofusion_combine_offset   <- td_demofusion_combine with the dilated views starting at
 //                                     jitter_range + (by, bx)                                      demofusion.py:279-322
+//   td_scatter_bboxes_wrap,        <- the two list forms on a periodic canvas (seamless DemoFusion, new: the reference
+//   td_blend_bboxes_wrap              has no wrap): modular on the wrapped axes, zero-fill / skip on the bounded ones
 //
 // Numerics as everywhere on this path: the canvas accumulates in the latent dtype with one rounding per
 // window, windows in list order.
@@ -128,6 +130,76 @@ blend_bboxes_kernel(const __grid_constant__ BlendListParams p, const int32_t* __
         out[e] = blend_bboxes_elem<T>(p, origins, e);
 }
 
+// ---- periodic canvas (seamless DemoFusion): the same list forms with a `wrap` mask (TD_WRAP_X | TD_WRAP_Y).  On a wrapped
+// axis of length L a window covers (o + u) mod L, 0 <= o < L, tile <= L; on a bounded axis it may start before 0 or end
+// past L (a jittered window with the latent not padded): the scatter reads zeros there and the blend drops those pixels.
+
+// canvas index of o + u on one axis: one subtraction on a wrapped axis (o < L, u < tile <= L), -1 off a bounded one
+__host__ __device__ __forceinline__ int wrap_axis_index(int o, int u, int L, bool wrapped) {
+    const int i = o + u;
+    if (wrapped) return i >= L ? i - L : i;
+    return (unsigned)i < (unsigned)L ? i : -1;
+}
+
+// tile coordinate of canvas index i in the window starting at o: one addition on a wrapped axis (both in [0, L))
+__host__ __device__ __forceinline__ int wrap_axis_offset(int i, int o, int L, bool wrapped) {
+    const int u = i - o;
+    return (wrapped && u < 0) ? u + L : u;
+}
+
+template <typename T>
+__host__ __device__ __forceinline__ T scatter_bboxes_wrap_elem(const T* __restrict__ x, const int32_t* __restrict__ origins, int NC, int H,
+                                                               int W, int th, int tw, int wrap, long long e) {
+    const int u = (int)(e % tw);
+    long long r = e / tw;
+    const int v = (int)(r % th);
+    r /= th;
+    const int plane = (int)(r % NC);
+    const int t = (int)(r / NC);
+    const int xx = wrap_axis_index(jload(origins + 2 * t), u, W, (wrap & TD_WRAP_X) != 0);
+    const int yy = wrap_axis_index(jload(origins + 2 * t + 1), v, H, (wrap & TD_WRAP_Y) != 0);
+    if (xx < 0 || yy < 0) return T(0);
+    return x[((long long)plane * H + yy) * W + xx];
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256)
+scatter_bboxes_wrap_kernel(const T* __restrict__ x, T* __restrict__ tiles, const int32_t* __restrict__ origins, int NC, int H, int W,
+                           int th, int tw, int wrap, long long total) {
+    for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x)
+        tiles[e] = scatter_bboxes_wrap_elem<T>(x, origins, NC, H, W, th, tw, wrap, e);
+}
+
+// blend_bboxes_elem with modular coverage on the wrapped axes
+template <typename T>
+__host__ __device__ __forceinline__ float blend_bboxes_wrap_elem(const BlendListParams& p, const int32_t* __restrict__ origins, int wrap,
+                                                                 long long e) {
+    const bool wx = (wrap & TD_WRAP_X) != 0, wy = (wrap & TD_WRAP_Y) != 0;
+    const int x = (int)(e % p.W);
+    const long long r = e / p.W;
+    const int y = (int)(r % p.H);
+    const int plane = (int)(r / p.H);
+    float acc = 0.0f;
+    int count = 0;
+    for (int t = 0; t < p.n_tiles; ++t) {
+        const int u = wrap_axis_offset(x, jload(origins + 2 * t), p.W, wx), v = wrap_axis_offset(y, jload(origins + 2 * t + 1), p.H, wy);
+        if ((unsigned)u >= (unsigned)p.tw || (unsigned)v >= (unsigned)p.th) continue;
+        const int b = t / p.tile_bs, ti = t - b * p.tile_bs;
+        const T* tp = reinterpret_cast<const T*>(p.batch_ptrs[b]) + (((long long)ti * p.NC + plane) * p.th + v) * p.tw + u;
+        acc = jround<T>(jadd(acc, JElem<T>::to_f32(*tp)));
+        ++count;
+    }
+    return count > 1 ? jdiv(acc, (float)count) : acc;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256)
+blend_bboxes_wrap_kernel(const __grid_constant__ BlendListParams p, const int32_t* __restrict__ origins, int wrap, float* __restrict__ out) {
+    const long long total = (long long)p.NC * p.H * p.W;
+    for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x)
+        out[e] = blend_bboxes_wrap_elem<T>(p, origins, wrap, e);
+}
+
 struct CombineOffsetParams {
     int NC, H, W, s, oh, ow, end_y, end_x, off;
     int views_per_batch, n_views, mixture;
@@ -187,6 +259,31 @@ int check_origins(const char* who, const int32_t* origins_host, int n_tiles, int
     return TD_OK;
 }
 
+// the wrap forms' host checks: known wrap bits, host origins present, and per axis 0 <= o < L with tile <= L when wrapped,
+// -(tile - 1) <= o <= L - 1 (at least one pixel on the canvas) when bounded
+int check_origins_wrap(const char* who, const int32_t* origins_host, int n_tiles, int H, int W, int th, int tw, int wrap) {
+    if ((wrap & ~(int)(TD_WRAP_X | TD_WRAP_Y)) != 0 || origins_host == nullptr) {
+        td_set_error("%s: bad arguments (wrap=%d, host origins %s)", who, wrap, origins_host ? "given" : "missing");
+        return TD_ERR_INVALID_ARG;
+    }
+    const bool wx = (wrap & TD_WRAP_X) != 0, wy = (wrap & TD_WRAP_Y) != 0;
+    if ((wx && tw > W) || (wy && th > H)) {
+        td_set_error("%s: window %dx%d exceeds a wrapped axis of the %dx%d canvas", who, tw, th, W, H);
+        return TD_ERR_INVALID_ARG;
+    }
+    for (int t = 0; t < n_tiles; ++t) {
+        const int ox = origins_host[2 * t], oy = origins_host[2 * t + 1];
+        const bool okx = wx ? (ox >= 0 && ox < W) : (ox >= -(tw - 1) && ox <= W - 1);
+        const bool oky = wy ? (oy >= 0 && oy < H) : (oy >= -(th - 1) && oy <= H - 1);
+        if (!okx || !oky) {
+            td_set_error("%s: window %d at (%d, %d) size %dx%d is out of range on the %dx%d canvas (wrap=%d)", who, t, ox, oy, tw, th, W, H,
+                         wrap);
+            return TD_ERR_INVALID_ARG;
+        }
+    }
+    return TD_OK;
+}
+
 }  // namespace
 
 extern "C" int td_scatter_bboxes(const void* x, void* tiles, const int32_t* origins_dev, const int32_t* origins_host, int n_tiles,
@@ -231,6 +328,50 @@ extern "C" int td_blend_bboxes(const void* const* batch_ptrs, int num_batches, i
     else if (dtype == TD_F32) blend_bboxes_kernel<float><<<blocks_for(total), 256, 0, st>>>(p, origins_dev, out);
     else { td_set_error("td_blend_bboxes: unknown dtype"); return TD_ERR_INVALID_ARG; }
     return launch_status("td_blend_bboxes");
+}
+
+extern "C" int td_scatter_bboxes_wrap(const void* x, void* tiles, const int32_t* origins_dev, const int32_t* origins_host, int n_tiles,
+                                      int N, int C, int H, int W, int tile_h, int tile_w, int wrap, int dtype, void* stream) {
+    if (x == nullptr || tiles == nullptr || origins_dev == nullptr || n_tiles <= 0 || N <= 0 || C <= 0 || H <= 0 || W <= 0 ||
+        tile_h <= 0 || tile_w <= 0) {
+        td_set_error("td_scatter_bboxes_wrap: bad arguments");
+        return TD_ERR_INVALID_ARG;
+    }
+    int rc = check_origins_wrap("td_scatter_bboxes_wrap", origins_host, n_tiles, H, W, tile_h, tile_w, wrap);
+    if (rc != TD_OK) return rc;
+    const long long total = (long long)n_tiles * N * C * tile_h * tile_w;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int es = td_dtype_size(dtype);
+    if (es == 2) scatter_bboxes_wrap_kernel<uint16_t><<<blocks_for(total), 256, 0, st>>>((const uint16_t*)x, (uint16_t*)tiles, origins_dev, N * C, H, W, tile_h, tile_w, wrap, total);
+    else if (es == 4) scatter_bboxes_wrap_kernel<uint32_t><<<blocks_for(total), 256, 0, st>>>((const uint32_t*)x, (uint32_t*)tiles, origins_dev, N * C, H, W, tile_h, tile_w, wrap, total);
+    else { td_set_error("td_scatter_bboxes_wrap: unknown dtype"); return TD_ERR_INVALID_ARG; }
+    return launch_status("td_scatter_bboxes_wrap");
+}
+
+extern "C" int td_blend_bboxes_wrap(const void* const* batch_ptrs, int num_batches, int tile_bs, const int32_t* origins_dev,
+                                    const int32_t* origins_host, int n_tiles, int N, int C, int H, int W, int tile_h, int tile_w, int wrap,
+                                    int dtype, float* out, void* stream) {
+    if (batch_ptrs == nullptr || origins_dev == nullptr || out == nullptr || num_batches <= 0 || num_batches > TD_MAX_BATCH_PTRS ||
+        tile_bs <= 0 || n_tiles <= 0 || (long long)num_batches * tile_bs < n_tiles || (long long)(num_batches - 1) * tile_bs >= n_tiles ||
+        N <= 0 || C <= 0 || H <= 0 || W <= 0 || tile_h <= 0 || tile_w <= 0) {
+        td_set_error("td_blend_bboxes_wrap: bad arguments");
+        return TD_ERR_INVALID_ARG;
+    }
+    int rc = check_origins_wrap("td_blend_bboxes_wrap", origins_host, n_tiles, H, W, tile_h, tile_w, wrap);
+    if (rc != TD_OK) return rc;
+    BlendListParams p;
+    p.NC = N * C; p.H = H; p.W = W; p.th = tile_h; p.tw = tile_w; p.n_tiles = n_tiles; p.tile_bs = tile_bs;
+    for (int b = 0; b < num_batches; ++b) {
+        if (batch_ptrs[b] == nullptr) { td_set_error("td_blend_bboxes_wrap: null batch %d", b); return TD_ERR_INVALID_ARG; }
+        p.batch_ptrs[b] = batch_ptrs[b];
+    }
+    const long long total = (long long)p.NC * H * W;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (dtype == TD_F16) blend_bboxes_wrap_kernel<__half><<<blocks_for(total), 256, 0, st>>>(p, origins_dev, wrap, out);
+    else if (dtype == TD_BF16) blend_bboxes_wrap_kernel<__nv_bfloat16><<<blocks_for(total), 256, 0, st>>>(p, origins_dev, wrap, out);
+    else if (dtype == TD_F32) blend_bboxes_wrap_kernel<float><<<blocks_for(total), 256, 0, st>>>(p, origins_dev, wrap, out);
+    else { td_set_error("td_blend_bboxes_wrap: unknown dtype"); return TD_ERR_INVALID_ARG; }
+    return launch_status("td_blend_bboxes_wrap");
 }
 
 extern "C" int td_demofusion_combine_offset(const void* x_local, const void* const* view_batch_ptrs, int num_batches,
@@ -287,6 +428,34 @@ extern "C" int td_emul_blend_bboxes(const void* const* batch_ptrs, int num_batch
         if (dtype == TD_F16) out[e] = blend_bboxes_elem<__half>(p, origins, e);
         else if (dtype == TD_BF16) out[e] = blend_bboxes_elem<__nv_bfloat16>(p, origins, e);
         else out[e] = blend_bboxes_elem<float>(p, origins, e);
+    }
+    return TD_OK;
+}
+
+extern "C" int td_emul_scatter_bboxes_wrap(const void* x, void* tiles, const int32_t* origins, int n_tiles, int N, int C, int H, int W,
+                                           int tile_h, int tile_w, int wrap, int elem_size) {
+    const int rc = check_origins_wrap("td_emul_scatter_bboxes_wrap", origins, n_tiles, H, W, tile_h, tile_w, wrap);
+    if (rc != TD_OK) return rc;
+    const long long total = (long long)n_tiles * N * C * tile_h * tile_w;
+    for (long long e = 0; e < total; ++e) {
+        if (elem_size == 2) ((uint16_t*)tiles)[e] = scatter_bboxes_wrap_elem<uint16_t>((const uint16_t*)x, origins, N * C, H, W, tile_h, tile_w, wrap, e);
+        else ((uint32_t*)tiles)[e] = scatter_bboxes_wrap_elem<uint32_t>((const uint32_t*)x, origins, N * C, H, W, tile_h, tile_w, wrap, e);
+    }
+    return TD_OK;
+}
+
+extern "C" int td_emul_blend_bboxes_wrap(const void* const* batch_ptrs, int num_batches, int tile_bs, const int32_t* origins, int n_tiles,
+                                         int N, int C, int H, int W, int tile_h, int tile_w, int wrap, int dtype, float* out) {
+    const int rc = check_origins_wrap("td_emul_blend_bboxes_wrap", origins, n_tiles, H, W, tile_h, tile_w, wrap);
+    if (rc != TD_OK) return rc;
+    BlendListParams p;
+    p.NC = N * C; p.H = H; p.W = W; p.th = tile_h; p.tw = tile_w; p.n_tiles = n_tiles; p.tile_bs = tile_bs;
+    for (int b = 0; b < num_batches; ++b) p.batch_ptrs[b] = batch_ptrs[b];
+    const long long total = (long long)p.NC * H * W;
+    for (long long e = 0; e < total; ++e) {
+        if (dtype == TD_F16) out[e] = blend_bboxes_wrap_elem<__half>(p, origins, wrap, e);
+        else if (dtype == TD_BF16) out[e] = blend_bboxes_wrap_elem<__nv_bfloat16>(p, origins, wrap, e);
+        else out[e] = blend_bboxes_wrap_elem<float>(p, origins, wrap, e);
     }
     return TD_OK;
 }

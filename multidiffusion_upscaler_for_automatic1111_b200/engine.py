@@ -264,31 +264,44 @@ def demofusion_combine(x_local: torch.Tensor, view_outs: Sequence[torch.Tensor],
 
 
 def scatter_bboxes(x: torch.Tensor, origins_dev: torch.Tensor, origins_host, n_tiles: int, tile_h: int, tile_w: int,
-                   out: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """Window LIST scatter (DemoFusion random jitter, demofusion.py:256): tiles[(t*N+n), c] = x[n, c, window t]."""
+                   out: Optional[torch.Tensor] = None, wrap: int = 0) -> torch.Tensor:
+    """Window LIST scatter (DemoFusion random jitter, demofusion.py:256): tiles[(t*N+n), c] = x[n, c, window t].
+
+    `wrap` (WRAP_X | WRAP_Y, seamless DemoFusion): windows read (o + u) mod L on those axes and zeros off the canvas on the
+    others (td_scatter_bboxes_wrap; origins_host is then required)."""
     _require_cuda(x, "x")
     N, C, H, W = x.shape
     shape = (n_tiles * N, C, tile_h, tile_w)
     if out is None or tuple(out.shape) != shape or out.dtype != x.dtype or out.device != x.device:
         out = torch.empty(shape, dtype=x.dtype, device=x.device)
     with torch.cuda.device(x.device):
-        check(lib.td_scatter_bboxes(x.data_ptr(), out.data_ptr(), origins_dev.data_ptr(), origins_host, int(n_tiles), N, C, H, W,
-                                    int(tile_h), int(tile_w), dtype_code(x.dtype), current_stream_ptr(x.device)))
+        if wrap:
+            check(lib.td_scatter_bboxes_wrap(x.data_ptr(), out.data_ptr(), origins_dev.data_ptr(), origins_host, int(n_tiles), N, C, H, W,
+                                             int(tile_h), int(tile_w), int(wrap), dtype_code(x.dtype), current_stream_ptr(x.device)))
+        else:
+            check(lib.td_scatter_bboxes(x.data_ptr(), out.data_ptr(), origins_dev.data_ptr(), origins_host, int(n_tiles), N, C, H, W,
+                                        int(tile_h), int(tile_w), dtype_code(x.dtype), current_stream_ptr(x.device)))
     return out
 
 
 def blend_bboxes(batch_outs: Sequence[torch.Tensor], tile_bs: int, origins_dev: torch.Tensor, origins_host, n_tiles: int, N: int, C: int,
-                 H: int, W: int, tile_h: int, tile_w: int) -> torch.Tensor:
+                 H: int, W: int, tile_h: int, tile_w: int, wrap: int = 0) -> torch.Tensor:
     """Window LIST count-normalised blend (demofusion.py:259-264): fp32 [N,C,H,W] = ordered sum (rounded through the tile
-    dtype per add) / max(count, 1)."""
+    dtype per add) / max(count, 1).  `wrap` as in `scatter_bboxes`: coverage is modular on those axes, and window pixels
+    off the canvas on a bounded axis are dropped (td_blend_bboxes_wrap)."""
     dev, dt = batch_outs[0].device, batch_outs[0].dtype
     _require_cuda(batch_outs[0], "tile output")
     ptrs = (ctypes.c_void_p * len(batch_outs))(*[t.data_ptr() for t in batch_outs])
     out = torch.empty((N, C, H, W), dtype=torch.float32, device=dev)
     with torch.cuda.device(dev):
-        check(lib.td_blend_bboxes(ptrs, len(batch_outs), int(tile_bs), origins_dev.data_ptr(), origins_host, int(n_tiles), N, C, H, W,
-                                  int(tile_h), int(tile_w), dtype_code(dt), out.data_ptr(), current_stream_ptr(dev)))
+        if wrap:
+            check(lib.td_blend_bboxes_wrap(ptrs, len(batch_outs), int(tile_bs), origins_dev.data_ptr(), origins_host, int(n_tiles), N, C, H,
+                                           W, int(tile_h), int(tile_w), int(wrap), dtype_code(dt), out.data_ptr(), current_stream_ptr(dev)))
+        else:
+            check(lib.td_blend_bboxes(ptrs, len(batch_outs), int(tile_bs), origins_dev.data_ptr(), origins_host, int(n_tiles), N, C, H, W,
+                                      int(tile_h), int(tile_w), dtype_code(dt), out.data_ptr(), current_stream_ptr(dev)))
     return out
+
 
 
 def _region_table(xb: torch.Tensor, regions: Sequence[tuple]):

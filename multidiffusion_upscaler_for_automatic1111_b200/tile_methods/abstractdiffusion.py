@@ -229,7 +229,7 @@ class AbstractDiffusion:
         crop goes through the engine, which reads the plan's wrap bits."""
         wrap = (engine.WRAP_X if wrap_x else 0) | (engine.WRAP_Y if wrap_y else 0)
         if wrap and self.method == "DemoFusion":
-            raise NotImplementedError("DemoFusion builds its own window lists: seamless tiling (wrap_x / wrap_y) is not supported")
+            raise NotImplementedError("DemoFusion builds its own window lists: pass wrap_x / wrap_y to DemoFusion.get_views(...)")
         self.enable_grid_bbox = True
         g = engine.make_grid(self.w, self.h, tile_w, tile_h, overlap, tile_bs, wrap=wrap)
         self._grid = g

@@ -10,6 +10,13 @@
 Random jitter (demofusion.py:116-134, offsets from Python's `random`) makes the window list non-separable: the
 local windows then go through the list-driven td_scatter_bboxes / td_blend_bboxes on the zero-padded latent and the
 add-back through td_demofusion_combine_offset (csrc/td_jitter.cu).
+
+Seamless tiling (new: the reference has no periodic canvas), get_views(..., wrap_x, wrap_y): the local windows are the
+periodic plan of td_grid_init (ring windows, count-normalised through td_wrap.cu), or with random jitter a ring window list
+on td_scatter_bboxes_wrap / td_blend_bboxes_wrap; the gaussian filter indexes the wrapped axes circularly
+(td_depthwise_conv2d_wrap).  The latent is never padded then: a jittered window on a bounded axis reads zeros off the
+canvas and drops them in the blend, and the dilated views cover the whole canvas from 0.  tests/demofusion_wrap_oracle.py
+(demofusion_views, demofusion_step) defines these semantics.
 """
 from __future__ import annotations
 
@@ -37,10 +44,16 @@ class DemoFusion(AbstractDiffusion):
         self.jitter_range = 0
         self.repeat_3 = False
         self._jitter = False                 # window LIST (random jitter) instead of the separable grid
+        self._wrap = 0                       # engine.WRAP_X | WRAP_Y: periodic canvas axes (get_views' wrap_x / wrap_y)
         self._origins_host = None
         self._origins_dev = None
         self._shard_on = False               # tile shard requested (init_tile_shard); re-derived by every get_views
         self._view_shard = None
+
+    @property
+    def _list_wrap(self) -> dict:
+        """The window-list engine calls take `wrap` only on a seamless canvas (the bounded calls are unchanged)."""
+        return {"wrap": self._wrap} if self._wrap else {}
 
     def _check_input(self, x_in: Tensor) -> Tensor:
         if not self._jitter:
@@ -112,17 +125,54 @@ class DemoFusion(AbstractDiffusion):
                 out.append(BBox(x + xj + jr, y + yj + jr, tile_w, tile_h))
         return out
 
+    def split_bboxes_jitter_wrap(self, g) -> List[BBox]:
+        """Random jitter on the periodic plan `g` (seamless tiling): the windows of the plan in row-major order, each moved
+        by draws from Python's global `random`, x before y, with the reference's jitter_range.  On a wrapped axis every
+        window draws randint(-jr, jr) and its origin is kept mod L; on a bounded axis the reference's border rule holds
+        (split_bboxes_jitter) and the origin is in canvas coordinates (no padding: it may start at -jr or end jr past L)."""
+        jr = min(max((min(self.w, self.h) - self.stride) // 4, 0), min(int(self.window_size / 2), int(self.overlap / 2)))
+        self.jitter_range = jr
+        ws = self.window_size
+
+        def draw(pos: int, size: int, extent: int, wrapped: bool) -> int:
+            at_start, at_end = pos == 0, pos + size == extent
+            if wrapped or (not at_start and not at_end):
+                return random.randint(-jr, jr)
+            if at_start and not at_end:
+                return random.randint(-jr, 0)
+            if at_end and not at_start:
+                return random.randint(0, jr)
+            return 0
+        wx, wy = bool(self._wrap & engine.WRAP_X), bool(self._wrap & engine.WRAP_Y)
+        out = []
+        for x, y, _, _ in engine.grid_bboxes_xywh(g):
+            x, y = int(x), int(y)
+            xj = draw(x, ws, self.w, wx)
+            yj = draw(y, ws, self.h, wy)
+            out.append(BBox((x + xj) % self.w if wx else x + xj, (y + yj) % self.h if wy else y + yj, ws, ws))
+        return out
+
     @grid_bbox
-    def get_views(self, overlap: int, tile_bs: int, tile_bs_g: int):
-        """demofusion.py:140-162: local window grid (stride = max(4, window - overlap)) + global view batches."""
+    def get_views(self, overlap: int, tile_bs: int, tile_bs_g: int, wrap_x: bool = False, wrap_y: bool = False):
+        """demofusion.py:140-162: local window grid (stride = max(4, window - overlap)) + global view batches.
+
+        wrap_x / wrap_y (the WebUI's "Tiling" option, passed again every upscaling phase) make the canvas periodic on that
+        axis: seamless output.  The windows then run around the circle, and the latent is not padded for jitter."""
         self.enable_grid_bbox = True
         self.tile_w = self.tile_h = self.window_size
         self.overlap = max(0, min(overlap, self.window_size - 4))
         self.stride = max(4, self.window_size - self.overlap)
         self.jitter_range = 0
         self._jitter = bool(getattr(self.p, "random_jitter", False))
+        self._wrap = (engine.WRAP_X if wrap_x else 0) | (engine.WRAP_Y if wrap_y else 0)
         if self._jitter:
-            bboxes = self.split_bboxes_jitter(self.w, self.h, self.tile_w, self.tile_h, self.overlap)
+            if self._wrap:
+                g = engine.make_grid(self.w, self.h, self.window_size, self.window_size, self.overlap, tile_bs, wrap=self._wrap)
+                if g.overlap != self.overlap or g.tile_w != self.window_size or g.tile_h != self.window_size:
+                    raise ValueError("window larger than the latent: DemoFusion clamps window_size before get_views")
+                bboxes = self.split_bboxes_jitter_wrap(g)
+            else:
+                bboxes = self.split_bboxes_jitter(self.w, self.h, self.tile_w, self.tile_h, self.overlap)
             self._grid = None
             flat = [v for b in bboxes for v in (b.x, b.y)]
             self._origins_host = (ctypes.c_int32 * len(flat))(*flat)
@@ -133,7 +183,7 @@ class DemoFusion(AbstractDiffusion):
         else:
             # split_bboxes_jitter without jitter is split_bboxes on the clamped overlap (demofusion.py:101-115);
             # init through td_grid_init with tile == window reproduces rows / cols / origins exactly
-            g = engine.make_grid(self.w, self.h, self.window_size, self.window_size, self.overlap, tile_bs)
+            g = engine.make_grid(self.w, self.h, self.window_size, self.window_size, self.overlap, tile_bs, wrap=self._wrap)
             if g.overlap != self.overlap or g.tile_w != self.window_size or g.tile_h != self.window_size:
                 raise ValueError("window larger than the latent: DemoFusion clamps window_size before get_views")
             self._grid = g
@@ -201,7 +251,12 @@ class DemoFusion(AbstractDiffusion):
         tcond = self.repeat_tensor(self.get_tcond(cond_in), n_rep)
         icond = self.get_icond(cond_in)
         if tuple(icond.shape[2:]) == (self.h, self.w):
-            if mode == 0:
+            if mode == 0 and self._wrap:  # ring windows: modular on the wrapped axes, zeros off a bounded one (as the latent)
+                flat = [v for b in bboxes for v in (b.x, b.y)]
+                origins_host = (ctypes.c_int32 * len(flat))(*flat)
+                origins_dev = torch.tensor(flat, dtype=torch.int32, device=icond.device)
+                icond = engine.scatter_bboxes(icond, origins_dev, origins_host, n_rep, self.window_size, self.window_size, wrap=self._wrap)
+            elif mode == 0:
                 if self._jitter:          # the windows live on the padded latent (demofusion.py:71-73)
                     jr = self.jitter_range
                     icond = F.pad(icond, (jr, jr, jr, jr), "constant", value=0)
@@ -226,14 +281,19 @@ class DemoFusion(AbstractDiffusion):
         return g2[None, None, :, :].repeat(channels, 1, 1, 1)
 
     def gaussian_filter(self, latents: Tensor, kernel_size=3, sigma=1.0) -> Tensor:
-        """demofusion.py:173-178 as one depthwise stencil launch (weights rounded to the latent dtype like `.to(dtype)`)."""
+        """demofusion.py:173-178 as one depthwise stencil launch (weights rounded to the latent dtype like `.to(dtype)`);
+        circular on the wrapped axes of a seamless canvas (td_depthwise_conv2d_wrap)."""
         k2 = self.gaussian_kernel(kernel_size, sigma, 1)[0, 0].to(latents.dtype).float().contiguous().numpy()
         x = latents.contiguous()
         out = torch.empty_like(x)
         n, c, hh, ww = x.shape
         with torch.cuda.device(x.device):
-            check(lib.td_depthwise_conv2d(x.data_ptr(), out.data_ptr(), n * c, hh, ww, k2.ctypes.data_as(ctypes.POINTER(ctypes.c_float)),
-                                          int(kernel_size), dtype_code(x.dtype), current_stream_ptr(x.device)))
+            if self._wrap:
+                check(lib.td_depthwise_conv2d_wrap(x.data_ptr(), out.data_ptr(), n * c, hh, ww, k2.ctypes.data_as(ctypes.POINTER(ctypes.c_float)),
+                                                   int(kernel_size), self._wrap, dtype_code(x.dtype), current_stream_ptr(x.device)))
+            else:
+                check(lib.td_depthwise_conv2d(x.data_ptr(), out.data_ptr(), n * c, hh, ww, k2.ctypes.data_as(ctypes.POINTER(ctypes.c_float)),
+                                              int(kernel_size), dtype_code(x.dtype), current_stream_ptr(x.device)))
         return out
 
     def _renormalise(self, g_: Tensor, x_in: Tensor) -> Tensor:
@@ -267,7 +327,7 @@ class DemoFusion(AbstractDiffusion):
         self.cosine_factor = 0.5 * (1 + torch.cos(torch.pi * torch.tensor(((p.current_step + 1) / (self.t_enc + 1)))))
         c1 = self.cosine_factor ** p.cosine_scale_1
         x_in = x_in * (1 - c1) + x_noisy * c1
-        jr = self.jitter_range if getattr(p, "random_jitter", False) else 0
+        jr = self.jitter_range if getattr(p, "random_jitter", False) and not self._wrap else 0   # a seamless canvas is not padded
         H, W = x_in.shape[2:]
         x_in_ = F.pad(x_in, (jr, jr, jr, jr), "constant", value=0) if jr else x_in      # demofusion.py:200-204
         cfg = self.sampler.model_wrap_cfg
@@ -283,7 +343,7 @@ class DemoFusion(AbstractDiffusion):
     @keep_signature
     def sample_one_step(self, x_in: Tensor, sigma: Tensor, cond):
         """demofusion.py:219-324.  With random jitter `x_in` is the latent zero-padded by jitter_range (the callers
-        pad and crop: forward_one_step, get_noise)."""
+        pad and crop: forward_one_step, get_noise), except on a seamless canvas (get_views' wrap_x / wrap_y)."""
         p = self.p
         sd_model = getattr(p, "sd_model", None) or self._sd_model()
 
@@ -299,7 +359,7 @@ class DemoFusion(AbstractDiffusion):
 
         x = self._check_input(x_in)
         N, C, H, W = x.shape
-        jr = self.jitter_range if self._jitter else 0
+        jr = self.jitter_range if self._jitter and not self._wrap else 0     # the padding x_in carries
         if (H, W) != (self.h + 2 * jr, self.w + 2 * jr):
             raise ValueError(f"latent {(H, W)} does not match the views built for {(self.h, self.w)} (+ 2 x jitter {jr})")
         dt, dev = x.dtype, x.device
@@ -336,8 +396,11 @@ class DemoFusion(AbstractDiffusion):
             raise ValueError("DemoFusion without mixture needs gaussian_filter=True (the reference reads x_in_g unconditionally)")
 
         # ---- global dilated views ------------------------------------------------------------------------------------
-        end = W - jr   # the reference's slice bound `end = shape[3] - jitter_range` is used on both axes
-        end_y, end_x = min(H, end), end
+        if self._wrap:     # views from 0 over the whole canvas
+            end_y, end_x = H, W
+        else:
+            end = W - jr   # the reference's slice bound `end = shape[3] - jitter_range` is used on both axes
+            end_y, end_x = min(H, end), end
         oh, ow = len(range(jr, end_y, s)), len(range(jr, end_x, s))
         if any(len(range(jr + b, end_y, s)) != oh for b in range(s)) or any(len(range(jr + b, end_x, s)) != ow for b in range(s)):
             raise ValueError("latent size must be a multiple of the scale (the reference's torch.cat needs equal views)")
@@ -374,7 +437,8 @@ class DemoFusion(AbstractDiffusion):
                 if self._origins_dev.device != dev:
                     self._origins_dev = self._origins_dev.to(dev)
                 host_part = (ctypes.c_int32 * (2 * sh.num_local))(*self._origins_host[2 * sh.begin:2 * sh.end])
-                tiles = engine.scatter_bboxes(x, self._origins_dev[2 * sh.begin:2 * sh.end], host_part, sh.num_local, ws, ws)
+                tiles = engine.scatter_bboxes(x, self._origins_dev[2 * sh.begin:2 * sh.end], host_part, sh.num_local, ws, ws,
+                                              **self._list_wrap)
             else:
                 tiles = engine.scatter_tiles(self._grid, x, tile_begin=sh.begin, tile_end=sh.end, flags=self._blend_flags)
             off = 0
@@ -385,7 +449,8 @@ class DemoFusion(AbstractDiffusion):
                 off += len(bboxes)
         chunks = self._gather_chunks(outs, sh, N, (C, ws, ws), dt, dev)
         if self._jitter:
-            return engine.blend_bboxes(chunks, sh.chunk, self._origins_dev, self._origins_host, self.num_tiles, N, C, H, W, ws, ws).to(dt)
+            return engine.blend_bboxes(chunks, sh.chunk, self._origins_dev, self._origins_host, self.num_tiles, N, C, H, W, ws, ws,
+                                       **self._list_wrap).to(dt)
         if self._counts.device != dev:
             self._counts, self._rcp_counts = self._counts.to(dev), self._rcp_counts.to(dev)
         rcp = self._rcp_counts if dt in (torch.float16, torch.bfloat16) else None
@@ -399,19 +464,21 @@ class DemoFusion(AbstractDiffusion):
         dt, dev, ws, T = x.dtype, x.device, self.window_size, self.num_tiles
         if self._origins_dev.device != dev:
             self._origins_dev = self._origins_dev.to(dev)
-        self._tiles = engine.scatter_bboxes(x, self._origins_dev, self._origins_host, T, ws, ws, out=self._tiles)
+        self._tiles = engine.scatter_bboxes(x, self._origins_dev, self._origins_host, T, ws, ws, out=self._tiles, **self._list_wrap)
         outs = []
         for batch_id, bboxes in enumerate(self.batched_bboxes):
             if host.interrupted():
                 return None
             outs.append(repeat_func(self._tile_batch(self._tiles, batch_id, N), bboxes).to(dt).contiguous())
-        return engine.blend_bboxes(outs, self.tile_bs, self._origins_dev, self._origins_host, T, N, C, H, W, ws, ws).to(dt)
+        return engine.blend_bboxes(outs, self.tile_bs, self._origins_dev, self._origins_host, T, N, C, H, W, ws, ws,
+                                   **self._list_wrap).to(dt)
 
     def get_noise(self, x_in: Tensor, sigma_in: Tensor, cond_in: Dict[str, Tensor], step: int) -> Tensor:
-        """demofusion.py:345-353: the tiled eps on the latent padded by jitter_range, cropped back."""
+        """demofusion.py:345-353: the tiled eps on the latent padded by jitter_range, cropped back (never padded on a
+        seamless canvas)."""
         self.repeat_3 = True
         self.cosine_factor = 0.5 * (1 + torch.cos(torch.pi * torch.tensor(((self.p.current_step + 1) / (self.t_enc + 1)))))
-        jr = self.jitter_range
+        jr = 0 if self._wrap else self.jitter_range
         if not jr:
             return self.sample_one_step(x_in, sigma_in, cond_in.copy())
         H, W = x_in.shape[2:]
