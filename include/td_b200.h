@@ -225,7 +225,8 @@ int td_copy_region(const void* src, void* dst, int planes, int rows, int cols,
  * td_resample_nearest: out[p, i, j] = in[p, src_y[i], src_x[j]] (F.interpolate
  * nearest-exact; the index tables are computed on the host with ATen's float32 rule).
  * td_affine_clamp: x = clamp((x - mean_new[c]) / std_new[c] * std_old[c] + mean_old[c],
- * lo[0], hi[0]) in place, every step rounded through `dtype` like the eager ops. */
+ * lo[0], hi[0]) in place, every step rounded through `dtype` like the eager ops.  NaN follows
+ * torch.clamp: a NaN value stays NaN (0 / 0 where std_new is 0), otherwise a NaN bound is the result. */
 int td_resample_nearest(const void* in, void* out, int planes, int H, int W, int oh, int ow,
                         const int32_t* src_y, const int32_t* src_x, int dtype, void* stream);
 int td_affine_clamp(void* x, int B, int C, int64_t HW, int dtype, const float* mean_new,

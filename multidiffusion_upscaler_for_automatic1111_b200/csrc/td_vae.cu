@@ -149,6 +149,7 @@ __global__ void gn_stats_final_kernel(const float* __restrict__ ws, int chunks_p
     for (int off = 16; off > 0; off >>= 1) m = merge(m, shfl_down(m, off));
     if (lane == 0) {
         mean[seg] = m.mean;
+        // an unbiased one-element segment gets 0 (torch: NaN); fast mode never asks for one
         var[seg] = m.m2 / (unbiased ? fmaxf(m.n - 1.f, 1.f) : m.n);
         if (lo) lo[seg] = m.lo;
         if (hi) hi[seg] = m.hi;
@@ -250,7 +251,9 @@ affine_clamp_kernel(T* __restrict__ x, int C, long long HW, const float* __restr
         v = round_through<T>(__fdiv_rn(v, sn));
         v = round_through<T>(__fmul_rn(v, so));
         v = round_through<T>(__fadd_rn(v, mo));
-        p[i] = Elem<T>::from_f32(fminf(fmaxf(v, l), h));
+        // torch.clamp's NaN rule: a NaN operand stays NaN, else a NaN bound is the result.  A constant channel makes
+        // the estimator's (x - mean_new) / std_new 0 / 0; the NaN must reach the caller, which then disables fast mode.
+        p[i] = Elem<T>::from_f32(isnan(v) ? v : isnan(l) ? l : isnan(h) ? h : fminf(fmaxf(v, l), h));
     }
 }
 

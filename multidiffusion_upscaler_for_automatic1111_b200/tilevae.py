@@ -153,7 +153,9 @@ def fast_mode_estimator_input(z: torch.Tensor, tile_size: int) -> torch.Tensor:
         out = _segment_stats(t, B * C, hw, unbiased=True, want_minmax=want_minmax)
         var, mean = out[0].view(B, C), out[1].view(B, C)
         if B > 1:   # torch.std_mean over dims [0, 2, 3]: merge the per-(b, c) moments (equal counts)
-            m = mean.mean(dim=0)
+            # shifted by the first image's mean: equal means merge to exactly that mean (a plain fp32 mean of three
+            # equal values can miss it by an ulp, and a channel that is constant over the batch would get std > 0)
+            m = mean[0] + (mean - mean[0]).mean(dim=0)
             m2 = (var * (hw - 1)).sum(dim=0) + hw * ((mean - m) ** 2).sum(dim=0)
             var, mean = m2 / (B * hw - 1), m
         else:
