@@ -109,6 +109,8 @@ typedef struct td_grid {
     int32_t ys[TD_MAX_GRID_DIM]; /* tile-row origins, utils.py:169                 */
     int32_t xs[TD_MAX_GRID_DIM]; /* tile-col origins, utils.py:171                 */
 } td_grid;
+/* The scatter / blend entries refuse (TD_ERR_INVALID_ARG, naming the axis and the index) a plan whose ys[0 .. rows) or
+ * xs[0 .. cols) decrease: their origin searches need non-decreasing origins.  Equal neighbours are legal. */
 
 /* init_grid_bbox -- abstractdiffusion.py:172-186.  w, h are LATENT sizes.  Returns T or a td_status.
  * `wrap` (TD_WRAP_X | TD_WRAP_Y, stored in g->wrap) tiles those axes as a circle -- seamless tiling, new: the reference
@@ -137,7 +139,8 @@ int td_rescale_factor(const float* weights, float* out, int64_t n);
  *   tiles[(t - tile_begin)*N + n, c, v, u] = x[n, c, ys[t/cols] + v, xs[t%cols] + u]
  * for t in [tile_begin, tile_end): ONE launch for the whole step (the reference
  * issues one torch.cat per tile batch).  x: [N,C,H,W] contiguous; tiles:
- * [(tile_end-tile_begin)*N, C, tile_h, tile_w] contiguous; same dtype. */
+ * [(tile_end-tile_begin)*N, C, tile_h, tile_w] contiguous; same dtype.  An empty range (tile_begin == tile_end)
+ * launches nothing and returns TD_OK, whatever x and tiles are (an empty tensor has a null data pointer). */
 int td_scatter_tiles(const td_grid* g, const void* x, void* tiles, int N, int C, int dtype,
                      int tile_begin, int tile_end, uint32_t flags, void* stream);
 /* Every grid entry below (and td_scatter_tiles) rejects with TD_ERR_INVALID_ARG a plan whose tiles leave the canvas

@@ -1073,6 +1073,18 @@ int fill_geom(const td_grid* g, int N, int C, GeomParams* o) {
             td_set_error("tile row %d (y=%d, h=%d) leaves the %d-high canvas", r, g->ys[r], g->tile_h, g->H);
             return TD_ERR_INVALID_ARG;
         }
+    // every origin search (last_le, the wrap blends' cover ranges, the row bands of td_rows.cu / td_strip.cu) assumes
+    // non-decreasing origins: out of order, it finds tiles that do not cover the pixel and reads outside them
+    for (int c = 1; c < g->cols; ++c)
+        if (g->xs[c] < g->xs[c - 1]) {
+            td_set_error("tile column origins out of order: xs[%d]=%d < xs[%d]=%d", c, g->xs[c], c - 1, g->xs[c - 1]);
+            return TD_ERR_INVALID_ARG;
+        }
+    for (int r = 1; r < g->rows; ++r)
+        if (g->ys[r] < g->ys[r - 1]) {
+            td_set_error("tile row origins out of order: ys[%d]=%d < ys[%d]=%d", r, g->ys[r], r - 1, g->ys[r - 1]);
+            return TD_ERR_INVALID_ARG;
+        }
     o->H = g->H; o->W = g->W; o->th = g->tile_h; o->tw = g->tile_w;
     o->rows = g->rows; o->cols = g->cols; o->N = N; o->C = C;
     for (int i = 0; i < g->rows; ++i) o->ys[i] = (short)g->ys[i];
@@ -1410,13 +1422,14 @@ extern "C" int td_scatter_tiles(const td_grid* g, const void* x, void* tiles, in
     int st = fill_geom(g, N, C, &gp);
     if (st != TD_OK) return st;
     if ((flags & kOptInForms) && (st = refuse_wrapped(g, "td_scatter_tiles")) != TD_OK) return st;
-    if (x == nullptr || tiles == nullptr) { td_set_error("td_scatter_tiles: null tensor"); return TD_ERR_INVALID_ARG; }
     if (tile_begin < 0 || tile_end < tile_begin || tile_end > g->num_tiles) {
         td_set_error("td_scatter_tiles: tile range [%d,%d) outside [0,%d)", tile_begin, tile_end, g->num_tiles);
         return TD_ERR_INVALID_ARG;
     }
     const int es = td_dtype_size(dtype);
     if (es == 0) { td_set_error("td_scatter_tiles: unknown dtype %d", dtype); return TD_ERR_INVALID_ARG; }
+    if (tile_begin == tile_end) return TD_OK;   // an empty range (a shard without tiles) launches nothing: its output may be empty
+    if (x == nullptr || tiles == nullptr) { td_set_error("td_scatter_tiles: null tensor"); return TD_ERR_INVALID_ARG; }
     const int vec = 16 / es;
     const bool pdl = !(flags & TD_FLAG_NO_PDL);
     const bool vec_ok = !(flags & TD_FLAG_FORCE_GENERIC) && gp.W % vec == 0 && gp.tw % vec == 0 && aligned16(x) && aligned16(tiles);

@@ -334,15 +334,22 @@ def test_bad_arguments_return_status_not_crash(eng):
         eng.blend_multidiffusion(g, [tiles], 2, 4, g.num_tiles - 1, w, x.dtype)  # table does not cover the tiles
 
 
-@pytest.mark.parametrize("graph", [False, True])
-def test_dependent_launch_chain_keeps_stream_order(eng, graph):
+@pytest.mark.parametrize("graph,wrap", [(False, 0), (True, 0), (False, 3), (True, 3)], ids=["False", "True", "False-wrap", "True-wrap"])
+def test_dependent_launch_chain_keeps_stream_order(eng, graph, wrap):
     """The default kernels are launched with programmatic dependent launch.  A chain in which every kernel consumes
     what its direct predecessor wrote (scatter reads the canvas the blend just wrote, the blend reads the tiles the
     scatter just wrote, and overwrites the canvas the scatter just read) must equal the plainly serialised run bit for
-    bit, eagerly and when replayed from a CUDA graph."""
+    bit, eagerly and when replayed from a CUDA graph, on a bounded and on a periodic plan (wrap = 3: x and y, the
+    td_wrap.cu kernels, whose blends load their origins and release the next launch before waiting), in the vector
+    and in the generic forms."""
     N, C, W, H, tw, th, ov, bs = 2, 4, 512, 512, 96, 96, 48, 4
-    g = _grid(eng, W, H, tw, th, ov, bs)
-    plan = tiling.GridPlan(W, H, tw, th, ov, bs, True)
+    g = eng.make_grid(W, H, tw, th, ov, bs, wrap=wrap)
+    if wrap:
+        import wrap_oracle as wo
+        plan = wo.WrapPlan(W, H, tw, th, ov, bs, wrap, gaussian=True)
+        assert list(g.xs[:g.cols]) == plan.xs and list(g.ys[:g.rows]) == plan.ys
+    else:
+        plan = tiling.GridPlan(W, H, tw, th, ov, bs, True)
     twt = torch.from_numpy(plan.tile_weights).cuda()
     rf = torch.from_numpy(plan.rescale_factor).cuda()
     x0 = synth.latent(31, (N, C, H, W), torch.float16).cuda()
@@ -372,7 +379,8 @@ def test_dependent_launch_chain_keeps_stream_order(eng, graph):
         torch.cuda.synchronize()
         return xb.clone()
 
-    want = chain(NO_PDL)
-    got = chain(0)
-    assert torch.isfinite(want.float()).all()
-    assert_bit_equal(got, want.cpu(), "PDL chain")
+    for form in (0, FORCE_GENERIC):
+        want = chain(form | NO_PDL)
+        got = chain(form)
+        assert torch.isfinite(want.float()).all()
+        assert_bit_equal(got, want.cpu(), f"PDL chain wrap={wrap} flags={form}")

@@ -86,7 +86,7 @@ def accumulate_md(x_buffer: torch.Tensor, tile_out: torch.Tensor, bboxes: Sequen
     for i, b in enumerate(bboxes):
         iy, ix = rows_cols(b, W, H)
         idx = (slice(None), slice(None), iy[:, None], ix[None, :])
-        x_buffer[idx] = x_buffer[idx] + tile_out[i * N:(i + 1) * N]          # one rounding in the buffer dtype
+        x_buffer[idx] = (x_buffer[idx] + tile_out[i * N:(i + 1) * N]).to(x_buffer.dtype)   # one rounding in the buffer dtype
 
 
 def accumulate_mod(x_buffer: torch.Tensor, tile_out: torch.Tensor, bboxes: Sequence[BBox], N: int, tile_weights: torch.Tensor,
