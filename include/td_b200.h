@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define TD_ABI_VERSION 13
+#define TD_ABI_VERSION 14
 
 typedef enum td_status {
     TD_OK = 0,
@@ -335,11 +335,14 @@ int td_push_regions(const td_push_region* regions, int n_regions, void* const* t
  * multiplied by the fp32 [h*w] `aux` when given: Mixture of Diffusers' custom_weights), mode 1 = FOREGROUND (`aux` =
  * fp32 [h*w] feather mask: averaged over overlapping regions and laid over the normalised background).
  * weights: fp32 [H*W] divide-where->1 canvas (MultiDiffusion) or NULL (Mixture of Diffusers).  out: fp32 [N,C,H,W].
+ * Each region output is read in its own td_dtype, which may differ from the canvas's (a UNet that returns fp32 for an
+ * fp16 latent): it is added as it is, so the accumulator is rounded once per add, as the reference's `+=` rounds it.
  * Every rounding of the reference's tensor expressions is reproduced (see csrc/td_region.cu). */
 #define TD_MAX_REGIONS 32
 typedef struct td_region {
     int32_t x, y, w, h;
     int32_t mode;
+    int32_t dtype;       /* td_dtype of `out` (independent of the canvas dtype) */
     const void* out;     /* region denoiser output [N, C, h, w] of `dtype`, device */
     const float* aux;
 } td_region;

@@ -33,7 +33,7 @@ TD_MAX_GRID_DIM = 256
 TD_MAX_BATCH_PTRS = 128
 TD_MAX_PEERS = 16
 TD_IPC_HANDLE_BYTES = 64
-ABI_VERSION = 13
+ABI_VERSION = 14
 
 DTYPE_CODE = {torch.float16: TD_F16, torch.bfloat16: TD_BF16, torch.float32: TD_F32}
 
@@ -63,7 +63,8 @@ TD_MAX_REGIONS = 32
 
 class TdRegion(ctypes.Structure):
     """struct td_region (include/td_b200.h)."""
-    _fields_ = [("x", c_int32), ("y", c_int32), ("w", c_int32), ("h", c_int32), ("mode", c_int32), ("out", c_void_p), ("aux", c_void_p)]
+    _fields_ = [("x", c_int32), ("y", c_int32), ("w", c_int32), ("h", c_int32), ("mode", c_int32), ("dtype", c_int32), ("out", c_void_p),
+                ("aux", c_void_p)]
 
 
 class TdPushRegion(ctypes.Structure):

@@ -10,6 +10,9 @@
 //   FOREGROUND   fb = round_T(float(fb) + float(r)); fm += mask; fc += 1   (feather buffer in T, mask / count in fp32)
 //   composite    if fc > 1: fbf = float(fb) / fc, fm = fm / fc;  if fc > 0: o = o * (1 - fm) + fbf * fm
 //                (each product and the sum rounded separately: no FMA contraction)
+// r is a region output read in ITS OWN dtype (td_region.dtype), which need not be T: the reference's `x_buffer[slicer] +=
+// x_tile_out` with an fp32 UNet output on an fp16 canvas adds in fp32 and rounds once, so the output must not be rounded
+// to T on its way in.  The dtype is uniform across a region, so the per-visit switch does not diverge.
 // td_region_composite_rows runs the same kernel over a window of canvas rows (the row-strip shard composites only the
 // rows a rank owns); td_region_composite is its [0, H) case.
 #include <cuda_bf16.h>
@@ -34,9 +37,19 @@ struct RegionParams {
     int row_begin, rows;              // canvas rows [row_begin, row_begin + rows) are produced; the rest of `out` is untouched
     int divide;                       // 1: MultiDiffusion normalisation by the weight canvas
     int x[TD_MAX_REGIONS], y[TD_MAX_REGIONS], w[TD_MAX_REGIONS], h[TD_MAX_REGIONS], mode[TD_MAX_REGIONS];
-    const void* out[TD_MAX_REGIONS];      // region denoiser output [N, C, h, w] of T
+    int dtype[TD_MAX_REGIONS];            // td_dtype of out[r]
+    const void* out[TD_MAX_REGIONS];      // region denoiser output [N, C, h, w] of dtype[r]
     const float* aux[TD_MAX_REGIONS];     // BACKGROUND: optional fp32 [h*w] multiplier; FOREGROUND: fp32 [h*w] feather mask
 };
+
+// Element i of a region output of td_dtype dt, exactly as fp32.
+__device__ __forceinline__ float load_region_value(const void* p, long long i, int dt) {
+    switch (dt) {
+        case TD_F16: return Elem<__half>::to_f32(reinterpret_cast<const __half*>(p)[i]);
+        case TD_BF16: return Elem<__nv_bfloat16>::to_f32(reinterpret_cast<const __nv_bfloat16*>(p)[i]);
+        default: return reinterpret_cast<const float*>(p)[i];
+    }
+}
 
 template <typename T>
 __global__ void __launch_bounds__(256)
@@ -55,7 +68,7 @@ region_composite_kernel(const __grid_constant__ RegionParams p, const T* __restr
             const int u = px - p.x[r], v = py - p.y[r];
             if ((unsigned)u >= (unsigned)p.w[r] || (unsigned)v >= (unsigned)p.h[r]) continue;
             const long long ro = (plane * p.h[r] + v) * (long long)p.w[r] + u;
-            const float val = Elem<T>::to_f32(reinterpret_cast<const T*>(p.out[r])[ro]);
+            const float val = load_region_value(p.out[r], ro, p.dtype[r]);
             if (p.mode[r] == 0) {
                 const float add = p.aux[r] != nullptr ? __fmul_rn(val, p.aux[r][(long long)v * p.w[r] + u]) : val;
                 acc = round_through<T>(__fadd_rn(acc, add));
@@ -86,6 +99,10 @@ int region_composite_launch(const char* fn, const void* x_buffer, const float* w
         td_set_error("%s: bad arguments", fn);
         return TD_ERR_INVALID_ARG;
     }
+    if (dtype != TD_F16 && dtype != TD_BF16 && dtype != TD_F32) {
+        td_set_error("%s: unknown dtype %d", fn, dtype);
+        return TD_ERR_INVALID_ARG;
+    }
     if (row_begin < 0 || row_begin > row_end || row_end > H) {
         td_set_error("%s: rows [%d,%d) outside [0,%d)", fn, row_begin, row_end, H);
         return TD_ERR_INVALID_ARG;
@@ -98,11 +115,11 @@ int region_composite_launch(const char* fn, const void* x_buffer, const float* w
     for (int r = 0; r < n_regions; ++r) {
         const td_region& g = regions[r];
         if (g.x < 0 || g.y < 0 || g.w <= 0 || g.h <= 0 || g.x + g.w > W || g.y + g.h > H || g.out == nullptr || (g.mode != 0 && g.mode != 1) ||
-            (g.mode == 1 && g.aux == nullptr)) {
+            (g.mode == 1 && g.aux == nullptr) || (g.dtype != TD_F16 && g.dtype != TD_BF16 && g.dtype != TD_F32)) {
             td_set_error("%s: region %d is invalid", fn, r);
             return TD_ERR_INVALID_ARG;
         }
-        p.x[r] = g.x; p.y[r] = g.y; p.w[r] = g.w; p.h[r] = g.h; p.mode[r] = g.mode; p.out[r] = g.out; p.aux[r] = g.aux;
+        p.x[r] = g.x; p.y[r] = g.y; p.w[r] = g.w; p.h[r] = g.h; p.mode[r] = g.mode; p.dtype[r] = g.dtype; p.out[r] = g.out; p.aux[r] = g.aux;
     }
     if (p.rows == 0) return TD_OK;
     const long long total = (long long)N * C * p.rows * W;
@@ -112,7 +129,6 @@ int region_composite_launch(const char* fn, const void* x_buffer, const float* w
         case TD_F16: region_composite_kernel<__half><<<grid, 256, 0, st>>>(p, (const __half*)x_buffer, weights, out); break;
         case TD_BF16: region_composite_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>(p, (const __nv_bfloat16*)x_buffer, weights, out); break;
         case TD_F32: region_composite_kernel<float><<<grid, 256, 0, st>>>(p, (const float*)x_buffer, weights, out); break;
-        default: td_set_error("%s: unknown dtype %d", fn, dtype); return TD_ERR_INVALID_ARG;
     }
     return launch_status(fn);
 }

@@ -312,7 +312,8 @@ def _region_table(xb: torch.Tensor, regions: Sequence[tuple]):
     keep = []
     for i, (rx, ry, rw, rh, mode, r_out, aux) in enumerate(regions):
         _require_cuda(r_out, "region output")
-        ro = r_out.to(xb.dtype).contiguous()
+        # read in the dtype the denoiser returned: rounding it to the canvas dtype first would round the add twice
+        ro = r_out.contiguous()
         if tuple(ro.shape) != (N, C, rh, rw):
             raise ValueError(f"region {i}: output shape {tuple(ro.shape)} != {(N, C, rh, rw)}")
         ax = None
@@ -320,7 +321,8 @@ def _region_table(xb: torch.Tensor, regions: Sequence[tuple]):
             ax = aux.to(device=xb.device, dtype=torch.float32).expand(rh, rw).contiguous() if aux.dim() == 2 else \
                 aux.to(device=xb.device, dtype=torch.float32).reshape(rh, rw).contiguous()
         keep += [ro, ax]
-        arr[i] = TdRegion(int(rx), int(ry), int(rw), int(rh), int(mode), ro.data_ptr(), ax.data_ptr() if ax is not None else None)
+        arr[i] = TdRegion(int(rx), int(ry), int(rw), int(rh), int(mode), dtype_code(ro.dtype), ro.data_ptr(),
+                          ax.data_ptr() if ax is not None else None)
     return arr, keep
 
 

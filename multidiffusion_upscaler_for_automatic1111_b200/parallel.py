@@ -89,12 +89,20 @@ class RegionShard:
         """Elements of one rank's padded output pack (planes = N * C)."""
         return planes * max(sum(self._area(j) for j in self.mine(r)) for r in range(self.world))
 
-    def pack_outputs(self, outs: Sequence[torch.Tensor], planes: int, like: torch.Tensor) -> torch.Tensor:
-        """This rank's region outputs (in `mine()` order, [N, C, h, w] each) -> one flat padded pack of like's dtype."""
+    def pack_outputs(self, outs: Sequence[torch.Tensor], planes: int, like: torch.Tensor,
+                     dtype: Optional[torch.dtype] = None) -> torch.Tensor:
+        """This rank's region outputs (in `mine()` order, [N, C, h, w] each) -> one flat padded pack of `dtype` (default:
+        like's dtype) on like's device.  The pack must carry the values the denoiser returned -- an fp32 output on an fp16
+        latent rounded to fp16 here would be rounded twice by the composite -- so an output is packed only into its own
+        dtype or into fp32, which holds every output dtype exactly; anything else is refused."""
         mine = self.mine()
         if len(outs) != len(mine):
             raise ValueError(f"{len(outs)} region outputs for {len(mine)} regions of rank {self.rank}")
-        pack = torch.zeros(self.output_pack_numel(planes), dtype=like.dtype, device=like.device)
+        dtype = like.dtype if dtype is None else dtype
+        for j, o in zip(mine, outs):
+            if o.dtype != dtype and dtype != torch.float32:
+                raise ValueError(f"region {j}: a {o.dtype} output does not fit a {dtype} pack exactly")
+        pack = torch.zeros(self.output_pack_numel(planes), dtype=dtype, device=like.device)
         off = 0
         for j, o in zip(mine, outs):
             n = planes * self._area(j)
@@ -166,9 +174,11 @@ def gather_region_inputs(rs: RegionShard, x: torch.Tensor, B: Sequence[int], gro
 
 
 def exchange_region_outputs(rs: RegionShard, outs: Sequence[torch.Tensor], like: torch.Tensor, group=None) -> List[torch.Tensor]:
-    """One all-gather of the packed region outputs -> every region's output, in list order, on every rank."""
+    """One all-gather of the packed region outputs -> every region's output, in list order, on every rank.  The packs are
+    fp32 on every rank: exact for every output dtype, and the same on a rank that owns no region and so cannot know the
+    UNet's output dtype, without a collective to agree on one (DESIGN.md section 5)."""
     N, C = like.shape[0], like.shape[1]
-    gathered = gather_tile_outputs(rs.pack_outputs(outs, N * C, like).view(1, -1), group)
+    gathered = gather_tile_outputs(rs.pack_outputs(outs, N * C, like, torch.float32).view(1, -1), group)
     return rs.unpack_outputs(gathered, N, C)
 
 

@@ -36,6 +36,18 @@ def test_grid_struct_layout_matches_header():
     assert _cabi.TdGrid.wrap.offset == 4 * 10 and _cabi.TdGrid.ys.offset == 4 * 11
 
 
+def test_region_struct_layout_matches_header():
+    """struct td_region: five int32 geometry / mode fields, the output's dtype in what used to be padding, two pointers."""
+    from multidiffusion_upscaler_for_automatic1111_b200 import _cabi
+    assert ctypes.sizeof(_cabi.TdRegion) == 40
+    assert [(n, getattr(_cabi.TdRegion, n).offset) for n, _ in _cabi.TdRegion._fields_] == \
+        [("x", 0), ("y", 4), ("w", 8), ("h", 12), ("mode", 16), ("dtype", 20), ("out", 24), ("aux", 32)]
+    src = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "td_b200.h")).read(), flags=re.S)
+    body = re.search(r"typedef struct td_region \{(.*?)\} td_region;", src, flags=re.S).group(1)
+    declared = [n for decl in body.split(";") if decl.strip() for n in re.findall(r"\*?\s*(\w+)\s*(?:,|$)", decl.strip())]
+    assert declared == [n for n, _ in _cabi.TdRegion._fields_], f"header fields {declared}"
+
+
 def test_missing_library_fails_loudly(tmp_path, monkeypatch):
     """No silent fallback: a missing .so is an ImportError naming the build command."""
     import importlib

@@ -90,6 +90,36 @@ def test_region_plan_owns_every_region_once_and_round_trips(world):
                 assert torch.equal(t.view(torch.int16), x[:, :, ry:ry + h, rx:rx + w].contiguous().view(torch.int16))
 
 
+@pytest.mark.parametrize("world", [1, 3])
+def test_region_output_exchange_carries_every_output_dtype_exactly(world, monkeypatch):
+    """The exchange packs fp32 whatever the latent dtype, so fp16, bf16 and fp32 outputs all reach the composite as the UNet
+    returned them; a pack that would round an output (fp32 into fp16, fp16 into bf16) is refused."""
+    from multidiffusion_upscaler_for_automatic1111_b200 import parallel
+    N, C, H, W = 2, 3, 48, 64
+    rects = _rects(5)
+    shards = [parallel.RegionShard(rects, r, world) for r in range(world)]
+    like = torch.empty((N, C, H, W), dtype=torch.float16)
+    for odt in (torch.float16, torch.bfloat16, torch.float32):
+        # values with more significant bits than fp16 / bf16 keep, before the cast to odt
+        outs = [synth.latent(100 + j, (N, C, h, w), torch.float32).mul_(1.0 + 2 ** -20).to(odt) for j, (_, _, w, h) in enumerate(rects)]
+        packs = [s.pack_outputs([outs[j] for j in s.mine()], N * C, like, torch.float32) for s in shards]
+        assert all(p.dtype == torch.float32 for p in packs)
+        def all_gather(local, group=None):       # every rank's pack, as the collective returns them
+            assert local.dtype == torch.float32 and local.numel() == packs[0].numel()
+            return torch.stack(packs)
+        monkeypatch.setattr(parallel, "gather_tile_outputs", all_gather)
+        for s in shards:
+            got = parallel.exchange_region_outputs(s, [outs[j] for j in s.mine()], like)
+            assert all(a.dtype == torch.float32 and torch.equal(a, b.float()) and torch.equal(a.to(odt).view(torch.uint8), b.view(torch.uint8))
+                       for a, b in zip(got, outs)), odt
+    mine = shards[0].mine()
+    f32 = [synth.latent(7, (N, C, rects[j][3], rects[j][2]), torch.float32) for j in mine]
+    with pytest.raises(ValueError, match="does not fit"):
+        shards[0].pack_outputs(f32, N * C, like)
+    with pytest.raises(ValueError, match="does not fit"):
+        shards[0].pack_outputs([o.half() for o in f32], N * C, like, torch.bfloat16)
+
+
 # ------------------------------------------------------------------------------------------------ strip simulation (no GPU)
 # canvas 48 x 120, tiles 16 / overlap 8: 14 tile rows; at 6 ranks the strips are [0,24) [24,48) [48,64) [64,80) [80,96) [96,120)
 STRIP_GEOM = dict(W=48, H=120, tw=16, th=16, ov=8)
@@ -290,6 +320,85 @@ def _gloo_region_worker(rank, world, port, result_dir):
 @pytest.mark.parametrize("world", [2, 3])
 def test_gloo_sharded_delegates_with_regions_equal_single(tmp_path, world):
     mp.spawn(_gloo_region_worker, args=(world, _free_port(), str(tmp_path)), nprocs=world, join=True)
+    assert all((tmp_path / f"ok{r}").exists() for r in range(world))
+
+
+_K = torch.tensor(0.7071, dtype=torch.float32)      # fp32 UNet stand-ins: outputs with more bits than the fp16 latent
+
+
+def _f32_denoise(t, bb, N):
+    return synth.fake_denoise(t.float(), bb, N) * _K
+
+
+def _f32_region_denoise(t, j):
+    return synth.fake_region_denoise(t.float(), j) * _K
+
+
+def _oracle_step_f32(method, x, bg, rows, region_denoise=_f32_region_denoise):
+    c = GRID
+    N = x.shape[0]
+    plan = tiling.GridPlan(c["W"], c["H"], c["tw"], c["th"], c["ov"], c["bs"], method == "mod")
+    regs = region.make_regions(rows, c["W"], c["H"])
+    w = region.weights_with_regions(plan.weights if bg else None, regs, c["H"], c["W"], method)
+    den = lambda t, bb: _f32_denoise(t, bb, N)
+    if method == "md":
+        return region.multidiffusion_region_step(x, plan.batched_bboxes, w, regs, den, region_denoise, bg)
+    return region.mixture_region_step(x, plan.batched_bboxes, plan.tile_weights, w, regs, den, region_denoise, bg)
+
+
+def _gloo_f32_unet_worker(rank, world, port, result_dir, n_rows):
+    """A UNet that returns fp32 for an fp16 latent, sharded: the region outputs cross the all-gather as the UNet returned
+    them (also from and to a rank that owns no region), so every rank composites what one process composites."""
+    from multidiffusion_upscaler_for_automatic1111_b200 import MixtureOfDiffusers, MultiDiffusion, host
+    _install_oracle_engine()
+    _init(rank, world, port, "gloo")
+    try:
+        c = GRID
+        N = c["N"]
+        rows = ROWS[:n_rows]
+        for method in ("md", "mod"):
+            for bg in (True, False):
+                host.use_shared(types.SimpleNamespace(state=types.SimpleNamespace(interrupted=False, sampling_step=0, sampling_steps=1),
+                                                      sd_model=None))
+                d = (MultiDiffusion if method == "md" else MixtureOfDiffusers)(_p(c), _sampler())
+                d.init_grid_bbox(c["tw"], c["th"], c["ov"], c["bs"])
+                d.init_custom_bbox({i: row for i, row in enumerate(rows)}, bg, False)
+                d.init_done()
+                d.init_tile_shard(None, fused=False)
+                x = synth.latent(45, (N, c["C"], c["H"], c["W"]), torch.float16)
+                if method == "md":
+                    got = d.sample_one_step(x, None, lambda t, bb: _f32_denoise(t, bb, N), lambda t, j, b: _f32_region_denoise(t, j))
+                else:
+                    it = {"i": 0}
+
+                    def apply_model(x_tile, t, c_):
+                        bb = d.local_batched_bboxes[it["i"]]
+                        it["i"] += 1
+                        return _f32_denoise(x_tile, bb, N)
+                    model = types.SimpleNamespace(apply_model=apply_model, cond_stage_key="txt",
+                                                  model=types.SimpleNamespace(conditioning_key="crossattn"))
+                    host.get_shared().sd_model = model
+                    d.custom_apply_model = lambda x_tile, t, c_, bbox_id, bbox: _f32_region_denoise(x_tile, bbox_id)
+                    d.hook()
+                    got = model.apply_model(x, torch.ones(N), {"c_crossattn": [torch.zeros(N, 2, 4)], "c_concat": [torch.zeros(N, 5, 1, 1)]})
+                    MixtureOfDiffusers.unhook()
+                want = _oracle_step_f32(method, x, bg, rows)
+                assert got.dtype == want.dtype and torch.equal(got.view(torch.uint8), want.view(torch.uint8)), \
+                    f"rank {rank} {method} bg={bg}: sharded step with fp32 region outputs differs from one process"
+                # outputs rounded to the latent dtype before the add give another result (not without a background: the
+                # first add into zeros is that rounding)
+                rounded = _oracle_step_f32(method, x, bg, rows, lambda t, j: _f32_region_denoise(t, j).to(t.dtype))
+                assert not bg or not torch.equal(rounded, want), f"{method}: rounding the region outputs first changes nothing"
+                host.use_shared(None)
+        open(os.path.join(result_dir, f"ok{rank}"), "w").close()
+    finally:
+        dist.destroy_process_group()
+
+
+@pytest.mark.parametrize("world,n_rows", [(2, len(ROWS)), (3, 2)])
+def test_gloo_sharded_delegates_with_fp32_region_outputs_equal_single(tmp_path, world, n_rows):
+    """(3, 2): rank 2 owns no region and still packs and receives fp32."""
+    mp.spawn(_gloo_f32_unet_worker, args=(world, _free_port(), str(tmp_path), n_rows), nprocs=world, join=True)
     assert all((tmp_path / f"ok{r}").exists() for r in range(world))
 
 
