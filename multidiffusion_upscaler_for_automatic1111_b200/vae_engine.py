@@ -385,10 +385,13 @@ class ModuleBackend:
 
 FOLD_UPSAMPLE = os.environ.get("TD_VAE_FOLD_UPSAMPLE", "1") != "0"     # 0: materialise the upsampled tensor (measurement only)
 DUAL_OUTPUT = os.environ.get("TD_VAE_DUAL_OUTPUT", "1") != "0"         # 0: separate GroupNorm pass at block boundaries (measurement only)
-# Attention tiles with more tokens than this run the fused kernel (vae_ops.attention): their fp16 [T, T] score matrix
-# would pass 2^31 elements (4 GiB), and the reference's H100 default tiles (decoder 256, encoder 3072) need 11-27 GiB of
-# it.  Smaller tiles keep the four-GEMM path and its exact output.  The bound depends only on the tile, so a tile takes
-# the same path, with the same bits, on any card.
+# Attention tiles with more tokens than this run the fused kernel (vae_ops.attention): 46340 = floor(sqrt(2^31)), so
+# their [T, T] score matrix would pass 2^31 elements (4 GiB in fp16), and the reference's H100 default tiles (decoder
+# 256, encoder 3072) need 11-27 GiB of it.  Smaller tiles keep the four-GEMM path and its exact output.  That path
+# allocates the scores as [T, Tp], Tp = round_up(T, 8), so its largest matrix (T = 46340: 46340 x 46344 =
+# 2^31 + 97312 elements) does pass 2^31 elements; the score GEMM, softmax_rows and the P V GEMM address it with 64-bit
+# offsets (tests/test_gpu_vae_large_tiles.py checks that tile).  The bound depends only on the tile, so a tile takes the
+# same path, with the same bits, on any card.
 SCORE_MATRIX_MAX_TOKENS = 46340
 
 

@@ -58,16 +58,23 @@ def launched(fn) -> set:
     no kernel at all, so that a profiler without CUPTI cannot make the form assertions vacuous.
 
     A single session can come back incomplete: back-to-back short sessions occasionally lose an activity buffer, all of
-    it (an empty trace) or part of it (one kernel of the call missing).  So `fn`, which must be repeatable and launch
-    the same kernels every time, runs in sessions until two non-empty ones in a row record the same names (at most six
-    sessions), and the union of what they recorded is returned: a kernel counts as launched when any session saw it."""
+    it (an empty trace) or part of it (the kernels launched first or last missing: every session of a call can lose
+    the same leading kernels).  So each session brackets `fn` with a marker kernel (torch's spin_kernel) before and
+    after it, each waited for, and counts as complete only when both markers are in its trace.  `fn`, which must be
+    repeatable and launch the same kernels every time, runs in sessions until two complete ones in a row record the
+    same names (at most eight sessions), and the union of what all sessions recorded is returned: a kernel counts as
+    launched when any session saw it."""
     from torch.profiler import ProfilerActivity, profile
     seen, prev = set(), None
-    for attempt in range(6):
+    for attempt in range(8):
         time.sleep(0.1 * attempt)
         torch.cuda.synchronize()
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            torch.cuda._sleep(1000)
+            torch.cuda.synchronize()
             fn()
+            torch.cuda.synchronize()
+            torch.cuda._sleep(1000)
             torch.cuda.synchronize()
         names = {e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA}
         with tempfile.TemporaryDirectory() as d:
@@ -75,11 +82,16 @@ def launched(fn) -> set:
             prof.export_chrome_trace(path)
             with open(path) as f:
                 trace = json.load(f)
-        names |= {e.get("name", "") for e in trace.get("traceEvents", []) if e.get("cat") == "kernel"}
+        kernels = [e.get("name", "") for e in trace.get("traceEvents", []) if e.get("cat") == "kernel"]
+        names |= set(kernels)
         names.discard("")
+        markers = sum("spin_kernel" in n for n in kernels)
+        names = {n for n in names if "spin_kernel" not in n}
         if not names:
             continue
         seen |= names
+        if markers < 2:
+            continue
         if names == prev:
             break
         prev = names

@@ -26,6 +26,7 @@ Bounds (u_out: unit roundoff of the output format, 2^-11 fp16 / 2^-8 bf16; tau: 
   gn_apply       see `_gn_apply64`; gn_stats uses the tolerances of the existing statistics tests.
   layout, upsample, wrap: bit-exact.
 """
+import contextlib
 import ctypes
 import copy
 import inspect
@@ -244,8 +245,9 @@ def _assert_nan_kept(buf, region, what):
 
 
 # ------------------------------------------------------------------------------------------------ attention / softmax / GN
-def _attention64(q, k, v, alpha, dt, rows=256, stale_max=False):
-    """Float64 softmax(alpha q k^T) v and its per-element bound, `rows` queries at a time (no T x T matrix for large T).
+def _attention64(q, k, v, alpha, dt, rows=256, stale_max=False, qidx=None):
+    """Float64 softmax(alpha q k^T) v and its per-element bound, `rows` queries at a time (no T x T matrix for large T);
+    qidx: only these query rows (the output has one row per index), against all T keys.
 
     The kernel computes S in fp32 (products over C: gamma_C = C 2^-22 per |q||k| sum; the two warpgroup partials'
     add, the scale by alpha log2(e) and that constant: 4 e32 |S| more), so the logit of key j is off by at most
@@ -259,16 +261,16 @@ def _attention64(q, k, v, alpha, dt, rows=256, stale_max=False):
         kappa = u_in + 2 E + 2 blocks (2^-22 + e32) + T 2^-22 + T e32 + 2^-22 (the final 1 / l and product),
         |got - ref| <= u_out |ref| + (1 + u_out) (kappa sum_j p_j |v_j| + tau_P sum_j |v_j| / l) + tau.
     stale_max: the mutated reference of an online softmax that never rescales earlier key blocks."""
-    T, C = q.shape
+    T, C = k.shape
     alpha = float(torch.tensor(alpha, dtype=torch.float32))
-    qd, kd, vd = q.double(), k.double(), v.double()
+    qd, kd, vd = (q if qidx is None else q[qidx]).double(), k.double(), v.double()
     kabs, vabs = kd.abs(), vd.abs()
     vsum = vabs.sum(0, keepdim=True)
-    out = torch.empty((T, C), dtype=torch.float64, device=q.device)
+    out = torch.empty((qd.shape[0], C), dtype=torch.float64, device=q.device)
     bnd = torch.empty_like(out)
     blocks = (T + 63) // 64
     tau_p = 2.0 ** -25 if dt == torch.float16 else 0.0
-    for r0 in range(0, T, rows):
+    for r0 in range(0, qd.shape[0], rows):
         S = qd[r0:r0 + rows] @ kd.t()
         Sabs = qd[r0:r0 + rows].abs() @ kabs.t()
         L = alpha * S
@@ -436,12 +438,10 @@ def _sd_width_net(is_dec, seed):
 CENSUS_RUNS = [(True, 40, 52, 16), (False, 200, 264, 64)]
 
 
-def record_census():
-    """Distinct call signatures TensorCoreBackend issues for the SD-width encoder and decoder, fp16 and bf16, fast and
-    slow mode."""
-    from multidiffusion_upscaler_for_automatic1111_b200 import tilevae
+@contextlib.contextmanager
+def census_spy():
+    """While active, the signature of every vae_engine.ops call in SPIED is added to the yielded set."""
     from multidiffusion_upscaler_for_automatic1111_b200 import vae_engine as ve
-    from oracle import synth
     seen = set()
     real = {n: getattr(ve.ops, n) for n in SPIED}
 
@@ -453,20 +453,32 @@ def record_census():
     try:
         for n in SPIED:
             setattr(ve.ops, n, spy(n))
-        for is_dec, H, W, tile in CENSUS_RUNS:
+        yield seen
+    finally:
+        for n in SPIED:
+            setattr(ve.ops, n, real[n])
+
+
+def record_census(runs=CENSUS_RUNS, dtypes=tuple(DTS.values())):
+    """Distinct call signatures TensorCoreBackend issues for the SD-width encoder and decoder, fp16 and bf16, fast and
+    slow mode.  runs: (is_decoder, H, W, tile[, one_tile]); one_tile: the input is exactly one padded tile, run through
+    vae_tile_forward (VAEHook.__call__ runs an input that small through the network untiled)."""
+    from multidiffusion_upscaler_for_automatic1111_b200 import tilevae
+    from oracle import synth
+    with census_spy() as seen:
+        for is_dec, H, W, tile, *one in runs:
             base = _sd_width_net(is_dec, 3 if is_dec else 4)
-            for dt in DTS.values():
+            for dt in dtypes:
                 net = copy.deepcopy(base).cuda().to(dt)
                 z = synth.latent(5 if is_dec else 6, (1, 4 if is_dec else 3, H, W), dt).cuda()
                 for fast in (True, False):
                     hook = tilevae.VAEHook(net, tile, is_dec, fast_decoder=fast, fast_encoder=fast, color_fix=False)
                     with torch.no_grad():
-                        hook(z)
+                        out = hook.vae_tile_forward(z) if one and one[0] else hook(z)
                     assert hook.backend_name == "wgmma"
-                del net
-    finally:
-        for n in SPIED:
-            setattr(ve.ops, n, real[n])
+                    del out
+                del net, z
+                torch.cuda.empty_cache()
     return sorted(seen, key=repr)
 
 

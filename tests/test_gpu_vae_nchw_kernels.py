@@ -230,13 +230,21 @@ def _stats64(x, nseg, seg_len, unbiased, aligned=True):
     del k
     S = (sh * sh).sum(1)
     del sh
+    var, e_mean, e_var = _stats_bounds(mu, m2, R, S, seg_len, n_t, D, unbiased)
+    return mu, var, xs.amin(1), xs.amax(1), e_mean, e_var
+
+
+def _stats_bounds(mu, m2, R, S, n, n_t, D, unbiased, merge_roundings=(3, 4)):
+    """(var, e_mean, e_var) of the module docstring from the float64 moments of each segment (n elements, at most n_t
+    per thread, merge depth D).  merge_roundings: the roundings per merge in the mean and M2 terms (3 and 4 here)."""
+    rm, rq = merge_roundings
     u = E32
-    e_mean = u * ((D + 2) * (mu.abs() + R) + (n_t + 3 * D) * 2 * R)
-    e_m2 = u * (n_t + 4 + 4 * D) * (S + m2) + 4 * D * seg_len * R * e_mean
-    nd = seg_len - 1 if unbiased else seg_len
+    e_mean = u * ((D + 2) * (mu.abs() + R) + (n_t + rm * D) * 2 * R)
+    e_m2 = u * (n_t + 4 + rq * D) * (S + m2) + 4 * D * n * R * e_mean
+    nd = n - 1 if unbiased else n
     var = m2 / max(nd, 1)
     e_var = e_m2 / max(nd, 1) + u * var
-    return mu, var, xs.amin(1), xs.amax(1), e_mean, e_var
+    return var, e_mean, e_var
 
 
 def _check_stats(x, nseg, seg_len, unbiased, what, minmax=True, aligned=True):
