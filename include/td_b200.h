@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define TD_ABI_VERSION 14
+#define TD_ABI_VERSION 15
 
 typedef enum td_status {
     TD_OK = 0,
@@ -130,6 +130,30 @@ int td_grid_weights(const td_grid* g, const float* tile_weights, float* out_weig
 
 /* rescale_factor = 1 / weights -- mixtureofdiffusers.py:32 (fp32 IEEE divide). */
 int td_rescale_factor(const float* weights, float* out, int64_t n);
+
+/* SpotDiffusion step plans (new: the reference has no such method).  `base` is a td_grid_init plan.  On each axis let L be
+ * its length, t the tile size, b_0 < ... < b_{n-1} the base origins and g the smallest gap between neighbouring origins
+ * (on a wrapped axis the gap L + b_0 - b_{n-1} across the seam included, g = L when n = 1).  One denoiser call with shift s
+ * on an axis uses:
+ *   bounded, n >= 2 and g >= 2:  s in [1, g), origins 0, b_1 - s, ..., b_{n-1} - s, L - t   (n + 1 windows, inside the canvas);
+ *   bounded, n == 1 or g < 2:    s == 0, the base origins;
+ *   wrapped:                     s in [0, g), origins (b_k - s) mod L in ascending order   (n windows).
+ * The window count depends on the geometry only.
+ *
+ * td_grid_shift_bounds writes [lo_x, hi_x, lo_y, hi_y): the shifts td_grid_shift accepts.  TD_OK or TD_ERR_INVALID_ARG.
+ * td_grid_shift writes the step plan of (shift_x, shift_y) to `out`, with num_batches / tile_bs re-balanced from `tile_bs` as
+ * td_grid_init does, and returns its tile count T.  TD_ERR_INVALID_ARG for a null pointer, a malformed base or a shift
+ * outside the bounds; TD_ERR_UNSUPPORTED when an axis would get more than TD_MAX_GRID_DIM windows.  `out` is left untouched
+ * on every refusal. */
+int td_grid_shift_bounds(const td_grid* base, int32_t out[4]);
+int td_grid_shift(const td_grid* base, int shift_x, int shift_y, int tile_bs, td_grid* out);
+
+/* Device weight canvas of a plan (csrc/td_spot.cu): weights[y*W + x] = (tile rows covering y) * (tile columns covering x),
+ * coverage modular on wrapped axes, and, when rcp_weights is not NULL, rcp_weights = RN(1 / weights).  Bit-equal to
+ * td_grid_weights(g, NULL, .) and td_rescale_factor.  weights, rcp_weights: DEVICE fp32 [H*W], 16-byte aligned.  Refuses
+ * (TD_ERR_INVALID_ARG, outputs untouched) what td_grid_weights and the grid entries refuse -- a tile leaving a bounded axis,
+ * decreasing origins -- and null or misaligned outputs; TD_ERR_UNSUPPORTED for a canvas side of 32768 or more. */
+int td_grid_counts(const td_grid* g, float* weights, float* rcp_weights, void* stream);
 
 /* ------------------------------------------------------------------------- *
  *  Device kernels: per-sampler-step hot path.

@@ -9,9 +9,9 @@ Importing this package loads `libtd_b200.so`; if it is missing the import fails
 (there is no CPU / PyTorch fallback).
 """
 from . import _cabi  # noqa: F401  (loads the shared library or raises)
-from .tile_methods import AbstractDiffusion, DemoFusion, MixtureOfDiffusers, MultiDiffusion
+from .tile_methods import AbstractDiffusion, DemoFusion, MixtureOfDiffusers, MultiDiffusion, SpotDiffusion
 from .tile_utils.utils import BBox, Method, gaussian_weights, split_bboxes, splitable
 from .tilevae import GroupNormParam, VAEHook
 
-__all__ = ["AbstractDiffusion", "MultiDiffusion", "MixtureOfDiffusers", "DemoFusion", "VAEHook", "GroupNormParam", "BBox", "Method", "split_bboxes",
+__all__ = ["AbstractDiffusion", "MultiDiffusion", "MixtureOfDiffusers", "DemoFusion", "SpotDiffusion", "VAEHook", "GroupNormParam", "BBox", "Method", "split_bboxes",
            "splitable", "gaussian_weights"]

@@ -33,7 +33,7 @@ TD_MAX_GRID_DIM = 256
 TD_MAX_BATCH_PTRS = 128
 TD_MAX_PEERS = 16
 TD_IPC_HANDLE_BYTES = 64
-ABI_VERSION = 14
+ABI_VERSION = 15
 
 DTYPE_CODE = {torch.float16: TD_F16, torch.bfloat16: TD_BF16, torch.float32: TD_F32}
 
@@ -103,6 +103,9 @@ _SIGNATURES = {
     "td_grid_init": (c_int, [POINTER(TdGrid), c_int, c_int, c_int, c_int, c_int, c_int, c_int]),
     "td_grid_weights": (c_int, [POINTER(TdGrid), POINTER(c_float), POINTER(c_float)]),
     "td_rescale_factor": (c_int, [POINTER(c_float), POINTER(c_float), c_int64]),
+    "td_grid_shift_bounds": (c_int, [POINTER(TdGrid), POINTER(c_int32)]),
+    "td_grid_shift": (c_int, [POINTER(TdGrid), c_int, c_int, c_int, POINTER(TdGrid)]),
+    "td_grid_counts": (c_int, [POINTER(TdGrid), c_void_p, c_void_p, c_void_p]),
     "td_scatter_tiles": (c_int, [POINTER(TdGrid), c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_uint32, c_void_p]),
     "td_blend_multidiffusion": (c_int, [POINTER(TdGrid), POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_int,
                                         c_void_p, c_void_p, c_void_p, c_void_p, c_uint32, c_void_p]),

@@ -283,6 +283,107 @@ extern "C" int td_grid_weights(const td_grid* g, const float* tile_weights, floa
     return TD_OK;
 }
 
+// ---------------------------------------------------------------------------------------------------------
+// SpotDiffusion step plans: the base plan with every window moved back by a per-call shift (td_b200.h).
+// ---------------------------------------------------------------------------------------------------------
+namespace {
+
+struct ShiftAxis {
+    int lo, hi;  // accepted shifts [lo, hi)
+    bool grows;  // bounded axis that gains the window at L - t
+};
+
+// One axis of a base plan: origins in [0, L), inside the canvas when bounded, non-decreasing.
+bool valid_axis(const int32_t* b, int n, int L, int t, bool periodic) {
+    if (n < 1 || n > TD_MAX_GRID_DIM || L <= 0 || t <= 0 || t > L) return false;
+    for (int k = 0; k < n; ++k)
+        if (b[k] < 0 || b[k] >= L || (!periodic && b[k] + t > L) || (k > 0 && b[k] < b[k - 1])) return false;
+    return true;
+}
+
+ShiftAxis shift_axis_bounds(const int32_t* b, int n, int L, bool periodic) {
+    int gap = periodic ? L + b[0] - b[n - 1] : L;  // n == 1: L
+    for (int k = 1; k < n; ++k) gap = std::min(gap, b[k] - b[k - 1]);
+    if (periodic) return {0, gap, false};
+    if (n >= 2 && gap >= 2) return {1, gap, true};
+    return {0, 1, false};
+}
+
+int shift_axis(const int32_t* b, int n, int L, int t, bool periodic, const ShiftAxis& ax, int s, int32_t* out) {
+    if (periodic) {
+        for (int k = 0; k < n; ++k) out[k] = ((b[k] - s) % L + L) % L;
+        std::sort(out, out + n);
+        return n;
+    }
+    if (!ax.grows) {
+        std::copy(b, b + n, out);
+        return n;
+    }
+    out[0] = 0;
+    for (int k = 1; k < n; ++k) out[k] = b[k] - s;
+    out[n] = L - t;
+    return n + 1;
+}
+
+int check_base(const td_grid* g, const char* what) {
+    if (g == nullptr || (g->wrap & ~(int)(TD_WRAP_X | TD_WRAP_Y)) != 0 ||
+        !valid_axis(g->xs, g->cols, g->W, g->tile_w, (g->wrap & TD_WRAP_X) != 0) ||
+        !valid_axis(g->ys, g->rows, g->H, g->tile_h, (g->wrap & TD_WRAP_Y) != 0)) {
+        td_set_error("%s: null or malformed base plan", what);
+        return TD_ERR_INVALID_ARG;
+    }
+    return TD_OK;
+}
+
+}  // namespace
+
+extern "C" int td_grid_shift_bounds(const td_grid* base, int32_t out[4]) {
+    int st = check_base(base, "grid_shift_bounds");
+    if (st != TD_OK) return st;
+    if (out == nullptr) {
+        td_set_error("grid_shift_bounds: null output");
+        return TD_ERR_INVALID_ARG;
+    }
+    const ShiftAxis ax = shift_axis_bounds(base->xs, base->cols, base->W, (base->wrap & TD_WRAP_X) != 0);
+    const ShiftAxis ay = shift_axis_bounds(base->ys, base->rows, base->H, (base->wrap & TD_WRAP_Y) != 0);
+    out[0] = ax.lo; out[1] = ax.hi; out[2] = ay.lo; out[3] = ay.hi;
+    return TD_OK;
+}
+
+extern "C" int td_grid_shift(const td_grid* base, int shift_x, int shift_y, int tile_bs, td_grid* out) {
+    int st = check_base(base, "grid_shift");
+    if (st != TD_OK) return st;
+    if (out == nullptr || tile_bs <= 0) {
+        td_set_error("grid_shift: null output or tile_bs %d <= 0", tile_bs);
+        return TD_ERR_INVALID_ARG;
+    }
+    const bool px = (base->wrap & TD_WRAP_X) != 0, py = (base->wrap & TD_WRAP_Y) != 0;
+    const ShiftAxis ax = shift_axis_bounds(base->xs, base->cols, base->W, px);
+    const ShiftAxis ay = shift_axis_bounds(base->ys, base->rows, base->H, py);
+    if (shift_x < ax.lo || shift_x >= ax.hi || shift_y < ay.lo || shift_y >= ay.hi) {
+        td_set_error("grid_shift: shift (%d, %d) outside [%d, %d) x [%d, %d)", shift_x, shift_y, ax.lo, ax.hi, ay.lo, ay.hi);
+        return TD_ERR_INVALID_ARG;
+    }
+    if (base->cols + (ax.grows ? 1 : 0) > TD_MAX_GRID_DIM || base->rows + (ay.grows ? 1 : 0) > TD_MAX_GRID_DIM) {
+        td_set_error("grid_shift: a %dx%d base plan gains a window row / column past TD_MAX_GRID_DIM=%d", base->rows, base->cols,
+                     TD_MAX_GRID_DIM);
+        return TD_ERR_UNSUPPORTED;
+    }
+    td_grid g;
+    std::memset(&g, 0, sizeof(g));
+    g.W = base->W; g.H = base->H;
+    g.tile_w = base->tile_w; g.tile_h = base->tile_h;
+    g.overlap = base->overlap;
+    g.wrap = base->wrap;
+    g.cols = shift_axis(base->xs, base->cols, base->W, base->tile_w, px, ax, shift_x, g.xs);
+    g.rows = shift_axis(base->ys, base->rows, base->H, base->tile_h, py, ay, shift_y, g.ys);
+    g.num_tiles = g.rows * g.cols;
+    g.num_batches = ceil_div_py(g.num_tiles, tile_bs);                  // as td_grid_init
+    g.tile_bs = ceil_div_py(g.num_tiles, g.num_batches);
+    *out = g;
+    return g.num_tiles;
+}
+
 extern "C" int td_rescale_factor(const float* weights, float* out, int64_t n) {
     if (weights == nullptr || out == nullptr || n < 0) {
         td_set_error("rescale_factor: bad args");

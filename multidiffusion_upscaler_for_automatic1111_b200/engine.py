@@ -156,6 +156,60 @@ def exact_reciprocals(weights_host: np.ndarray) -> Optional[np.ndarray]:
         return rescale_factor(w)
 
 
+def shift_bounds(g: TdGrid):
+    """(lo_x, hi_x, lo_y, hi_y): the shifts `shift_grid` accepts on the base plan g, [lo, hi) per axis (td_grid_shift_bounds)."""
+    out = (ctypes.c_int32 * 4)()
+    check(lib.td_grid_shift_bounds(ctypes.byref(g), out))
+    return tuple(int(v) for v in out)
+
+
+def shift_grid(g: TdGrid, shift_x: int, shift_y: int, tile_bs: int) -> TdGrid:
+    """SpotDiffusion step plan: the base plan g with its windows moved back by (shift_x, shift_y) (td_grid_shift)."""
+    out = TdGrid()
+    check(lib.td_grid_shift(ctypes.byref(g), int(shift_x), int(shift_y), int(tile_bs), ctypes.byref(out)))
+    return out
+
+
+def grid_counts(g: TdGrid, weights: torch.Tensor, rcp_weights: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Writes the plan's count canvas into the device fp32 `weights` (H*W elements), and RN(1/count) into `rcp_weights` when
+    given: `grid_weights(g)` and `rescale_factor` without the host pass and the upload (td_grid_counts).  Returns weights."""
+    n = g.H * g.W
+    for t, what in ((weights, "weights"), (rcp_weights, "rcp_weights")):
+        if t is None:
+            continue
+        _require_cuda(t, what)
+        if t.dtype != torch.float32 or t.numel() != n or not t.is_contiguous():
+            raise ValueError(f"{what} must be a contiguous fp32 tensor of {n} elements (got {t.dtype}, {t.numel()})")
+    with torch.cuda.device(weights.device):
+        check(lib.td_grid_counts(ctypes.byref(g), weights.data_ptr(), rcp_weights.data_ptr() if rcp_weights is not None else None,
+                                 current_stream_ptr(weights.device)))
+    return weights
+
+
+def axis_coverage(origins: Sequence[int], L: int, t: int, periodic: bool) -> np.ndarray:
+    """int64 [L]: how many windows of length t at `origins` cover each position of an axis (modular when periodic).  O(n + L)."""
+    diff = np.zeros(L + 1, dtype=np.int64)
+    for o in origins:
+        end = o + t
+        if periodic and end > L:
+            diff[o] += 1
+            diff[L] -= 1
+            diff[0] += 1
+            diff[end - L] -= 1
+        else:
+            diff[o] += 1
+            diff[end] -= 1
+    return np.cumsum(diff[:L])
+
+
+def counts_allow_fast_divide(g: TdGrid) -> bool:
+    """Whether every count of the plan's canvas is at most 4096, the precondition of td_blend_multidiffusion's rcp_weights.
+    The canvas is the outer product of the per-axis coverages, so their maxima decide it."""
+    cx = axis_coverage(list(g.xs[:g.cols]), g.W, g.tile_w, bool(g.wrap & WRAP_X))
+    cy = axis_coverage(list(g.ys[:g.rows]), g.H, g.tile_h, bool(g.wrap & WRAP_Y))
+    return int(cx.max()) * int(cy.max()) <= 4096
+
+
 def blend_mixture(g: TdGrid, batch_outs: Sequence[torch.Tensor], N: int, C: int, tile_bs: int,
                   tile_weights: torch.Tensor, rescale: torch.Tensor, x_buffer: torch.Tensor, flags: int = 0) -> torch.Tensor:
     """mixtureofdiffusers.py:122-126; writes and returns x_buffer."""

@@ -153,8 +153,7 @@ class AbstractDiffusion:
 
     def init_done(self):
         """abstractdiffusion.py:104-117: sanity check + progress accounting."""
-        rcp = engine.exact_reciprocals(self.weights.detach().to("cpu", torch.float32).numpy().reshape(self.h, self.w))
-        self._rcp_weights = None if rcp is None else torch.from_numpy(rcp).to(self.weights.device)
+        self._init_rcp_weights()
         self.total_bboxes = 0
         if self.enable_grid_bbox:
             self.total_bboxes += self.num_batches
@@ -166,6 +165,11 @@ class AbstractDiffusion:
             from tqdm import tqdm
             steps = getattr(host.get_shared().state, "sampling_steps", 1)
             self.pbar = tqdm(total=self.total_bboxes * steps, desc=f"{self.method} Sampling: ")
+
+    def _init_rcp_weights(self):
+        """RN(1/weights) of the job's weight canvas for the blend's exact fast divide, or None when the canvas does not qualify."""
+        rcp = engine.exact_reciprocals(self.weights.detach().to("cpu", torch.float32).numpy().reshape(self.h, self.w))
+        self._rcp_weights = None if rcp is None else torch.from_numpy(rcp).to(self.weights.device)
 
     # ------------------------------------------------------- cond-dict access
     def _tcond_key(self, cond_dict: CondDict) -> str:
@@ -242,6 +246,10 @@ class AbstractDiffusion:
             raise ValueError("scalar tile weights other than 1.0 are not part of the reference")
         weights = engine.grid_weights(g, tw_np)
         self.weights += torch.from_numpy(weights).view(1, 1, self.h, self.w).to(self.weights.device)
+        self._set_grid_bboxes(g)
+
+    def _set_grid_bboxes(self, g):
+        """num_tiles, num_batches, tile_bs and batched_bboxes of the tile plan g."""
         bboxes = [BBox(int(x), int(y), int(w), int(h)) for x, y, w, h in engine.grid_bboxes_xywh(g)]
         self.num_tiles = len(bboxes)
         self.num_batches = int(g.num_batches)

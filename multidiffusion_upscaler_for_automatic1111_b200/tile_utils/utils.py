@@ -36,6 +36,7 @@ class ComparableEnum(Enum):
 class Method(ComparableEnum):
     MULTI_DIFF = "MultiDiffusion"
     MIX_DIFF = "Mixture of Diffusers"
+    SPOT_DIFF = "SpotDiffusion"
 
 
 class Method_2(ComparableEnum):
