@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define TD_ABI_VERSION 15
+#define TD_ABI_VERSION 16
 
 typedef enum td_status {
     TD_OK = 0,
@@ -483,6 +483,10 @@ typedef struct td_conv_desc {
      * normalised + activated input): the GroupNorm pass over the activation disappears */
     void* y2;
     int64_t y2_pitch;
+    /* elements between the images' post_scale / post_shift vectors: image n reads post_scale[n * post_stride + co].  0: one
+     * vector shared by every image.  Else >= Cout and a multiple of 4 (16 bytes), with post_scale set and a bias per channel.
+     * A tile of output pixels never spans two images, so every pixel takes its own image's constants. */
+    int64_t post_stride;
 } td_conv_desc;
 int td_conv2d_nhwc(const td_conv_desc* d, const void* x, const void* w, const float* bias, const void* residual,
                    void* y, void* stream);
@@ -493,7 +497,8 @@ int td_conv2d_nhwc(const td_conv_desc* d, const void* x, const void* w, const fl
  * convolutions of the low-resolution image, one per output parity, with the 3x3 taps that fall on the same source pixel
  * summed (4/9 of the multiply-adds, no 4x intermediate in HBM).  `d` describes the block as the reference sees it:
  * H x W input, OH = 2H, OW = 2W, kh = kw = 3, stride 1, pad 1; w16: folded taps [16 = (py*2+px)*4 + ty*2 + tx][Cout][w_pitch]
- * (fold in fp32, round once: vae_ops.fold_upsample_weight); no residual; the post_scale / post_shift stage applies. */
+ * (fold in fp32, round once: vae_ops.fold_upsample_weight); no residual; the post_scale / post_shift stage applies (per image with
+ * post_stride).  The N images run in one launch, each on the tiles of its one-image call. */
 int td_upconv2x_nhwc(const td_conv_desc* d, const void* x, const void* w16, const float* bias, void* y, void* stream);
 
 /* The mid-block's single-head attention core (tile_utils/attn.py:49-72: q·kᵀ scaled by alpha, softmax over the keys,
@@ -504,6 +509,12 @@ int td_upconv2x_nhwc(const td_conv_desc* d, const void* x, const void* w16, cons
  * written: the call needs no memory beyond its four operands.  One rounding of o to the storage dtype. */
 int td_attention(const void* q, const void* k, const void* v, void* o, int T, int C, int64_t q_pitch, int64_t k_pitch,
                  int64_t v_pitch, int64_t o_pitch, float alpha, int dtype, void* stream);
+/* td_attention over N images in one launch (1 <= N <= 65535): image n's operands start at q + n * q_img_stride (k, v, o
+ * alike; elements).  Each image runs the CTAs, loads and arithmetic of its td_attention call: the same bits.  Image strides
+ * must be >= T * pitch and multiples of 8 elements; else TD_ERR_INVALID_ARG, o untouched. */
+int td_attention_batched(const void* q, const void* k, const void* v, void* o, int N, int T, int C, int64_t q_pitch,
+                         int64_t k_pitch, int64_t v_pitch, int64_t o_pitch, int64_t q_img_stride, int64_t k_img_stride,
+                         int64_t v_img_stride, int64_t o_img_stride, float alpha, int dtype, void* stream);
 
 /* Channels-last (NHWC) streaming kernels around the tensor-core convolutions (csrc/td_nhwc.cu).  fp16 / bf16.
  *
@@ -532,6 +543,15 @@ int td_gn_stats_nhwc(const void* x, int64_t pixels, int C, int groups, int dtype
 int td_gn_apply_nhwc(const void* x, void* y, int64_t pixels, int C, int groups, int dtype, const float* mean,
                      const float* var, const float* gamma, const float* beta, float eps, int act, void* stream);
 int td_softmax_rows(const void* x, void* y, int rows, int cols, int64_t pitch, int dtype, void* stream);
+/* td_gn_stats_nhwc / td_gn_apply_nhwc of N images in one launch (1 <= N <= 65535).  x (and y): [N, pixels, C] contiguous,
+ * 16-byte aligned; mean / var: fp32 [N, groups].  Each image is reduced with the grid, partials and merge order its
+ * one-image call uses, so its statistics (and its normalised output) are the same bits; offsets are 64-bit.  The workspace
+ * holds N one-image workspaces.  Refusals (sizes, layout, alignment, a short workspace) leave every output untouched. */
+int64_t td_gn_stats_nhwc_batched_workspace_bytes(int N, int64_t pixels, int C, int groups);
+int td_gn_stats_nhwc_batched(const void* x, int N, int64_t pixels, int C, int groups, int dtype, void* workspace,
+                             int64_t workspace_bytes, float* mean, float* var, void* stream);
+int td_gn_apply_nhwc_batched(const void* x, void* y, int N, int64_t pixels, int C, int groups, int dtype, const float* mean,
+                             const float* var, const float* gamma, const float* beta, float eps, int act, void* stream);
 
 #ifdef __cplusplus
 }

@@ -33,7 +33,7 @@ TD_MAX_GRID_DIM = 256
 TD_MAX_BATCH_PTRS = 128
 TD_MAX_PEERS = 16
 TD_IPC_HANDLE_BYTES = 64
-ABI_VERSION = 15
+ABI_VERSION = 16
 
 DTYPE_CODE = {torch.float16: TD_F16, torch.bfloat16: TD_BF16, torch.float32: TD_F32}
 
@@ -86,7 +86,7 @@ class TdConvDesc(ctypes.Structure):
         ("alpha", c_float),
         ("x_pitch", c_int64), ("w_pitch", c_int64), ("y_pitch", c_int64), ("res_pitch", c_int64),
         ("post_scale", c_void_p), ("post_shift", c_void_p), ("post_act", c_int32),
-        ("y2", c_void_p), ("y2_pitch", c_int64),
+        ("y2", c_void_p), ("y2_pitch", c_int64), ("post_stride", c_int64),
     ]
 
 
@@ -166,6 +166,8 @@ _SIGNATURES = {
     "td_upconv2x_nhwc": (c_int, [POINTER(TdConvDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "td_attention": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int64, c_int64, c_int64, c_int64, c_float, c_int,
                              c_void_p]),
+    "td_attention_batched": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int64, c_int64, c_int64, c_int64,
+                                     c_int64, c_int64, c_int64, c_int64, c_float, c_int, c_void_p]),
     "td_nchw_to_nhwc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int64, c_int64, c_int64, c_int, c_int, c_void_p]),
     "td_nhwc_to_nchw_region": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int64, c_int, c_int64, c_int64, c_int64, c_int64,
                                        c_int, c_void_p]),
@@ -174,6 +176,10 @@ _SIGNATURES = {
     "td_gn_stats_nhwc": (c_int, [c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
     "td_gn_apply_nhwc": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_int,
                                  c_void_p]),
+    "td_gn_stats_nhwc_batched_workspace_bytes": (c_int64, [c_int, c_int64, c_int, c_int]),
+    "td_gn_stats_nhwc_batched": (c_int, [c_void_p, c_int, c_int64, c_int, c_int, c_int, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
+    "td_gn_apply_nhwc_batched": (c_int, [c_void_p, c_void_p, c_int, c_int64, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                         c_float, c_int, c_void_p]),
     "td_softmax_rows": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int64, c_int, c_void_p]),
     "td_blend_mixture": (c_int, [POINTER(TdGrid), POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_int,
                                  c_void_p, c_void_p, c_void_p, c_uint32, c_void_p]),

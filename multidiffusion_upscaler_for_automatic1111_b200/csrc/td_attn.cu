@@ -21,7 +21,9 @@
 //       - keys past T are masked with -inf, then the running max / sum update and the O rescale;
 //       - P (rounded to fp16 / bf16) goes straight from the S registers into the A operand of
 //         O[:, out_w] += P V[:, out_w] (wgmma with A in registers, V read MN-major from the same swizzled boxes);
-//   * the epilogue divides by the row sum and stores O from the registers, rows past T clipped; offsets are 64-bit.
+//   * the epilogue divides by the row sum and stores O from the registers, rows past T clipped; offsets are 64-bit;
+//   * a batch of images is one launch: blockIdx.z is the image, the operands are 3-D tensor maps {C, T, images}, so an
+//     image's CTAs load, compute and store exactly what its one-image launch does.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -54,12 +56,13 @@ struct AttnParams {
     int key_blocks;       // ceil(T / 64)
     float scale_log2;     // alpha * log2(e): the softmax runs on exp2
     long long o_pitch;
+    long long o_img;      // elements between images of O
 };
 
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
+__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map, int c0, int c1, int c2, uint64_t* bar) {
     asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-        ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(smem_u32(bar)) : "memory");
+        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
+        ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(c2), "r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void attn_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
@@ -93,6 +96,7 @@ attn_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ C
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int q0 = blockIdx.x * kAttnRows;
     const int obeg = blockIdx.y * 2 * NO;      // first output chunk of this CTA
+    const int img = blockIdx.z;
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < p.stages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }   // one arrive per consumer warpgroup
@@ -109,7 +113,7 @@ attn_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ C
             asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_k)) : "memory");
             asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_v)) : "memory");
             mbar_arrive_expect_tx(&q_bar, stage_bytes);
-            for (int c = 0; c < 2 * NC; ++c) tma_load_2d(sq + (uint32_t)(c * kAttnChunkBytes), &map_q, c * 64, q0, &q_bar);
+            for (int c = 0; c < 2 * NC; ++c) tma_load_3d(sq + (uint32_t)(c * kAttnChunkBytes), &map_q, c * 64, q0, img, &q_bar);
             int stage = 0; uint32_t phase = 0;
             for (int j = 0; j < p.key_blocks; ++j)
                 for (int kv = 0; kv < 2; ++kv) {
@@ -117,11 +121,11 @@ attn_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ C
                     const uint32_t sa = ring + (uint32_t)stage * stage_bytes;
                     if (kv == 0) {
                         mbar_arrive_expect_tx(&full_bar[stage], stage_bytes);
-                        for (int c = 0; c < 2 * NC; ++c) tma_load_2d(sa + (uint32_t)(c * kAttnChunkBytes), &map_k, c * 64, j * kAttnRows, &full_bar[stage]);
+                        for (int c = 0; c < 2 * NC; ++c) tma_load_3d(sa + (uint32_t)(c * kAttnChunkBytes), &map_k, c * 64, j * kAttnRows, img, &full_bar[stage]);
                     } else {                       // only this CTA's slice of V
                         mbar_arrive_expect_tx(&full_bar[stage], (uint32_t)(2 * NO * kAttnChunkBytes));
                         for (int c = 0; c < 2 * NO; ++c)
-                            tma_load_2d(sa + (uint32_t)(c * kAttnChunkBytes), &map_v, (obeg + c) * 64, j * kAttnRows, &full_bar[stage]);
+                            tma_load_3d(sa + (uint32_t)(c * kAttnChunkBytes), &map_v, (obeg + c) * 64, j * kAttnRows, img, &full_bar[stage]);
                     }
                     if (++stage == p.stages) { stage = 0; phase ^= 1u; }
                 }
@@ -247,6 +251,7 @@ attn_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ C
     l1 += __shfl_xor_sync(0xffffffffu, l1, 1); l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
     const float inv0 = 1.0f / l0, inv1 = 1.0f / l1;
     const long long row0 = (long long)q0 + r;
+    o += (long long)img * p.o_img;
 #pragma unroll
     for (int cc = 0; cc < NO; ++cc) {
 #pragma unroll
@@ -262,17 +267,17 @@ attn_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ C
     }
 }
 
-int encode_operand(CUtensorMap* m, const void* base, int is_bf16, int T, int C, int64_t pitch, const char* what) {
-    const uint64_t dims[2] = {(uint64_t)C, (uint64_t)T};
-    const uint64_t str[1] = {(uint64_t)pitch * 2};
-    const uint32_t box[2] = {64, (uint32_t)kAttnRows};
-    const uint32_t es[2] = {1, 1};
-    return td_encode_map(m, base, is_bf16, 2, dims, str, box, es, true, what);
+int encode_operand(CUtensorMap* m, const void* base, int is_bf16, int N, int T, int C, int64_t pitch, int64_t img_stride, const char* what) {
+    const uint64_t dims[3] = {(uint64_t)C, (uint64_t)T, (uint64_t)N};
+    const uint64_t str[2] = {(uint64_t)pitch * 2, (uint64_t)img_stride * 2};
+    const uint32_t box[3] = {64, (uint32_t)kAttnRows, 1};
+    const uint32_t es[3] = {1, 1, 1};
+    return td_encode_map(m, base, is_bf16, 3, dims, str, box, es, true, what);
 }
 
 // one launch of the <BF16, NC> form: shared-memory opt-in and the ring depth
 template <bool BF16, int NC, int NO>
-int attn_launch(const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv, AttnParams p, uint16_t* o, cudaStream_t st) {
+int attn_launch(const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv, AttnParams p, int images, uint16_t* o, cudaStream_t st) {
     const DeviceProps dev = device_props();
     cudaFuncAttributes fa;
     if (!dev.ok || cudaFuncGetAttributes(&fa, attn_kernel<BF16, NC, NO>) != cudaSuccess) {
@@ -293,33 +298,39 @@ int attn_launch(const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap&
         td_set_error("td_attention: the kernel (%d registers, %d bytes of shared memory) does not fit on an SM", fa.numRegs, smem);
         return TD_ERR_UNSUPPORTED;
     }
-    attn_kernel<BF16, NC, NO><<<dim3(p.key_blocks, NC / NO), kAttnThreads, smem, st>>>(mq, mk, mv, p, o);
+    attn_kernel<BF16, NC, NO><<<dim3(p.key_blocks, NC / NO, images), kAttnThreads, smem, st>>>(mq, mk, mv, p, o);
     return launch_status("td_attention");
 }
 
 template <bool BF16>
-int attn_dispatch(const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv, const AttnParams& p, uint16_t* o, cudaStream_t st) {
+int attn_dispatch(const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv, const AttnParams& p, int images, uint16_t* o,
+                  cudaStream_t st) {
     switch ((p.C + 127) / 128) {
-        case 1: return attn_launch<BF16, 1, 1>(mq, mk, mv, p, o, st);
-        case 2: return attn_launch<BF16, 2, 2>(mq, mk, mv, p, o, st);
-        case 3: return attn_launch<BF16, 3, 3>(mq, mk, mv, p, o, st);
+        case 1: return attn_launch<BF16, 1, 1>(mq, mk, mv, p, images, o, st);
+        case 2: return attn_launch<BF16, 2, 2>(mq, mk, mv, p, images, o, st);
+        case 3: return attn_launch<BF16, 3, 3>(mq, mk, mv, p, images, o, st);
         // C > 384: O in two 256-channel slices (64 accumulators per thread, not 128: the kernel has 168 registers)
-        default: return attn_launch<BF16, 4, 2>(mq, mk, mv, p, o, st);
+        default: return attn_launch<BF16, 4, 2>(mq, mk, mv, p, images, o, st);
     }
 }
 
-}  // namespace
-
-extern "C" int td_attention(const void* q, const void* k, const void* v, void* o, int T, int C, int64_t q_pitch, int64_t k_pitch,
-                            int64_t v_pitch, int64_t o_pitch, float alpha, int dtype, void* stream) {
-    if (q == nullptr || k == nullptr || v == nullptr || o == nullptr) { td_set_error("td_attention: null argument"); return TD_ERR_INVALID_ARG; }
-    if (dtype != TD_F16 && dtype != TD_BF16) { td_set_error("td_attention: dtype must be fp16 or bf16"); return TD_ERR_UNSUPPORTED; }
-    if (T <= 0 || C <= 0) { td_set_error("td_attention: non-positive size"); return TD_ERR_INVALID_ARG; }
-    if (C % 64 != 0 || C > 64 * kAttnMaxChunks) { td_set_error("td_attention: C (%d) must be a multiple of 64 and <= 512", C); return TD_ERR_UNSUPPORTED; }
+int attn_run(const char* what, const void* q, const void* k, const void* v, void* o, int N, int T, int C, int64_t q_pitch, int64_t k_pitch,
+             int64_t v_pitch, int64_t o_pitch, int64_t q_img, int64_t k_img, int64_t v_img, int64_t o_img, float alpha, int dtype, void* stream) {
+    if (q == nullptr || k == nullptr || v == nullptr || o == nullptr) { td_set_error("%s: null argument", what); return TD_ERR_INVALID_ARG; }
+    if (dtype != TD_F16 && dtype != TD_BF16) { td_set_error("%s: dtype must be fp16 or bf16", what); return TD_ERR_UNSUPPORTED; }
+    if (T <= 0 || C <= 0 || N <= 0 || N > 65535) { td_set_error("%s: non-positive size or more than 65535 images", what); return TD_ERR_INVALID_ARG; }
+    if (C % 64 != 0 || C > 64 * kAttnMaxChunks) { td_set_error("%s: C (%d) must be a multiple of 64 and <= 512", what, C); return TD_ERR_UNSUPPORTED; }
     for (int64_t pitch : {q_pitch, k_pitch, v_pitch, o_pitch})
-        if (pitch < C || pitch % 8 != 0) { td_set_error("td_attention: pitches must cover C and be multiples of 8 elements (16 bytes)"); return TD_ERR_INVALID_ARG; }
+        if (pitch < C || pitch % 8 != 0) { td_set_error("%s: pitches must cover C and be multiples of 8 elements (16 bytes)", what); return TD_ERR_INVALID_ARG; }
+    // an image holds its T rows: the operands' images may not overlap (o's would race), and each starts 16-byte aligned
+    const int64_t pitches[4] = {q_pitch, k_pitch, v_pitch, o_pitch}, imgs[4] = {q_img, k_img, v_img, o_img};
+    for (int i = 0; i < 4; ++i)
+        if (imgs[i] < (int64_t)T * pitches[i] || imgs[i] % 8 != 0) {
+            td_set_error("%s: image strides must be >= T * pitch and multiples of 8 elements (16 bytes)", what);
+            return TD_ERR_INVALID_ARG;
+        }
     for (const void* ptr : {q, k, v, (const void*)o})
-        if (!aligned16(ptr)) { td_set_error("td_attention: tensors must be 16-byte aligned"); return TD_ERR_INVALID_ARG; }
+        if (!aligned16(ptr)) { td_set_error("%s: tensors must be 16-byte aligned", what); return TD_ERR_INVALID_ARG; }
 
     AttnParams p;
     std::memset(&p, 0, sizeof(p));
@@ -328,13 +339,31 @@ extern "C" int td_attention(const void* q, const void* k, const void* v, void* o
     p.key_blocks = (T + kAttnRows - 1) / kAttnRows;
     p.scale_log2 = alpha * 1.4426950408889634f;
     p.o_pitch = o_pitch;
+    p.o_img = o_img;
     const bool bf16 = dtype == TD_BF16;
     alignas(64) CUtensorMap mq, mk, mv;
-    int rc = encode_operand(&mq, q, bf16, T, C, q_pitch, "q");
-    if (rc == TD_OK) rc = encode_operand(&mk, k, bf16, T, C, k_pitch, "k");
-    if (rc == TD_OK) rc = encode_operand(&mv, v, bf16, T, C, v_pitch, "v");
+    int rc = encode_operand(&mq, q, bf16, N, T, C, q_pitch, q_img, "q");
+    if (rc == TD_OK) rc = encode_operand(&mk, k, bf16, N, T, C, k_pitch, k_img, "k");
+    if (rc == TD_OK) rc = encode_operand(&mv, v, bf16, N, T, C, v_pitch, v_img, "v");
     if (rc != TD_OK) return rc;
     uint16_t* out = static_cast<uint16_t*>(o);
     cudaStream_t st = (cudaStream_t)stream;
-    return bf16 ? attn_dispatch<true>(mq, mk, mv, p, out, st) : attn_dispatch<false>(mq, mk, mv, p, out, st);
+    return bf16 ? attn_dispatch<true>(mq, mk, mv, p, N, out, st) : attn_dispatch<false>(mq, mk, mv, p, N, out, st);
+}
+
+}  // namespace
+
+extern "C" int td_attention(const void* q, const void* k, const void* v, void* o, int T, int C, int64_t q_pitch, int64_t k_pitch,
+                            int64_t v_pitch, int64_t o_pitch, float alpha, int dtype, void* stream) {
+    // one image: the image strides only have to be legal for the tensor maps
+    const int64_t t = T > 0 ? T : 0;
+    return attn_run("td_attention", q, k, v, o, 1, T, C, q_pitch, k_pitch, v_pitch, o_pitch, t * q_pitch, t * k_pitch, t * v_pitch,
+                    t * o_pitch, alpha, dtype, stream);
+}
+
+extern "C" int td_attention_batched(const void* q, const void* k, const void* v, void* o, int N, int T, int C, int64_t q_pitch,
+                                    int64_t k_pitch, int64_t v_pitch, int64_t o_pitch, int64_t q_img_stride, int64_t k_img_stride,
+                                    int64_t v_img_stride, int64_t o_img_stride, float alpha, int dtype, void* stream) {
+    return attn_run("td_attention_batched", q, k, v, o, N, T, C, q_pitch, k_pitch, v_pitch, o_pitch, q_img_stride, k_img_stride,
+                    v_img_stride, o_img_stride, alpha, dtype, stream);
 }

@@ -62,10 +62,11 @@ struct ConvParams {
     int bias_per_row;          // bias indexed by output pixel (GEMM row) instead of channel
     int post_act;              // with post_scale / post_shift: 1 = SiLU after the per-channel affine
     float alpha;
-    int up2;                   // 1: nearest-2x upsample folded into the 3x3 convolution -- four 2x2 convolutions of the LOW-resolution
-                               // image, one per output parity (py, px) = "image" index (py * 2 + px); weights [16 taps, Cout, Cin];
-                               // tile pixel (x, y) of parity (py, px) is output pixel (2 x + px, 2 y + py)
+    int up2;                   // 1: nearest-2x upsample folded into the 3x3 convolution -- four 2x2 convolutions of each LOW-resolution
+                               // image, one per output parity (py, px): "image" index 4 n + (py * 2 + px); weights [16 taps, Cout, Cin];
+                               // tile pixel (x, y) of parity (py, px) is output pixel (2 x + px, 2 y + py) of image n
     long long y_pitch, y2_pitch, res_pitch;   // elements between pixels
+    long long post_stride;     // elements between the images' post_scale / post_shift vectors (0: one vector for all)
 };
 
 __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map, int c0, int c1, int c2, int c3, uint64_t* bar) {
@@ -146,8 +147,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
             for (int g = blockIdx.x; g < p.num_tiles; g += gridDim.x) {
                 const TileCoord c = decode_tile(p, g);
                 // up2: output parity (py, px) shifts the 2x2 window by one low-resolution pixel and selects its 4 folded taps
-                const int par = p.up2 ? c.img : 0;
-                const int img = p.up2 ? 0 : c.img;
+                const int par = p.up2 ? (c.img & 3) : 0;
+                const int img = p.up2 ? (c.img >> 2) : c.img;
                 const int x0 = c.px * p.BW * p.stride - p.pad_left + (par & 1);
                 const int y0 = c.py * p.BH * p.stride - p.pad_top + (par >> 1);
                 int tap = par * 4;
@@ -206,9 +207,12 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
             const int ox = c.px * p.BW + lx, oy = c.py * p.BH + ly;
             if (ox >= p.OW || oy >= p.OH || c.img >= p.NI) continue;
             const long long pix = ((long long)c.img * p.OH + oy) * p.OW + ox;
-            // output pixel: the parity view of the 2x-upsampled image when up2 (one image, N = 1), else the tile pixel
-            const long long opix = p.up2 ? (long long)(2 * oy + (c.img >> 1)) * (2 * p.OW) + 2 * ox + (c.img & 1) : pix;
+            // output pixel: the parity view of the 2x-upsampled image n = img / 4 when up2, else the tile pixel
+            const int par = c.img & 3;
+            const long long opix = p.up2 ? ((long long)(c.img >> 2) * 2 * p.OH + 2 * oy + (par >> 1)) * (2 * p.OW) + 2 * ox + (par & 1) : pix;
             const float bb = (bias != nullptr && p.bias_per_row) ? __ldg(bias + pix) : 0.0f;
+            // a tile lies in one image (the walk is per image), so its rows share the image's constants
+            const long long post_off = (long long)(p.up2 ? (c.img >> 2) : c.img) * p.post_stride;
 #pragma unroll
             for (int j = 0; j < BN / 8; ++j) {
                 const int co = c.nb * BN + 8 * j + cq;
@@ -228,8 +232,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
                 if (post_scale != nullptr) {
                     // the GroupNorm (+ SiLU) that follows this convolution, statistics frozen (fast mode):
                     // y = act(v * scale[c] + shift[c]) on the fp32 accumulator, before the one rounding to fp16
-                    v0 = __fmaf_rn(v0, __ldg(post_scale + co), __ldg(post_shift + co));
-                    if (two) v1 = __fmaf_rn(v1, __ldg(post_scale + co + 1), __ldg(post_shift + co + 1));
+                    v0 = __fmaf_rn(v0, __ldg(post_scale + post_off + co), __ldg(post_shift + post_off + co));
+                    if (two) v1 = __fmaf_rn(v1, __ldg(post_scale + post_off + co + 1), __ldg(post_shift + post_off + co + 1));
                     if (p.post_act) {
                         v0 = __fdividef(v0, 1.0f + __expf(-v0));
                         v1 = __fdividef(v1, 1.0f + __expf(-v1));
@@ -278,21 +282,22 @@ int td_encode_map(CUtensorMap* out, const void* base, int is_bf16, int rank, con
 }
 
 namespace {
-// up2 = 1: `d` describes nearest-2x upsample + 3x3 / pad 1 (OH = 2 H, OW = 2 W) of ONE image; `w` holds the 16 folded taps.
-int conv_run(const td_conv_desc* d, const void* x, const void* w, const float* bias, const void* residual, void* y, void* stream, int up2,
-             size_t y2_off = 0) {
+// up2 = 1: `d` describes nearest-2x upsample + 3x3 / pad 1 (OH = 2 H, OW = 2 W) of N images; `w` holds the 16 folded taps.
+int conv_run(const td_conv_desc* d, const void* x, const void* w, const float* bias, const void* residual, void* y, void* stream, int up2) {
     if (d == nullptr || x == nullptr || w == nullptr || y == nullptr) { td_set_error("td_conv2d_nhwc: null argument"); return TD_ERR_INVALID_ARG; }
     if (d->dtype != TD_F16 && d->dtype != TD_BF16) { td_set_error("td_conv2d_nhwc: dtype must be fp16 or bf16"); return TD_ERR_UNSUPPORTED; }
     if (d->N <= 0 || d->H <= 0 || d->W <= 0 || d->OH <= 0 || d->OW <= 0 || d->Cin <= 0 || d->Cout <= 0) { td_set_error("td_conv2d_nhwc: non-positive size"); return TD_ERR_INVALID_ARG; }
     if (d->Cin % 8 != 0) { td_set_error("td_conv2d_nhwc: Cin (%d) must be a multiple of 8", d->Cin); return TD_ERR_UNSUPPORTED; }
     if ((d->kh != 1 && d->kh != 3) || d->kh != d->kw || (d->stride != 1 && d->stride != 2)) { td_set_error("td_conv2d_nhwc: only 1x1 / 3x3, stride 1 / 2"); return TD_ERR_UNSUPPORTED; }
-    if (up2 && (d->kh != 3 || d->stride != 1 || d->pad_top != 1 || d->pad_left != 1 || d->OH != 2 * d->H || d->OW != 2 * d->W || d->N != 1 ||
+    if (up2 && (d->kh != 3 || d->stride != 1 || d->pad_top != 1 || d->pad_left != 1 || d->OH != 2 * d->H || d->OW != 2 * d->W ||
                 residual != nullptr || d->bias_per_row)) {
         td_set_error("td_upconv2x_nhwc: describes upsample(2x nearest) + 3x3 / stride 1 / pad 1 (OH = 2H, OW = 2W), no residual, bias per channel");
         return TD_ERR_INVALID_ARG;
     }
-    // grid of output pixels the tiles walk: the low-resolution image (once per output parity) when the upsample is folded
-    const int gOW = up2 ? d->W : d->OW, gOH = up2 ? d->H : d->OH, gN = up2 ? 4 : d->N;
+    // grid of output pixels the tiles walk: the low-resolution images (once per output parity) when the upsample is folded
+    const int gOW = up2 ? d->W : d->OW, gOH = up2 ? d->H : d->OH;
+    const long long gN = up2 ? 4LL * d->N : d->N;
+    if (gN > 0x3fffffffLL) { td_set_error("td_conv2d_nhwc: too many images"); return TD_ERR_UNSUPPORTED; }
     if (d->x_pitch < d->Cin || d->x_pitch % 8 != 0 || d->y_pitch < d->Cout || d->y_pitch % 8 != 0 || d->w_pitch < d->Cin || d->w_pitch % 8 != 0 ||
         (residual != nullptr && (d->res_pitch < d->Cout || d->res_pitch % 8 != 0))) {
         td_set_error("td_conv2d_nhwc: pitches must cover the channels and be multiples of 8 elements (16 bytes)");
@@ -306,6 +311,11 @@ int conv_run(const td_conv_desc* d, const void* x, const void* w, const float* b
         return TD_ERR_INVALID_ARG;
     }
     if ((d->post_scale == nullptr) != (d->post_shift == nullptr)) { td_set_error("td_conv2d_nhwc: post_scale and post_shift come together"); return TD_ERR_INVALID_ARG; }
+    if (d->post_stride != 0 && (d->post_scale == nullptr || d->post_stride < d->Cout || d->post_stride % 4 != 0 || d->bias_per_row)) {
+        td_set_error("td_conv2d_nhwc: post_stride (%lld) needs post_scale / post_shift, >= Cout and a multiple of 4 (16 bytes), and a "
+                     "bias per channel", (long long)d->post_stride);
+        return TD_ERR_INVALID_ARG;
+    }
     const DeviceProps dev = device_props();
     const int smem_limit = conv_dyn_smem_limit(dev);
     if (smem_limit < 0) { td_set_error("td_conv2d_nhwc: device query failed"); return TD_ERR_CUDA; }
@@ -313,7 +323,7 @@ int conv_run(const td_conv_desc* d, const void* x, const void* w, const float* b
     ConvParams p;
     std::memset(&p, 0, sizeof(p));
     p.taps_x = up2 ? 2 : d->kw; p.taps_y = up2 ? 2 : d->kh; p.stride = d->stride; p.pad_left = d->pad_left; p.pad_top = d->pad_top;
-    p.OW = gOW; p.OH = gOH; p.NI = gN; p.up2 = up2;
+    p.OW = gOW; p.OH = gOH; p.NI = (int)gN; p.up2 = up2;
     p.Cin_chunks = (d->Cin + 63) / 64;   // a partial last chunk is zero-filled by the TMA unit on BOTH operands
     p.Cout = d->Cout;
     int bn = 256;
@@ -335,6 +345,7 @@ int conv_run(const td_conv_desc* d, const void* x, const void* w, const float* b
     p.y_pitch = d->y_pitch;
     p.y2_pitch = d->y2 != nullptr ? d->y2_pitch : 0;
     p.res_pitch = residual != nullptr ? d->res_pitch : 0;
+    p.post_stride = d->post_stride;
     const int stage_bytes = kConvStageA + bn * 128;
     p.stages = std::min(kConvMaxStages, (smem_limit - 1024) / stage_bytes);
     if (p.stages < 2) { td_set_error("td_conv2d_nhwc: not enough shared memory"); return TD_ERR_UNSUPPORTED; }
@@ -358,7 +369,7 @@ int conv_run(const td_conv_desc* d, const void* x, const void* w, const float* b
         if (rc != TD_OK) return rc;
     }
     uint16_t* yo = static_cast<uint16_t*>(y);
-    uint16_t* y2o = d->y2 != nullptr ? static_cast<uint16_t*>(d->y2) + (up2 ? y2_off : 0) : nullptr;
+    uint16_t* y2o = static_cast<uint16_t*>(d->y2);
     const int grid = std::min(p.num_tiles, dev.sms);
     const uint16_t* res = static_cast<const uint16_t*>(residual);
     cudaStream_t st = (cudaStream_t)stream;
@@ -389,14 +400,6 @@ extern "C" int td_conv2d_nhwc(const td_conv_desc* d, const void* x, const void* 
 }
 
 extern "C" int td_upconv2x_nhwc(const td_conv_desc* d, const void* x, const void* w16, const float* bias, void* y, void* stream) {
-    if (d == nullptr || x == nullptr || y == nullptr) { td_set_error("td_upconv2x_nhwc: null argument"); return TD_ERR_INVALID_ARG; }
-    td_conv_desc one = *d;
-    one.N = 1;
-    for (int n = 0; n < d->N; ++n) {
-        const uint16_t* xn = static_cast<const uint16_t*>(x) + (size_t)n * d->H * d->W * d->x_pitch;
-        uint16_t* yn = static_cast<uint16_t*>(y) + (size_t)n * d->OH * d->OW * d->y_pitch;
-        const int rc = conv_run(&one, xn, w16, bias, nullptr, yn, stream, 1, (size_t)n * d->OH * d->OW * (size_t)d->y2_pitch);
-        if (rc != TD_OK) return rc;
-    }
-    return TD_OK;
+    // all images in one launch: image n's tiles are "images" 4 n .. 4 n + 3 of the walk, the same tiles its own launch walks
+    return conv_run(d, x, w16, bias, nullptr, y, stream, 1);
 }

@@ -7,6 +7,7 @@
 //                          'upsample', tilevae.py:163)
 //   td_gn_stats_nhwc       get_var_mean (tilevae.py:207-215) on channels-last data: ONE read
 //   td_gn_apply_nhwc       custom_group_norm + SiLU (tilevae.py:218-245, :102-104): one read + one write
+//                          (the *_batched entries: N images in one launch, each on the grid of its one-image call)
 //   td_softmax_rows        softmax over the keys of the VAE attention (tile_utils/attn.py:58-60)
 //
 // All HBM-bound: 128-bit accesses along the channel dimension, per-thread constants hoisted out of the pixel loop,
@@ -137,10 +138,11 @@ upsample2x_nhwc_kernel(const T* __restrict__ x, T* __restrict__ y, int H, int W,
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// GroupNorm statistics, channels-last.  x: [P, C] (one image), groups of cpg = C / groups adjacent channels.
+// GroupNorm statistics, channels-last.  x: [P, C] per image, groups of cpg = C / groups adjacent channels.
 // A thread owns one 8-channel vector position and walks pixels; its two 4-channel halves are accumulated on data
 // shifted by the first value seen, turned into (n, mean, M2) and merged per group with Chan's update:
-// thread -> CTA (shared memory) -> finaliser kernel.
+// thread -> CTA (shared memory) -> finaliser kernel.  blockIdx.y is the image: each image runs the grid, the partials
+// and the merge order of its one-image launch, so its statistics are the same bits.
 // ---------------------------------------------------------------------------------------------------------------
 struct Mom { float n, mean, m2; };
 __device__ __forceinline__ Mom mom_merge(const Mom& a, const Mom& b) {
@@ -158,6 +160,8 @@ template <typename T>
 __global__ void __launch_bounds__(kNhwcThreads)
 gn_stats_nhwc_partial_kernel(const T* __restrict__ x, long long P, int C, int groups, float* __restrict__ ws) {
     __shared__ Mom s_m[kNhwcThreads * 2];
+    x += (long long)blockIdx.y * P * C;
+    ws += (long long)blockIdx.y * gridDim.x * groups * 3;
     const int cv = C / 8, cpg = C / groups;
     const int ppi = kNhwcThreads / cv;                 // pixels per CTA iteration
     const int v = threadIdx.x % cv, pl = threadIdx.x / cv;
@@ -199,12 +203,15 @@ gn_stats_nhwc_partial_kernel(const T* __restrict__ x, long long P, int C, int gr
     }
 }
 
-// One warp per group: lanes stride over the per-CTA partials, then merge by shuffles (a single thread walking ~600
-// partials with a dependent divide each took 0.3 ms -- longer than the streaming pass it finishes).
+// One warp per (image, group): lanes stride over the per-CTA partials, then merge by shuffles (a single thread walking
+// ~600 partials with a dependent divide each took 0.3 ms -- longer than the streaming pass it finishes).
 __global__ void __launch_bounds__(256)
-gn_stats_nhwc_final_kernel(const float* __restrict__ ws, int nblocks, int groups, float* __restrict__ mean, float* __restrict__ var) {
-    const int g = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
-    if (g >= groups) return;
+gn_stats_nhwc_final_kernel(const float* __restrict__ ws, int nblocks, int groups, int images, float* __restrict__ mean,
+                           float* __restrict__ var) {
+    const int gi = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+    if (gi >= images * groups) return;
+    const int img = gi / groups, g = gi - img * groups;
+    ws += (long long)img * nblocks * groups * 3;
     Mom r{0.f, 0.f, 0.f};
     for (int b = lane; b < nblocks; b += 32) {
         const float* o = ws + ((long long)b * groups + g) * 3;
@@ -219,18 +226,23 @@ gn_stats_nhwc_final_kernel(const float* __restrict__ ws, int nblocks, int groups
         r = mom_merge(r, t);
     }
     if (lane == 0) {
-        mean[g] = r.mean;
-        var[g] = r.n > 0.f ? r.m2 / r.n : 0.f;     // biased (torch.var_mean(unbiased=False))
+        mean[gi] = r.mean;
+        var[gi] = r.n > 0.f ? r.m2 / r.n : 0.f;    // biased (torch.var_mean(unbiased=False))
     }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
 // GroupNorm apply (+ SiLU), channels-last: y = act((x - mean[g]) * rsqrt(var[g] + eps) * gamma[c] + beta[c])
+// blockIdx.y is the image; mean / var are [images, groups].
 // ---------------------------------------------------------------------------------------------------------------
 template <typename T>
 __global__ void __launch_bounds__(kNhwcThreads)
 gn_apply_nhwc_kernel(const T* __restrict__ x, T* __restrict__ y, long long P, int C, int groups, const float* __restrict__ mean,
                      const float* __restrict__ var, const float* __restrict__ gamma, const float* __restrict__ beta, float eps, int act) {
+    x += (long long)blockIdx.y * P * C;
+    y += (long long)blockIdx.y * P * C;
+    mean += blockIdx.y * groups;
+    var += blockIdx.y * groups;
     const int cv = C / 8, cpg = C / groups;
     const long long total = P * cv;
     const long long i0 = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -369,6 +381,54 @@ extern "C" int td_upsample2x_nhwc(const void* x, void* y, int N, int H, int W, i
     return launch_status("td_upsample2x_nhwc");
 }
 
+namespace {
+
+// The one-image entries are the batched ones at N = 1: one plan, so a batched image gets its one-image bits.
+int gn_stats_grid(int64_t pixels, int C) {
+    const int ppi = kNhwcThreads / (C / 8);
+    return (int)std::max<int64_t>(1, std::min<int64_t>((pixels + ppi - 1) / ppi, (int64_t)nhwc_sms() * 4));
+}
+
+int gn_stats_run(const char* what, const void* x, int N, int64_t pixels, int C, int groups, int dtype, void* workspace,
+                 int64_t workspace_bytes, float* mean, float* var, void* stream) {
+    if (x == nullptr || workspace == nullptr || mean == nullptr || var == nullptr || pixels <= 0 || N <= 0 || N > 65535 || !half_like(dtype)) {
+        td_set_error("%s: bad arguments", what);
+        return TD_ERR_INVALID_ARG;
+    }
+    if (groups <= 0 || groups > 64 || C <= 0 || C % groups != 0 || (C / groups) % 4 != 0 || C % 8 != 0 || kNhwcThreads % (C / 8) != 0) {
+        td_set_error("%s: unsupported channel layout C=%d groups=%d (need C/groups %% 4 == 0 and C/8 dividing 256)", what, C, groups);
+        return TD_ERR_UNSUPPORTED;
+    }
+    const int grid = gn_stats_grid(pixels, C);
+    if ((int64_t)N * grid * groups * 3 * (int64_t)sizeof(float) > workspace_bytes) { td_set_error("%s: workspace too small", what); return TD_ERR_CAPACITY; }
+    cudaStream_t st = (cudaStream_t)stream;
+    const dim3 g2(grid, N);
+    if (dtype == TD_F16) gn_stats_nhwc_partial_kernel<__half><<<g2, kNhwcThreads, 0, st>>>((const __half*)x, pixels, C, groups, (float*)workspace);
+    else gn_stats_nhwc_partial_kernel<__nv_bfloat16><<<g2, kNhwcThreads, 0, st>>>((const __nv_bfloat16*)x, pixels, C, groups, (float*)workspace);
+    gn_stats_nhwc_final_kernel<<<(N * groups * 32 + 255) / 256, 256, 0, st>>>((const float*)workspace, grid, groups, N, mean, var);
+    return launch_status(what);
+}
+
+int gn_apply_run(const char* what, const void* x, void* y, int N, int64_t pixels, int C, int groups, int dtype, const float* mean,
+                 const float* var, const float* gamma, const float* beta, float eps, int act, void* stream) {
+    if (x == nullptr || y == nullptr || mean == nullptr || var == nullptr || pixels <= 0 || N <= 0 || N > 65535 || !half_like(dtype)) {
+        td_set_error("%s: bad arguments", what);
+        return TD_ERR_INVALID_ARG;
+    }
+    if (groups <= 0 || C <= 0 || C % groups != 0 || C % 8 != 0 || kNhwcThreads % (C / 8) != 0) {
+        td_set_error("%s: unsupported channel layout C=%d groups=%d", what, C, groups);
+        return TD_ERR_UNSUPPORTED;
+    }
+    const long long total = (long long)pixels * (C / 8);
+    const dim3 grid(grid_for(total, kNhwcThreads * 4), N);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (dtype == TD_F16) gn_apply_nhwc_kernel<__half><<<grid, kNhwcThreads, 0, st>>>((const __half*)x, (__half*)y, pixels, C, groups, mean, var, gamma, beta, eps, act);
+    else gn_apply_nhwc_kernel<__nv_bfloat16><<<grid, kNhwcThreads, 0, st>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)y, pixels, C, groups, mean, var, gamma, beta, eps, act);
+    return launch_status(what);
+}
+
+}  // namespace
+
 extern "C" int64_t td_gn_stats_nhwc_workspace_bytes(int64_t pixels, int C, int groups) {
     if (pixels <= 0 || C <= 0 || groups <= 0) return 0;
     return (int64_t)nhwc_sms() * 4 * groups * 3 * (int64_t)sizeof(float);
@@ -376,40 +436,32 @@ extern "C" int64_t td_gn_stats_nhwc_workspace_bytes(int64_t pixels, int C, int g
 
 extern "C" int td_gn_stats_nhwc(const void* x, int64_t pixels, int C, int groups, int dtype, void* workspace, int64_t workspace_bytes,
                                 float* mean, float* var, void* stream) {
-    if (x == nullptr || workspace == nullptr || mean == nullptr || var == nullptr || pixels <= 0 || !half_like(dtype)) {
-        td_set_error("td_gn_stats_nhwc: bad arguments");
-        return TD_ERR_INVALID_ARG;
-    }
-    if (groups <= 0 || groups > 64 || C % groups != 0 || (C / groups) % 4 != 0 || C % 8 != 0 || kNhwcThreads % (C / 8) != 0) {
-        td_set_error("td_gn_stats_nhwc: unsupported channel layout C=%d groups=%d (need C/groups %% 4 == 0 and C/8 dividing 256)", C, groups);
-        return TD_ERR_UNSUPPORTED;
-    }
-    const int ppi = kNhwcThreads / (C / 8);
-    int grid = (int)std::max<int64_t>(1, std::min<int64_t>((pixels + ppi - 1) / ppi, (int64_t)nhwc_sms() * 4));
-    if ((int64_t)grid * groups * 3 * (int64_t)sizeof(float) > workspace_bytes) { td_set_error("td_gn_stats_nhwc: workspace too small"); return TD_ERR_CAPACITY; }
-    cudaStream_t st = (cudaStream_t)stream;
-    if (dtype == TD_F16) gn_stats_nhwc_partial_kernel<__half><<<grid, kNhwcThreads, 0, st>>>((const __half*)x, pixels, C, groups, (float*)workspace);
-    else gn_stats_nhwc_partial_kernel<__nv_bfloat16><<<grid, kNhwcThreads, 0, st>>>((const __nv_bfloat16*)x, pixels, C, groups, (float*)workspace);
-    gn_stats_nhwc_final_kernel<<<(groups * 32 + 255) / 256, 256, 0, st>>>((const float*)workspace, grid, groups, mean, var);
-    return launch_status("td_gn_stats_nhwc");
+    return gn_stats_run("td_gn_stats_nhwc", x, 1, pixels, C, groups, dtype, workspace, workspace_bytes, mean, var, stream);
 }
 
 extern "C" int td_gn_apply_nhwc(const void* x, void* y, int64_t pixels, int C, int groups, int dtype, const float* mean, const float* var,
                                 const float* gamma, const float* beta, float eps, int act, void* stream) {
-    if (x == nullptr || y == nullptr || mean == nullptr || var == nullptr || pixels <= 0 || !half_like(dtype)) {
-        td_set_error("td_gn_apply_nhwc: bad arguments");
+    return gn_apply_run("td_gn_apply_nhwc", x, y, 1, pixels, C, groups, dtype, mean, var, gamma, beta, eps, act, stream);
+}
+
+extern "C" int64_t td_gn_stats_nhwc_batched_workspace_bytes(int N, int64_t pixels, int C, int groups) {
+    if (N <= 0 || pixels <= 0 || C <= 0 || groups <= 0) return 0;
+    return (int64_t)N * td_gn_stats_nhwc_workspace_bytes(pixels, C, groups);
+}
+
+extern "C" int td_gn_stats_nhwc_batched(const void* x, int N, int64_t pixels, int C, int groups, int dtype, void* workspace,
+                                        int64_t workspace_bytes, float* mean, float* var, void* stream) {
+    if (x != nullptr && !aligned16(x)) { td_set_error("td_gn_stats_nhwc_batched: x must be 16-byte aligned"); return TD_ERR_INVALID_ARG; }
+    return gn_stats_run("td_gn_stats_nhwc_batched", x, N, pixels, C, groups, dtype, workspace, workspace_bytes, mean, var, stream);
+}
+
+extern "C" int td_gn_apply_nhwc_batched(const void* x, void* y, int N, int64_t pixels, int C, int groups, int dtype, const float* mean,
+                                        const float* var, const float* gamma, const float* beta, float eps, int act, void* stream) {
+    if ((x != nullptr && !aligned16(x)) || (y != nullptr && !aligned16(y))) {
+        td_set_error("td_gn_apply_nhwc_batched: x and y must be 16-byte aligned");
         return TD_ERR_INVALID_ARG;
     }
-    if (groups <= 0 || C % groups != 0 || C % 8 != 0 || kNhwcThreads % (C / 8) != 0) {
-        td_set_error("td_gn_apply_nhwc: unsupported channel layout C=%d groups=%d", C, groups);
-        return TD_ERR_UNSUPPORTED;
-    }
-    const long long total = (long long)pixels * (C / 8);
-    const int grid = grid_for(total, kNhwcThreads * 4);
-    cudaStream_t st = (cudaStream_t)stream;
-    if (dtype == TD_F16) gn_apply_nhwc_kernel<__half><<<grid, kNhwcThreads, 0, st>>>((const __half*)x, (__half*)y, pixels, C, groups, mean, var, gamma, beta, eps, act);
-    else gn_apply_nhwc_kernel<__nv_bfloat16><<<grid, kNhwcThreads, 0, st>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)y, pixels, C, groups, mean, var, gamma, beta, eps, act);
-    return launch_status("td_gn_apply_nhwc");
+    return gn_apply_run("td_gn_apply_nhwc_batched", x, y, N, pixels, C, groups, dtype, mean, var, gamma, beta, eps, act, stream);
 }
 
 extern "C" int td_softmax_rows(const void* x, void* y, int rows, int cols, int64_t pitch, int dtype, void* stream) {

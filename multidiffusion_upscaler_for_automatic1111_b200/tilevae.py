@@ -232,19 +232,32 @@ class GroupNormParam:
         var, mean = get_var_mean(tile, NUM_GROUPS)
         self.add(var, mean, tile.shape[2] * tile.shape[3])
 
-    def summary(self, stat_len: Optional[int] = None, device=None):
-        """-> (mean, var) fp32 tensors, or None when no tile contributed anywhere."""
+    def summary(self, stat_len: Optional[int] = None, device=None, images: int = 1):
+        """-> (mean, var) fp32 tensors, or None when no tile contributed anywhere.
+
+        images > 1: each tile's statistics hold `images` images one after the other (a batched tensor-core pass) and
+        every image is merged on its own, with the operations and the all-reduce its one-image pass would run, so
+        its statistics are the same bits.  stat_len then counts all images."""
+        if images == 1:
+            return self._merge(self.var_list, self.mean_list, stat_len, device)
+        per = [self._merge([v.view(images, -1)[j] for v in self.var_list], [m.view(images, -1)[j] for m in self.mean_list],
+                           None if stat_len is None else int(stat_len) // images, device) for j in range(images)]
+        if any(p is None for p in per):
+            return None
+        return torch.cat([p[0] for p in per]), torch.cat([p[1] for p in per])
+
+    def _merge(self, var_list, mean_list, stat_len, device):
         if not self.sharded:
-            if not self.var_list:
+            if not var_list:
                 return None
-            var, mean = torch.vstack(self.var_list), torch.vstack(self.mean_list)
+            var, mean = torch.vstack(var_list), torch.vstack(mean_list)
             px = torch.tensor(self.pixel_list, dtype=torch.float32, device=var.device)
             px = (px / px.sum()).unsqueeze(1)
             return torch.sum(mean * px, dim=0), torch.sum(var * px, dim=0)
         import torch.distributed as dist
-        if self.var_list:
-            px = torch.tensor(self.pixel_list, dtype=torch.float32, device=self.var_list[0].device).unsqueeze(1)
-            packed = torch.cat([(torch.vstack(self.var_list) * px).sum(0), (torch.vstack(self.mean_list) * px).sum(0), px.sum().view(1)])
+        if var_list:
+            px = torch.tensor(self.pixel_list, dtype=torch.float32, device=var_list[0].device).unsqueeze(1)
+            packed = torch.cat([(torch.vstack(var_list) * px).sum(0), (torch.vstack(mean_list) * px).sum(0), px.sum().view(1)])
         else:
             packed = torch.zeros(2 * int(stat_len) + 1, dtype=torch.float32, device=device)
         dist.all_reduce(packed, group=self.group)
@@ -393,6 +406,14 @@ class _Parking:
 
 
 # --------------------------------------------------------------------------- the hook
+def pick_images_per_pass(n: int, fits: Callable[[int], bool]) -> int:
+    """The largest k <= n with fits(k) (k > 1 only: one image at a time is the schedule that always runs), else 1."""
+    for k in range(n, 1, -1):
+        if fits(k):
+            return k
+    return 1
+
+
 class VAEHook:
 
     def __init__(self, net, tile_size, is_decoder: bool, fast_decoder: bool, fast_encoder: bool, color_fix: bool, to_gpu: bool = False):
@@ -409,6 +430,11 @@ class VAEHook:
         # pinned host memory.  None: the free device memory at the start of the call, less the working reserve.
         self.max_resident_bytes: Optional[int] = None
         self.last_park_stats: Optional[dict] = None    # what the last call parked (see _run_tiles)
+        # Tensor-core backend: images of a batch that go through the tiles together, each with its own GroupNorm statistics,
+        # fast-mode estimate and color fix (bit-identical to one image at a time).  None: the largest count whose working set
+        # fits in GPU memory and whose tiles all stay resident under the parking budget (`_images_per_pass`); 1: one pass per
+        # image.  The count used is last_park_stats["images_per_pass"].
+        self.images_per_pass: Optional[int] = None
         # Seamless tiling: the latent / image is periodic along x (y).  The tiles are then cut around the circle and read
         # their halo from the opposite edge, so a wrapped decode of a seamless latent has no seam (td_vae_split_tiles' `wrap`).
         self.wrap_x: bool = False
@@ -488,32 +514,51 @@ class VAEHook:
         program = self._program
         backend = ve.pick_backend(program, device, dtype)
         self.backend_name = backend.name
-        per_image = isinstance(backend, ve.TensorCoreBackend)     # channels-last kernels take one image at a time
         est_in = fast_mode_estimator_input(z, tile_size) if self.fast_mode else None
 
         sharded = self._shard_world > 1
         mine = [i for i in range(len(in_bboxes)) if i % self._shard_world == self._shard_rank] if sharded else list(range(len(in_bboxes)))
+        my_in, my_out = [in_bboxes[i] for i in mine], [out_bboxes[i] for i in mine]
         out_c = [op for op in program.ops if isinstance(op, ve.Conv)][-1].module.out_channels
         oh, ow = (height * 8, width * 8) if is_decoder else (height // 8, width // 8)
         result = torch.zeros((N, out_c, oh, ow), dtype=dtype, device=device)   # zeros: a partial (interrupted) result reads 0 elsewhere
         # budget / reserve: bytes (None when no barrier); host_bytes: pinned host memory (its peak: buffers live until the
         # call ends); d2h / h2d_bytes: bytes copied each way; pin_s: seconds spent pinning; tiles_parked: {site: tiles}
+        # images_per_pass: images that went through the tiles together
         self.last_park_stats = {"budget": None, "reserve": None, "host_bytes": 0, "d2h_bytes": 0, "h2d_bytes": 0, "pin_s": 0.0,
                                 "tiles_parked": {}}
-        finished = 0
-        images = [slice(n, n + 1) for n in range(N)] if per_image else [slice(0, N)]
-        for img in images:
+        k = self._images_per_pass(program, backend, z, my_in) if isinstance(backend, ve.TensorCoreBackend) else N
+        self.last_park_stats["images_per_pass"] = k
+
+        def one_pass(img):
+            """Tiles finished by one pass over images `img`; None when the estimate of a batched pass met a NaN."""
             ex = ve.Executor(program, backend)
             if est_in is not None:
-                ex.estimate(backend.load(est_in[img]), self.color_fix)
-            finished += self._run_tiles(ex, backend, z[img], result[img], [in_bboxes[i] for i in mine], [out_bboxes[i] for i in mine])
+                if isinstance(backend, ve.TensorCoreBackend) and img.stop - img.start > 1:
+                    if not ex.estimate(backend.load(est_in[img]), self.color_fix, report=False):
+                        return None
+                else:
+                    ex.estimate(backend.load(est_in[img]), self.color_fix)
+            return self._run_tiles(ex, backend, z[img], result[img], my_in, my_out)
+
+        finished = 0
+        for start in range(0, N, k):
+            done = one_pass(slice(start, min(start + k, N)))
+            if done is None:
+                # an image whose estimate met a NaN runs without frozen statistics while the others keep theirs: one pass
+                # per image, as a one-image schedule runs them (the estimate is the same on every rank of a tile shard)
+                for n in range(start, min(start + k, N)):
+                    finished += one_pass(slice(n, n + 1))
+                    if host.interrupted():
+                        break
+            else:
+                finished += done
             if host.interrupted():
                 break
         interrupted = host.interrupted()
         if sharded:
             self._exchange_regions(result, in_bboxes, out_bboxes)
-        total = len(mine) * len(images)
-        if finished == 0 and total > 0 and interrupted:
+        if finished == 0 and mine and interrupted:
             return self._cheap_fallback(z, device, dtype)
         if not interrupted and torch.isnan(result).any():
             raise RuntimeError("[Tiled VAE]: NaN in the result (the reference's test_for_nans, tilevae.py:625)")
@@ -571,8 +616,8 @@ class VAEHook:
                     site = barriers[rnd]
                 if site is None:
                     break
-                stat_len = NUM_GROUPS * (z.shape[0] if not isinstance(backend, ve.TensorCoreBackend) else 1)
-                merged = collect.summary(stat_len, z.device)
+                stat_len = NUM_GROUPS * z.shape[0]
+                merged = collect.summary(stat_len, z.device, z.shape[0] if isinstance(backend, ve.TensorCoreBackend) else 1)
                 if merged is None:
                     break
                 mean, var = merged
@@ -597,20 +642,7 @@ class VAEHook:
         from . import vae_engine as ve
         if not barriers or not in_bboxes:
             return None
-        fps = {}
-        for b in in_bboxes:
-            key = (b[3] - b[2], b[1] - b[0])
-            if key not in fps:
-                fps[key] = ve.tile_footprint(ex.program, backend.name, backend.dtype, key[0], key[1], z.shape[0])
-        tiles = [fps[(b[3] - b[2], b[1] - b[0])] for b in in_bboxes]
-        held = [[fp.held(op.site) for fp in tiles] for op in barriers]            # what a park / upload moves
-        resident = [[fp.resident(op.site) for fp in tiles] for op in barriers]    # what a waiting tile holds
-        reserve = max(fp.working for fp in fps.values()) + 2 * max(max(h) for h in held)
-        dev = z.device
-        free = torch.cuda.mem_get_info(dev)[0] + torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev)
-        budget = max(free - reserve, 0)
-        if self.max_resident_bytes is not None:
-            budget = min(budget, max(int(self.max_resident_bytes), 0))
+        held, resident, reserve, budget = self._residency(ex.program, backend, z.shape[0], in_bboxes, barriers, self._free_bytes(z.device))
         self.last_park_stats.update(budget=budget, reserve=reserve)
         n = len(in_bboxes)
         orders = [list(range(n)) if r % 2 == 0 else list(range(n - 1, -1, -1)) for r in range(len(barriers))]
@@ -623,6 +655,64 @@ class VAEHook:
                 sizes[i] = max(sizes.get(i, 0), held[r][i])
         ve.require_host_memory(sum(sizes.values()))
         return parked, sizes
+
+    @staticmethod
+    def _free_bytes(dev) -> int:
+        """Free device memory: the driver's, plus the caching allocator's unused blocks."""
+        return torch.cuda.mem_get_info(dev)[0] + torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev)
+
+    def _residency(self, program, backend, images, in_bboxes, barriers, free):
+        """Bytes the tiles of a pass over `images` images move (held) and keep (resident) at each barrier, the working
+        reserve (the largest working set of one tile and two tiles' parked bytes: one upload and one write-back in
+        flight) and the budget for the resident tiles: free less the reserve, lowered by `max_resident_bytes`."""
+        from . import vae_engine as ve
+        fps = {}
+        for b in in_bboxes:
+            key = (b[3] - b[2], b[1] - b[0])
+            if key not in fps:
+                fps[key] = ve.tile_footprint(program, backend.name, backend.dtype, key[0], key[1], images, images=images)
+        tiles = [fps[(b[3] - b[2], b[1] - b[0])] for b in in_bboxes]
+        held = [[fp.held(op.site) for fp in tiles] for op in barriers]            # what a park / upload moves
+        resident = [[fp.resident(op.site) for fp in tiles] for op in barriers]    # what a waiting tile holds
+        reserve = max(fp.working for fp in fps.values()) + 2 * max((max(h) for h in held), default=0)
+        budget = max(free - reserve, 0)
+        if self.max_resident_bytes is not None:
+            budget = min(budget, max(int(self.max_resident_bytes), 0))
+        return held, resident, reserve, budget
+
+    def _images_per_pass(self, program, backend, z, in_bboxes) -> int:
+        """How many images of the batch z go through the tensor-core tiles together: `images_per_pass` when set, else
+        the largest k whose pass fits in GPU memory (working reserve within the free memory) with no tile parked at any
+        barrier under the budget `_park_plan` would use.  1 (a pass per image) when no k > 1 does.  Under the tile
+        shard every rank takes the smallest rank's choice, so the statistics rounds pair up."""
+        from . import vae_engine as ve
+        N = z.shape[0]
+        if self.images_per_pass is not None:
+            k = max(1, min(int(self.images_per_pass), N))
+        else:
+            if self.fast_mode:
+                _, end = ve.estimated_ops(program, self.color_fix)
+                barriers = [op for i, op in enumerate(program.ops) if isinstance(op, ve.Norm) and i >= end]
+            else:
+                barriers = [op for op in program.ops if isinstance(op, ve.Norm)]
+            free = self._free_bytes(z.device)
+            n = len(in_bboxes)
+            orders = [list(range(n)) if r % 2 == 0 else list(range(n - 1, -1, -1)) for r in range(len(barriers))]
+
+            def fits(k):
+                if not in_bboxes:
+                    return True
+                _, resident, reserve, budget = self._residency(program, backend, k, in_bboxes, barriers, free)
+                if reserve > free or any(sum(r) > budget for r in resident):
+                    return False
+                return not any(ve.plan_residency(orders, resident, budget))
+            k = pick_images_per_pass(N, fits)
+        if self._shard_world > 1:
+            import torch.distributed as dist
+            t = torch.tensor([k], dtype=torch.int64, device=z.device)
+            dist.all_reduce(t, op=dist.ReduceOp.MIN, group=self._shard_group)
+            k = int(t.item())
+        return k
 
     def _exchange_regions(self, result, in_bboxes, out_bboxes):
         """Tile shard: every rank pasted its own tiles; gather the disjoint output regions (one all-gather of the

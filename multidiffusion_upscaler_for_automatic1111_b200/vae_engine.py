@@ -143,13 +143,14 @@ class TileFootprint:
         return self.act[site] + (self.act[site] if self.alias[site] else self.skip[site])
 
 
-def tile_footprint(program: Program, backend_name: str, dtype, h: int, w: int, batch: int = 1) -> TileFootprint:
-    """Shape walk of `program` for an input tile of h x w pixels.  backend_name "wgmma": channels-last, one image,
-    conv_in's input padded to 64 channels, output channels rounded up to 16; "modules": NCHW, `batch` images,
-    exact channels."""
+def tile_footprint(program: Program, backend_name: str, dtype, h: int, w: int, batch: int = 1,
+                   images: Optional[int] = None) -> TileFootprint:
+    """Shape walk of `program` for an input tile of h x w pixels.  backend_name "wgmma": channels-last, `images` images
+    per pass (None: one), conv_in's input padded to 64 channels, output channels rounded up to 16; "modules": NCHW,
+    `batch` images, exact channels."""
     e = torch.empty((), dtype=dtype).element_size()
     tc = backend_name == TensorCoreBackend.name
-    n = 1 if tc else batch
+    n = (images or 1) if tc else batch
 
     def nbytes(c, hh, ww):
         return n * c * hh * ww * e
@@ -206,12 +207,12 @@ def tile_footprint(program: Program, backend_name: str, dtype, h: int, w: int, b
             T = H * W
             y = nbytes(c, H, W)
             if tc:
-                qk = 2 * T * ops.round_up(c, 8) * e
+                qk = 2 * n * T * ops.round_up(c, 8) * e
                 if T > SCORE_MATRIX_MAX_TOKENS:
-                    extra = qk + 2 * T * c * e                                  # v, o
-                else:
+                    extra = qk + 2 * n * T * c * e                              # v, o
+                else:                                                           # one image's v^T and scores at a time
                     Tp = ops.round_up(T, 8)
-                    extra = qk + c * Tp * e + T * Tp * e + T * ops.round_up(c, 8) * e   # v^T, scores, o
+                    extra = qk + c * Tp * e + T * Tp * e + n * T * ops.round_up(c, 8) * e   # v^T, scores, o
                 live(extra, y, y)
             else:
                 live(3 * y, 2 * y, y)                      # q, k, v; the attention output and its NCHW copy
@@ -481,14 +482,15 @@ class TensorCoreBackend:
         return ops.conv2d_nhwc(a, wp, b, ksize=k, pad=(k // 2, k // 2), residual=skip, cout=cout_rows, post=post, dual=dual)
 
     def norm_affine(self, op: Norm, mean, var):
-        """Per-channel (scale, shift, act) equivalent to custom_group_norm (+ SiLU) with these statistics:
-        y = x * gamma[c] / sqrt(var[g] + eps) + (beta[c] - mean[g] * gamma[c] / sqrt(var[g] + eps))."""
+        """Per-image, per-channel (scale [n, C], shift [n, C], act) equivalent to custom_group_norm (+ SiLU) with the
+        statistics mean / var [n * groups]: y = x * gamma[c] / sqrt(var[g] + eps) + (beta[c] - mean[g] * gamma[c] /
+        sqrt(var[g] + eps)).  Element-wise, so an image's constants do not depend on the other images."""
         gamma, beta = self._affine(op.module)
         c = op.module.num_channels
         cpg = c // NUM_GROUPS
-        rstd = (1.0 / torch.sqrt(var.float() + GN_EPS)).repeat_interleave(cpg)
+        rstd = (1.0 / torch.sqrt(var.float().view(-1, NUM_GROUPS) + GN_EPS)).repeat_interleave(cpg, dim=1)
         scale = rstd * gamma if gamma is not None else rstd
-        shift = -mean.float().repeat_interleave(cpg) * scale
+        shift = -mean.float().view(-1, NUM_GROUPS).repeat_interleave(cpg, dim=1) * scale
         if beta is not None:
             shift = shift + beta
         return scale.contiguous(), shift.contiguous(), bool(op.act)
@@ -507,33 +509,42 @@ class TensorCoreBackend:
         return ops.gn_apply_nhwc(a, mean, var, gamma, beta, op.act, NUM_GROUPS, GN_EPS)
 
     def attention(self, a, op: Attention, skip, post=None, dual=False):
-        """softmax(q k^T / sqrt(C)) v + proj_out (tile_utils/attn.py:49-72).  Up to SCORE_MATRIX_MAX_TOKENS tokens:
-        four tensor-core GEMMs and one row softmax, the [tokens, tokens] score matrix in HBM (388 MB fp16 for a 118 x 118
-        tile); larger tiles: the fused online-softmax kernel, no score matrix."""
+        """softmax(q k^T / sqrt(C)) v + proj_out (tile_utils/attn.py:49-72) of each of the n images of a [n, H, W, C]
+        tile.  The q / k / v projections of all images are one GEMM (a row's result does not depend on its neighbours).
+        Up to SCORE_MATRIX_MAX_TOKENS tokens: per image, the scores, one row softmax and the P V GEMM, the [tokens, tokens]
+        score matrix in HBM (388 MB fp16 for a 118 x 118 tile); larger tiles: the fused online-softmax kernel over all
+        images in one launch, no score matrix."""
         m = op.module
-        _, H, W, C = a.shape
+        n, H, W, C = a.shape
         T = H * W
-        x2 = a.view(T, C)
+        x2 = a.view(n * T, C)
         wq, bq, *_ = self._conv_w(m.q)
         wk, bk, *_ = self._conv_w(m.k)
         wv, bv, *_ = self._conv_w(m.v)
         q = ops.gemm_nt(x2, wq[0], bias=bq)
         k = ops.gemm_nt(x2, wk[0], bias=bk)
         wp, bp, *_ = self._conv_w(m.proj_out)
+        alpha = float(int(C) ** -0.5)
         if T > SCORE_MATRIX_MAX_TOKENS:
-            o = ops.attention(q, k, ops.gemm_nt(x2, wv[0], bias=bv), float(int(C) ** -0.5))
-            return ops.conv2d_nhwc(o.view(1, H, W, C), wp, bp, ksize=1, residual=skip, post=post, dual=dual)
+            v = ops.gemm_nt(x2, wv[0], bias=bv)
+            per = (lambda t: t) if n == 1 else (lambda t: t.unflatten(0, (n, T)))     # [T, C] for one image, [n, T, C] for several
+            o = ops.attention(per(q), per(k), per(v), alpha)
+            return ops.conv2d_nhwc(o.view(n, H, W, C), wp, bp, ksize=1, residual=skip, post=post, dual=dual)
         Tp = ops.round_up(T, 8)
-        vt = torch.empty((C, Tp), dtype=self.dtype, device=self.device)
-        if Tp != T:
-            vt[:, T:].zero_()          # K of the P V GEMM runs over the padded pitch: P's padding is 0, V's must be finite
-        # V^T[c, t] = sum_i Wv[c, i] x[t, i] + bv[c]: the GEMM with the operands swapped, bias per output row
-        ops.gemm_nt(wv[0], x2, bias=bv, bias_per_row=True, out=vt[:, :T])
-        s = torch.empty((T, Tp), dtype=self.dtype, device=self.device)
-        ops.gemm_nt(q, k, alpha=float(int(C) ** -0.5), out=s[:, :T])
-        ops.softmax_rows(s, T, out=s)
-        o = ops.gemm_nt(s, vt)         # K = Tp (a multiple of 8; the last partial 64-chunk is zero-filled by the TMA unit)
-        return ops.conv2d_nhwc(o.view(1, H, W, C), wp, bp, ksize=1, residual=skip, post=post, dual=dual)
+        o = torch.empty((n * T, C), dtype=self.dtype, device=self.device)
+        for i in range(n):
+            rows = slice(i * T, (i + 1) * T)
+            vt = torch.empty((C, Tp), dtype=self.dtype, device=self.device)
+            if Tp != T:
+                vt[:, T:].zero_()      # K of the P V GEMM runs over the padded pitch: P's padding is 0, V's must be finite
+            # V^T[c, t] = sum_i Wv[c, i] x[t, i] + bv[c]: the GEMM with the operands swapped, bias per output row
+            ops.gemm_nt(wv[0], x2[rows], bias=bv, bias_per_row=True, out=vt[:, :T])
+            s = torch.empty((T, Tp), dtype=self.dtype, device=self.device)
+            ops.gemm_nt(q[rows], k[rows], alpha=alpha, out=s[:, :T])
+            ops.softmax_rows(s, T, out=s)
+            ops.gemm_nt(s, vt, out=o[rows])    # K = Tp (a multiple of 8; the last partial 64-chunk is zero-filled by the TMA unit)
+            del vt, s                  # one image's scores at a time
+        return ops.conv2d_nhwc(o.view(n, H, W, C), wp, bp, ksize=1, residual=skip, post=post, dual=dual)
 
     def tanh(self, a):
         return torch.tanh(a)
@@ -561,6 +572,13 @@ def pick_backend(program: Program, device, dtype):
 
 
 # ----------------------------------------------------------------------------------------------- executor
+def estimated_ops(program: Program, color_fix: bool) -> Tuple[int, int]:
+    """(index of the last Norm op, end of the ops `Executor.estimate` runs): fast mode freezes the sites of the Norm ops
+    before `end`; the others stay barriers."""
+    last_norm = max(i for i, op in enumerate(program.ops) if isinstance(op, Norm))
+    return last_norm, min(last_norm + 1, program.first_resample if color_fix else len(program.ops))
+
+
 @dataclass
 class TileState:
     act: object
@@ -646,15 +664,15 @@ class Executor:
         st.pc += 1
 
     @torch.no_grad()
-    def estimate(self, act, color_fix: bool) -> bool:
+    def estimate(self, act, color_fix: bool, report: bool = True) -> bool:
         """Fast mode (tilevae.py:464-505): run the program on the down-sampled input, freezing each GroupNorm site
-        with the statistics of that single tensor.  With color_fix the sites from the first down-sampling on stay
-        barriers.  Returns False (nothing frozen) when a NaN shows up."""
+        with the statistics of that single tensor (per image on the tensor cores).  With color_fix the sites from the
+        first down-sampling on stay barriers (`estimated_ops`).  Returns False (nothing frozen) when a NaN shows up;
+        `report`: say so on stdout."""
         if self.program.num_sites == 0:
             raise ValueError("No group norm found in the task queue")
         opsq = self.program.ops
-        last_norm = max(i for i, op in enumerate(opsq) if isinstance(op, Norm))
-        end = min(last_norm + 1, self.program.first_resample if color_fix else len(opsq))
+        last_norm, end = estimated_ops(self.program, color_fix)
         st = TileState(act)
         frozen: List[Optional[Tuple[torch.Tensor, torch.Tensor]]] = [None] * self.program.num_sites
         nan = None
@@ -671,7 +689,8 @@ class Executor:
             flag = self.be.has_nan(st.act)
             nan = flag if nan is None else (nan | flag)
         if nan is not None and bool(nan):
-            print("Nan detected in fast mode estimation. Fast mode disabled.")
+            if report:
+                print("Nan detected in fast mode estimation. Fast mode disabled.")
             return False
         self.frozen = frozen
         self._affine_cache = {}

@@ -62,10 +62,25 @@ def fold_upsample_weight(weight: torch.Tensor, dtype: torch.dtype, cin_pad: Opti
     return out.contiguous()
 
 
+def _post_stride(post, N: int, Cout: int) -> int:
+    """Elements between the images' post vectors: post = (scale, shift, act) with scale / shift [Cout] (one set for every
+    image) or [N, >= Cout] (image n's GroupNorm constants in row n)."""
+    if post is None:
+        return 0
+    scale, shift = post[0], post[1]
+    assert scale.dtype == torch.float32 and shift.dtype == torch.float32 and scale.shape == shift.shape and scale.is_contiguous() and shift.is_contiguous()
+    if scale.dim() == 1 or scale.shape[0] == 1:
+        assert scale.numel() >= Cout
+        return 0
+    assert scale.dim() == 2 and scale.shape[0] == N and scale.shape[1] >= Cout, f"post constants {tuple(scale.shape)} for {N} images"
+    return scale.stride(0)
+
+
 def upconv2x_nhwc(x: torch.Tensor, w16: torch.Tensor, bias: Optional[torch.Tensor] = None, *, cout: Optional[int] = None,
                   out: Optional[torch.Tensor] = None, post: Optional[Tuple[torch.Tensor, torch.Tensor, bool]] = None, dual: bool = False):
     """Nearest-2x upsample + 3x3 / pad 1 convolution in one pass over the LOW-resolution x [N, H, W, Cin] ->
-    [N, 2H, 2W, Cout]; w16 from fold_upsample_weight.  dual (needs post): returns (result before post, result after post)."""
+    [N, 2H, 2W, Cout]; w16 from fold_upsample_weight.  post as in conv2d_nhwc; dual (needs post): returns (result before
+    post, result after post)."""
     _cuda(x, "x"); _cuda(w16, "w16")
     N, H, W, Cin = x.shape
     taps, cout_rows, w_cin = w16.shape
@@ -77,14 +92,13 @@ def upconv2x_nhwc(x: torch.Tensor, w16: torch.Tensor, bias: Optional[torch.Tenso
     d = TdConvDesc(N=N, H=H, W=W, Cin=Cin, Cout=Cout, kh=3, kw=3, stride=1, pad_top=1, pad_left=1, OH=2 * H, OW=2 * W,
                    dtype=dtype_code(x.dtype), bias_per_row=0, alpha=1.0, x_pitch=x.stride(2), w_pitch=w16.stride(1), y_pitch=out.stride(2),
                    res_pitch=0, post_scale=post[0].data_ptr() if post is not None else None,
-                   post_shift=post[1].data_ptr() if post is not None else None, post_act=int(bool(post[2])) if post is not None else 0)
+                   post_shift=post[1].data_ptr() if post is not None else None, post_act=int(bool(post[2])) if post is not None else 0,
+                   post_stride=_post_stride(post, N, Cout))
     out2 = None
     if dual:
         assert post is not None, "the second output is the post stage's result"
         out2 = torch.empty_like(out)
         d.y2, d.y2_pitch = out2.data_ptr(), out2.stride(2)
-    if post is not None:
-        assert post[0].dtype == torch.float32 and post[1].dtype == torch.float32 and post[0].numel() >= Cout and post[1].numel() >= Cout
     if bias is not None:
         assert bias.dtype == torch.float32 and bias.is_cuda
     with torch.cuda.device(x.device):
@@ -100,8 +114,8 @@ def conv2d_nhwc(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] =
     """One convolution on the tensor cores.  x: [N, H, W, Cin] NHWC; w: packed [ksize*ksize, Cout_rows, Cin];
     bias: fp32 [Cout] (or [N*OH*OW] with bias_per_row); residual: [N, OH, OW, Cout] added in the epilogue.
     pad = (top, left) zero padding; out_hw defaults to the 'same' size for stride 1.
-    post = (scale, shift, silu): per-channel affine (+ SiLU) on the fp32 result; dual (needs post): two outputs, returns
-    (result before post, result after post)."""
+    post = (scale, shift, silu): per-channel affine (+ SiLU) on the fp32 result, scale / shift fp32 [Cout] for every image
+    or [N, Cout] per image; dual (needs post): two outputs, returns (result before post, result after post)."""
     _cuda(x, "x"); _cuda(w, "w")
     N, H, W, Cin = x.shape
     taps, cout_rows, w_cin = w.shape
@@ -118,15 +132,13 @@ def conv2d_nhwc(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] =
                    x_pitch=x.stride(2), w_pitch=w.stride(1), y_pitch=out.stride(2),
                    res_pitch=residual.stride(2) if residual is not None else 0,
                    post_scale=post[0].data_ptr() if post is not None else None, post_shift=post[1].data_ptr() if post is not None else None,
-                   post_act=int(bool(post[2])) if post is not None else 0)
+                   post_act=int(bool(post[2])) if post is not None else 0, post_stride=_post_stride(post, N, Cout))
     assert x.stride(3) == 1 and out.stride(3) == 1 and w.stride(2) == 1
     out2 = None
     if dual:
         assert post is not None, "the second output is the post stage's result"
         out2 = torch.empty_like(out)
         d.y2, d.y2_pitch = out2.data_ptr(), out2.stride(2)
-    if post is not None:
-        assert post[0].dtype == torch.float32 and post[1].dtype == torch.float32 and post[0].numel() >= Cout and post[1].numel() >= Cout
     if bias is not None:
         assert bias.dtype == torch.float32 and bias.is_cuda
     with torch.cuda.device(x.device):
@@ -156,19 +168,25 @@ def gemm_nt(a: torch.Tensor, b: torch.Tensor, bias: Optional[torch.Tensor] = Non
 def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, alpha: float, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """O[T, C] = softmax(alpha * Q K^T) V in one fused kernel (csrc/td_attn.cu): online softmax, nothing of size T x T is
     allocated.  q / k / v / out: [T, C] views with unit inner stride, row pitches multiples of 8 elements; C % 64 == 0,
-    C <= 512."""
+    C <= 512.  [N, T, C] views: N images in one launch (td_attention_batched), image strides multiples of 8 elements."""
     _cuda(q, "q"); _cuda(k, "k"); _cuda(v, "v")
-    T, C = q.shape
-    assert k.shape == (T, C) and v.shape == (T, C), f"q {tuple(q.shape)}, k {tuple(k.shape)}, v {tuple(v.shape)} differ"
+    shape = tuple(q.shape)
+    assert len(shape) in (2, 3) and k.shape == shape and v.shape == shape, f"q {shape}, k {tuple(k.shape)}, v {tuple(v.shape)} differ"
     assert k.dtype == q.dtype and v.dtype == q.dtype and k.device == q.device and v.device == q.device
     if out is None:
-        out = torch.empty((T, C), dtype=q.dtype, device=q.device)
-    assert out.shape == (T, C) and out.dtype == q.dtype
+        out = torch.empty(shape, dtype=q.dtype, device=q.device)
+    assert out.shape == shape and out.dtype == q.dtype
     for name, t in (("q", q), ("k", k), ("v", v), ("out", out)):
-        assert t.stride(1) == 1 and t.stride(0) % 8 == 0, f"{name}: unit inner stride and a row pitch that is a multiple of 8 (got {t.stride()})"
+        assert t.stride(-1) == 1 and t.stride(-2) % 8 == 0, f"{name}: unit inner stride and a row pitch that is a multiple of 8 (got {t.stride()})"
+    T, C = shape[-2:]
     with torch.cuda.device(q.device):
-        check(lib.td_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), T, C, q.stride(0), k.stride(0), v.stride(0),
-                               out.stride(0), float(alpha), dtype_code(q.dtype), current_stream_ptr(q.device)))
+        if len(shape) == 2:
+            check(lib.td_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), T, C, q.stride(0), k.stride(0), v.stride(0),
+                                   out.stride(0), float(alpha), dtype_code(q.dtype), current_stream_ptr(q.device)))
+        else:
+            check(lib.td_attention_batched(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), shape[0], T, C, q.stride(1), k.stride(1),
+                                           v.stride(1), out.stride(1), q.stride(0), k.stride(0), v.stride(0), out.stride(0), float(alpha),
+                                           dtype_code(q.dtype), current_stream_ptr(q.device)))
     return out
 
 
@@ -222,31 +240,36 @@ def upsample2x_nhwc(x: torch.Tensor) -> torch.Tensor:
 
 
 def gn_stats_nhwc(x: torch.Tensor, groups: int = NUM_GROUPS):
-    """Biased variance and mean per group of ONE channels-last image [1, H, W, C] -> (var, mean) fp32 [groups]."""
+    """Biased variance and mean per (image, group) of channels-last images [N, H, W, C] -> (var, mean) fp32 [N * groups].
+    Each image gets the bits of its own one-image reduction (td_gn_stats_nhwc_batched)."""
     _cuda(x, "x")
-    assert x.is_contiguous() and x.shape[0] == 1
-    _, H, W, C = x.shape
+    assert x.is_contiguous()
+    N, H, W, C = x.shape
     dev = x.device
-    ws_bytes = lib.td_gn_stats_nhwc_workspace_bytes(H * W, C, groups)
+    ws_bytes = lib.td_gn_stats_nhwc_batched_workspace_bytes(N, H * W, C, groups)
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-    mean = torch.empty(groups, dtype=torch.float32, device=dev)
-    var = torch.empty(groups, dtype=torch.float32, device=dev)
+    mean = torch.empty(N * groups, dtype=torch.float32, device=dev)
+    var = torch.empty(N * groups, dtype=torch.float32, device=dev)
     with torch.cuda.device(dev):
-        check(lib.td_gn_stats_nhwc(x.data_ptr(), H * W, C, groups, dtype_code(x.dtype), ws.data_ptr(), ws_bytes, mean.data_ptr(),
-                                   var.data_ptr(), current_stream_ptr(dev)))
+        check(lib.td_gn_stats_nhwc_batched(x.data_ptr(), N, H * W, C, groups, dtype_code(x.dtype), ws.data_ptr(), ws_bytes, mean.data_ptr(),
+                                           var.data_ptr(), current_stream_ptr(dev)))
     return var, mean
 
 
 def gn_apply_nhwc(x: torch.Tensor, mean: torch.Tensor, var: torch.Tensor, gamma: Optional[torch.Tensor], beta: Optional[torch.Tensor],
                   act: bool, groups: int = NUM_GROUPS, eps: float = GN_EPS, inplace: bool = False) -> torch.Tensor:
+    """GroupNorm (+ SiLU) of channels-last images [N, H, W, C] with per-image statistics mean / var fp32 [N * groups]."""
     _cuda(x, "x")
-    assert x.is_contiguous() and x.shape[0] == 1
-    _, H, W, C = x.shape
+    assert x.is_contiguous()
+    N, H, W, C = x.shape
+    assert mean.numel() == N * groups and var.numel() == N * groups, f"statistics of {mean.numel()} groups for {N} images"
+    assert mean.dtype == torch.float32 and var.dtype == torch.float32 and mean.is_contiguous() and var.is_contiguous()
     y = x if inplace else torch.empty_like(x)
     with torch.cuda.device(x.device):
-        check(lib.td_gn_apply_nhwc(x.data_ptr(), y.data_ptr(), H * W, C, groups, dtype_code(x.dtype), mean.data_ptr(), var.data_ptr(),
-                                   gamma.data_ptr() if gamma is not None else None, beta.data_ptr() if beta is not None else None,
-                                   float(eps), int(act), current_stream_ptr(x.device)))
+        check(lib.td_gn_apply_nhwc_batched(x.data_ptr(), y.data_ptr(), N, H * W, C, groups, dtype_code(x.dtype), mean.data_ptr(),
+                                           var.data_ptr(), gamma.data_ptr() if gamma is not None else None,
+                                           beta.data_ptr() if beta is not None else None, float(eps), int(act),
+                                           current_stream_ptr(x.device)))
     return y
 
 
