@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define TD_ABI_VERSION 16
+#define TD_ABI_VERSION 17
 
 typedef enum td_status {
     TD_OK = 0,
@@ -199,6 +199,32 @@ int td_blend_multidiffusion(const td_grid* g, const void* const* batch_ptrs, int
 int td_blend_mixture(const td_grid* g, const void* const* batch_ptrs, int num_batches, int tile_bs,
                      int N, int C, int tile_dtype, int acc_dtype, const float* tile_weights,
                      const float* rescale, void* x_buffer, uint32_t flags, void* stream);
+
+/* Inpainting (new: the reference denoises every tile and lets the WebUI discard the kept area afterwards).
+ *
+ * td_grid_active_tiles: active_dev[t] = 1 when at least one element of tile t's window, over all `planes` leading planes of
+ *   the mask, is not exactly 1.0 (NaN is not 1.0), else 0 -- one launch, T bytes.  mask: DEVICE [planes, H, W] contiguous in
+ *   `dtype` (the WebUI's latent mask, 1 = keep the original), aligned to its element size.  Refused (TD_ERR_INVALID_ARG, output
+ *   untouched): a null or misaligned pointer, planes <= 0, an unknown dtype, a canvas the grid entries refuse; a periodic plan
+ *   (g->wrap != 0) is TD_ERR_UNSUPPORTED.
+ *
+ * td_blend_multidiffusion_sparse / td_blend_mixture_sparse: td_blend_multidiffusion / td_blend_mixture over the active tiles
+ *   only.  slot_dev: DEVICE int32 [T]: tile t's position in the compact batches, or -1 for a skipped tile; slot_host: the same
+ *   values on the host, validated before any launch; n_slots must be T.  With K = the number of entries >= 0, the positions
+ *   0 .. K-1 must each appear once, and batch_ptrs / num_batches / tile_bs hold the K kept tiles as td_blend_multidiffusion's
+ *   table holds all T (K == 0: num_batches == 0, batch_ptrs may be NULL).  A skipped tile's visits are dropped, the others keep
+ *   tile order, so a pixel all of whose covering tiles are kept gets the dense result bit for bit; a pixel no kept tile covers
+ *   gets the blend of nothing (zeros).  weights / rescale are those of the full plan.  Forms: the default cp.async kernels, and
+ *   the generic one where they do not apply or under TD_FLAG_FORCE_GENERIC; flags other than FORCE_GENERIC, NO_PDL and
+ *   ONE_PLANE are refused, as are a periodic plan (TD_ERR_UNSUPPORTED) and a bad slot table (TD_ERR_INVALID_ARG). */
+int td_grid_active_tiles(const td_grid* g, const void* mask, int planes, int dtype, uint8_t* active_dev, void* stream);
+int td_blend_multidiffusion_sparse(const td_grid* g, const void* const* batch_ptrs, int num_batches, int tile_bs, int N, int C,
+                                   int tile_dtype, int acc_dtype, const float* weights, const float* rcp_weights, float* x_out,
+                                   void* x_buffer, const int32_t* slot_dev, const int32_t* slot_host, int n_slots, uint32_t flags,
+                                   void* stream);
+int td_blend_mixture_sparse(const td_grid* g, const void* const* batch_ptrs, int num_batches, int tile_bs, int N, int C,
+                            int tile_dtype, int acc_dtype, const float* tile_weights, const float* rescale, void* x_buffer,
+                            const int32_t* slot_dev, const int32_t* slot_host, int n_slots, uint32_t flags, void* stream);
 
 /* ------------------------------------------------------------------------- *
  *  Tiled VAE (scripts/tilevae.py of the reference).

@@ -33,7 +33,7 @@ TD_MAX_GRID_DIM = 256
 TD_MAX_BATCH_PTRS = 128
 TD_MAX_PEERS = 16
 TD_IPC_HANDLE_BYTES = 64
-ABI_VERSION = 16
+ABI_VERSION = 17
 
 DTYPE_CODE = {torch.float16: TD_F16, torch.bfloat16: TD_BF16, torch.float32: TD_F32}
 
@@ -183,6 +183,12 @@ _SIGNATURES = {
     "td_softmax_rows": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int64, c_int, c_void_p]),
     "td_blend_mixture": (c_int, [POINTER(TdGrid), POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_int,
                                  c_void_p, c_void_p, c_void_p, c_uint32, c_void_p]),
+    "td_grid_active_tiles": (c_int, [POINTER(TdGrid), c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "td_blend_multidiffusion_sparse": (c_int, [POINTER(TdGrid), POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_int,
+                                               c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int32), c_int, c_uint32,
+                                               c_void_p]),
+    "td_blend_mixture_sparse": (c_int, [POINTER(TdGrid), POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_int,
+                                        c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int32), c_int, c_uint32, c_void_p]),
 }
 
 

@@ -24,6 +24,7 @@
 #include <algorithm>
 #include <cstdint>
 #include <mutex>
+#include <vector>
 
 #include "td_b200.h"
 #include "td_device.cuh"
@@ -413,6 +414,51 @@ __device__ __forceinline__ int window_row_index(const BlendParams& p) {
 }
 __device__ __forceinline__ int plane_group_index(const BlendParams& p) { return p.sched == 0 ? (int)blockIdx.z : (int)blockIdx.y; }
 
+// Sparse blends (td_blend_*_sparse): the visit table of a cp.async CTA with the skipped tiles (slot[t] < 0) dropped and the others
+// kept in tile order, compacted with one ballot per warp.  Tile t lives at position slot[t] of the compact batches.  Every thread of
+// the CTA calls this (it contains the barrier that publishes the table); returns the number of visits kept.
+template <typename T>
+__device__ __forceinline__ int prepare_sparse_visits(const BlendParams& p, const int* __restrict__ slot, int nv, int r_lo, int c_lo,
+                                                     int nc, int x_lo, int y_lo, long long plane_elems, VisitEntry* s_visit,
+                                                     int* s_shift) {
+    constexpr int L2V = Vec<T>::kLog2;
+    constexpr int VEC = Vec<T>::kElems;
+    __shared__ int s_kept[kAsThreads / 32];
+    const GeomParams& g = p.g;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    int r = 0, c = 0, sl = -1;
+    if (tid < nv) {
+        const int ri = tid / nc;
+        r = r_lo + ri;
+        c = c_lo + (tid - ri * nc);
+        sl = __ldg(slot + r * g.cols + c);
+    }
+    const unsigned kept = __ballot_sync(0xffffffffu, sl >= 0);
+    if (lane == 0) s_kept[warp] = __popc(kept);
+    __syncthreads();
+    int pos = __popc(kept & ((1u << lane) - 1u)), total = 0;
+#pragma unroll
+    for (int w = 0; w < kAsThreads / 32; ++w) {
+        pos += w < warp ? s_kept[w] : 0;
+        total += s_kept[w];
+    }
+    if (sl >= 0) {
+        const unsigned b = fastdiv((unsigned)sl, p.bs_magic);
+        const int u0 = x_lo - (int)g.xs[c];
+        const int v0 = y_lo - (int)g.ys[r], k0 = u0 >> L2V;
+        const long long elem = (long long)((unsigned)sl - b * (unsigned)p.tile_bs) * p.tile_stride + plane_elems +
+                               (long long)v0 * g.tw + (long long)k0 * VEC;
+        VisitEntry e;
+        e.origin = (long long)reinterpret_cast<uintptr_t>(p.batch_ptrs[b]) + elem * (long long)sizeof(T);
+        e.v0 = v0;
+        e.k0 = k0;
+        s_visit[pos] = e;
+        s_shift[pos] = u0 & (VEC - 1);
+    }
+    __syncthreads();
+    return total;
+}
+
 template <typename T, int S, int PPC>
 __device__ __forceinline__ void consume_planes(uint4 (&acc)[PPC], const unsigned char* p) {
 #pragma unroll
@@ -421,10 +467,12 @@ __device__ __forceinline__ void consume_planes(uint4 (&acc)[PPC], const unsigned
 
 // PPC = planes per CTA: the (n, c) planes of a patch share the visit table, the zero-fill predicate, the weights
 // and the shift, so a CTA that blends PPC planes amortises its prologue and runs PPC independent add chains.
-template <typename T, bool WRITE_BUF, bool FASTDIV, int PPC>
+// SPARSE (td_blend_multidiffusion_sparse, PPC 1): `slot` maps tile t to its position in the compact batches, or -1 to drop its
+// visits; without it the parameter is not read and the kernel's instruction stream is the dense one.
+template <typename T, bool WRITE_BUF, bool FASTDIV, int PPC, bool SPARSE = false>
 __global__ void __launch_bounds__(kAsThreads)
 blend_md_async_kernel(const __grid_constant__ BlendParams p, const float* __restrict__ weights, const float* __restrict__ rcp_weights,
-                      float* __restrict__ out_f32, T* __restrict__ out_buf) {
+                      float* __restrict__ out_f32, T* __restrict__ out_buf, const int* __restrict__ slot) {
     constexpr int VEC = Vec<T>::kElems;
     constexpr int L2V = Vec<T>::kLog2;
     constexpr int BX = kAsX * VEC;
@@ -442,7 +490,7 @@ blend_md_async_kernel(const __grid_constant__ BlendParams p, const float* __rest
     // tiles touching this patch: host-computed per patch row / col (uniform constant-bank reads)
     const int r_lo = p.prow_lo[by], c_lo = p.pcol_lo[blockIdx.x];
     const int nc = p.pcol_n[blockIdx.x];
-    const int nv = g.dbg_no_tiles ? 0 : (int)p.prow_n[by] * nc;   // <= the host's stage count
+    int nv = g.dbg_no_tiles ? 0 : (int)p.prow_n[by] * nc;   // <= the host's stage count
 
     // this thread's output vector; its weights are fetched now so that their latency hides behind the tile copies
     const int tx = tid % kAsX, ty = tid / kAsX;
@@ -466,22 +514,26 @@ blend_md_async_kernel(const __grid_constant__ BlendParams p, const float* __rest
 
     // ---- per-visit constants: thread i prepares visit i -------------------------------------------------
     const long long plane_bytes = (long long)g.th * g.tw * (long long)sizeof(T);
-    if (tid < nv) {
-        const int ri = tid / nc, ci = tid - ri * nc;
-        const int r = r_lo + ri, c = c_lo + ci;
-        const unsigned t = (unsigned)(r * g.cols + c);
-        const unsigned b = fastdiv(t, p.bs_magic);
-        const int u0 = x_lo - (int)g.xs[c];
-        const int v0 = y_lo - (int)g.ys[r], k0 = u0 >> L2V;
-        const long long elem = (long long)(t - b * (unsigned)p.tile_bs) * p.tile_stride + (long long)v0 * g.tw + (long long)k0 * VEC;
-        VisitEntry e;
-        e.origin = (long long)reinterpret_cast<uintptr_t>(p.batch_ptrs[b]) + elem * (long long)sizeof(T) + (long long)plane * plane_bytes;
-        e.v0 = v0;
-        e.k0 = k0;
-        s_visit[tid] = e;
-        s_shift[tid] = u0 & (VEC - 1);
+    if constexpr (SPARSE) {
+        nv = prepare_sparse_visits<T>(p, slot, nv, r_lo, c_lo, nc, x_lo, y_lo, (long long)plane * g.th * g.tw, s_visit, s_shift);
+    } else {
+        if (tid < nv) {
+            const int ri = tid / nc, ci = tid - ri * nc;
+            const int r = r_lo + ri, c = c_lo + ci;
+            const unsigned t = (unsigned)(r * g.cols + c);
+            const unsigned b = fastdiv(t, p.bs_magic);
+            const int u0 = x_lo - (int)g.xs[c];
+            const int v0 = y_lo - (int)g.ys[r], k0 = u0 >> L2V;
+            const long long elem = (long long)(t - b * (unsigned)p.tile_bs) * p.tile_stride + (long long)v0 * g.tw + (long long)k0 * VEC;
+            VisitEntry e;
+            e.origin = (long long)reinterpret_cast<uintptr_t>(p.batch_ptrs[b]) + elem * (long long)sizeof(T) + (long long)plane * plane_bytes;
+            e.v0 = v0;
+            e.k0 = k0;
+            s_visit[tid] = e;
+            s_shift[tid] = u0 & (VEC - 1);
+        }
+        __syncthreads();
     }
-    __syncthreads();
 
     // ---- issue every copy of this CTA: src = origin(visit) + offset(thread) + plane, zero-fill outside the tile -----
     if (tid < kAsSlots) {
@@ -597,10 +649,11 @@ __device__ __forceinline__ void mod_accumulate(float (&acc)[Vec<T>::kElems], con
 
 // WINDOW: a row-window launch (td_blend_mixture_rows: py0 / py_count, sched, halo wait); without it the grid is the whole
 // canvas with blockIdx.y = patch row, and none of that code is compiled in (the whole-canvas blend keeps its instruction stream).
-template <typename T, bool WINDOW>
+// SPARSE (td_blend_mixture_sparse, whole canvas only): visits through the slot table, as in blend_md_async_kernel.
+template <typename T, bool WINDOW, bool SPARSE = false>
 __global__ void __launch_bounds__(kAsThreads)
 blend_mod_async_kernel(const __grid_constant__ BlendParams p, const float* __restrict__ tile_weights, const float* __restrict__ rescale,
-                       T* __restrict__ out_buf) {
+                       T* __restrict__ out_buf, const int* __restrict__ slot) {
     constexpr int VEC = Vec<T>::kElems;
     constexpr int L2V = Vec<T>::kLog2;
     constexpr int BX = kAsX * VEC;
@@ -614,7 +667,7 @@ blend_mod_async_kernel(const __grid_constant__ BlendParams p, const float* __res
     const int x_lo = blockIdx.x * BX, y_lo = by * kAsY;
     const int r_lo = p.prow_lo[by], c_lo = p.pcol_lo[blockIdx.x];
     const int nc = p.pcol_n[blockIdx.x];
-    const int nv = (int)p.prow_n[by] * nc;
+    int nv = (int)p.prow_n[by] * nc;
     pdl_launch_dependents();
 
     const int tx = tid % kAsX, ty = tid / kAsX;
@@ -632,23 +685,27 @@ blend_mod_async_kernel(const __grid_constant__ BlendParams p, const float* __res
         if (isinf(rs[j])) rs[j] = 0.0f;
     if constexpr (WINDOW) halo_wait(p, by, r_lo, tid);
 
-    if (tid < nv) {
-        const int ri = tid / nc, ci = tid - ri * nc;
-        const int r = r_lo + ri, c = c_lo + ci;
-        const unsigned t = (unsigned)(r * g.cols + c);
-        const unsigned b = fastdiv(t, p.bs_magic);
-        const int u0 = x_lo - (int)g.xs[c];
-        const int v0 = y_lo - (int)g.ys[r], k0 = u0 >> L2V;
-        const long long elem = (long long)(t - b * (unsigned)p.tile_bs) * p.tile_stride + (long long)plane * g.th * g.tw +
-                               (long long)v0 * g.tw + (long long)k0 * VEC;
-        VisitEntry e;
-        e.origin = (long long)reinterpret_cast<uintptr_t>(p.batch_ptrs[b]) + elem * (long long)sizeof(T);
-        e.v0 = v0;
-        e.k0 = k0;
-        s_visit[tid] = e;
-        s_shift[tid] = u0 & (VEC - 1);
+    if constexpr (SPARSE) {
+        nv = prepare_sparse_visits<T>(p, slot, nv, r_lo, c_lo, nc, x_lo, y_lo, (long long)plane * g.th * g.tw, s_visit, s_shift);
+    } else {
+        if (tid < nv) {
+            const int ri = tid / nc, ci = tid - ri * nc;
+            const int r = r_lo + ri, c = c_lo + ci;
+            const unsigned t = (unsigned)(r * g.cols + c);
+            const unsigned b = fastdiv(t, p.bs_magic);
+            const int u0 = x_lo - (int)g.xs[c];
+            const int v0 = y_lo - (int)g.ys[r], k0 = u0 >> L2V;
+            const long long elem = (long long)(t - b * (unsigned)p.tile_bs) * p.tile_stride + (long long)plane * g.th * g.tw +
+                                   (long long)v0 * g.tw + (long long)k0 * VEC;
+            VisitEntry e;
+            e.origin = (long long)reinterpret_cast<uintptr_t>(p.batch_ptrs[b]) + elem * (long long)sizeof(T);
+            e.v0 = v0;
+            e.k0 = k0;
+            s_visit[tid] = e;
+            s_shift[tid] = u0 & (VEC - 1);
+        }
+        __syncthreads();
     }
-    __syncthreads();
     if (tid < kAsSlots) {
         const int row = tid / kAsChunks, j = tid - row * kAsChunks;
         const int th1 = g.th - 1 - row, tw1 = (g.tw >> L2V) - 1 - j;
@@ -1001,11 +1058,12 @@ blend_md_tma_kernel(const __grid_constant__ TmaBlendParams<NB> p, const float* _
 
 // Blend, generic path: one element per thread, any width / alignment, tile
 // dtype and canvas dtype independent.
-template <typename TIn, typename TAcc, int MODE>
+// SPARSE: tile t is read at position slot[t] of the compact batches, and skipped when slot[t] < 0.
+template <typename TIn, typename TAcc, int MODE, bool SPARSE = false>
 __global__ void __launch_bounds__(256)
 blend_grid_generic_kernel(const __grid_constant__ BlendParams p, const float* __restrict__ weights,
                           const float* __restrict__ tile_weights, const float* __restrict__ rescale,
-                          float* __restrict__ out_f32, TAcc* __restrict__ out_buf, long long total) {
+                          float* __restrict__ out_f32, TAcc* __restrict__ out_buf, long long total, const int* __restrict__ slot) {
     __shared__ short s_ys[TD_MAX_GRID_DIM];
     __shared__ short s_xs[TD_MAX_GRID_DIM];
     const GeomParams& g = p.g;
@@ -1026,7 +1084,11 @@ blend_grid_generic_kernel(const __grid_constant__ BlendParams p, const float* __
     for (int r = r_lo; r <= r_hi; ++r) {
         const int v = y - (int)s_ys[r];
         for (int c = c_lo; c <= c_hi; ++c) {
-            const int t = r * g.cols + c;
+            int t = r * g.cols + c;
+            if constexpr (SPARSE) {
+                t = slot[t];
+                if (t < 0) continue;
+            }
             const int b = t / p.tile_bs;
             const int u = x - (int)s_xs[c];
             const TIn* tp = reinterpret_cast<const TIn*>(p.batch_ptrs[b]) + (long long)(t - b * p.tile_bs) * p.tile_stride +
@@ -1203,20 +1265,20 @@ void fill_patch_table(const int32_t* org, int n, int extent, int size, int patch
     }
 }
 
-template <typename T, bool WRITE_BUF, bool FASTDIV, int PPC>
+template <typename T, bool WRITE_BUF, bool FASTDIV, int PPC, bool SPARSE = false>
 int launch_blend_async_ppc(const BlendParams& bp, const float* weights, const float* rcp_weights, float* out_f32, void* out_buf,
-                           int nv_cap, bool pdl, cudaStream_t st) {
+                           int nv_cap, bool pdl, cudaStream_t st, const int* slot = nullptr) {
     constexpr int VEC = Vec<T>::kElems;
     constexpr int BX = kAsX * VEC;
     const int px = (bp.g.W + BX - 1) / BX, py = (bp.g.H + kAsY - 1) / kAsY, planes = bp.g.N * bp.g.C;
     const int smem = nv_cap * PPC * kAsStage;
     const char* what = "td_blend_multidiffusion (cp.async)";
-    int rc = smem_optin(blend_md_async_kernel<T, WRITE_BUF, FASTDIV, PPC>, smem, what);
+    int rc = smem_optin(blend_md_async_kernel<T, WRITE_BUF, FASTDIV, PPC, SPARSE>, smem, what);
     if (rc != TD_OK) return rc;
     const unsigned gy = (unsigned)(bp.py_count > 0 ? bp.py_count : py), gz = (unsigned)(planes / PPC);
     dim3 grid((unsigned)px, bp.sched ? gz : gy, bp.sched ? gy : gz);
-    return launch(what, blend_md_async_kernel<T, WRITE_BUF, FASTDIV, PPC>, grid, dim3(kAsThreads), (size_t)smem, st, pdl, bp, weights,
-                  rcp_weights, out_f32, (T*)out_buf);
+    return launch(what, blend_md_async_kernel<T, WRITE_BUF, FASTDIV, PPC, SPARSE>, grid, dim3(kAsThreads), (size_t)smem, st, pdl, bp,
+                  weights, rcp_weights, out_f32, (T*)out_buf, slot);
 }
 
 // planes per CTA: at most TD_AS_PPC, 1 under TD_FLAG_ONE_PLANE (ppc_max)
@@ -1225,11 +1287,14 @@ int launch_blend_async_ppc(const BlendParams& bp, const float* weights, const fl
 #endif
 int ppc_max(uint32_t flags) { return (flags & TD_FLAG_ONE_PLANE) ? 1 : TD_AS_PPC; }
 
-template <typename T, bool WRITE_BUF, bool FASTDIV>
+// SPARSE: one plane per CTA, never pipelined (the sparse entries take neither form)
+template <typename T, bool WRITE_BUF, bool FASTDIV, bool SPARSE = false>
 int launch_blend_async_impl(const BlendParams& bp, const float* weights, const float* rcp_weights, float* out_f32, void* out_buf,
-                            int nv_cap, bool pipelined, bool pdl, int max_ppc, cudaStream_t st) {
+                            int nv_cap, bool pipelined, bool pdl, int max_ppc, cudaStream_t st, const int* slot = nullptr) {
     constexpr int VEC = Vec<T>::kElems;
     constexpr int BX = kAsX * VEC;
+    if constexpr (SPARSE)
+        return launch_blend_async_ppc<T, WRITE_BUF, FASTDIV, 1, true>(bp, weights, rcp_weights, out_f32, out_buf, nv_cap, pdl, st, slot);
     const int px = (bp.g.W + BX - 1) / BX, py = (bp.g.H + kAsY - 1) / kAsY, planes = bp.g.N * bp.g.C;
     if (pipelined) {
         const int smem = 2 * nv_cap * kAsStage;
@@ -1265,9 +1330,9 @@ void schedule_halo_waits_last(BlendParams& bp) {
     bp.sched = (first_wait >= 0 && first_wait + last_wait <= mid2) ? 2 : 1;
 }
 
-template <typename T, bool WRITE_BUF>
+template <typename T, bool WRITE_BUF, bool SPARSE>
 int launch_blend_async(const td_grid* g, const BlendParams& bp_in, const float* weights, const float* rcp_weights, float* out_f32,
-                       void* out_buf, int nv_cap, bool pipelined, bool pdl, int max_ppc, cudaStream_t st) {
+                       void* out_buf, int nv_cap, bool pipelined, bool pdl, int max_ppc, cudaStream_t st, const int* slot) {
     constexpr int VEC = Vec<T>::kElems;
     constexpr int BX = kAsX * VEC;
     BlendParams bp = bp_in;
@@ -1275,27 +1340,29 @@ int launch_blend_async(const td_grid* g, const BlendParams& bp_in, const float* 
     fill_patch_table(g->xs, g->cols, g->tile_w, g->W, BX, bp.pcol_lo, bp.pcol_n);
     if (!pipelined) schedule_halo_waits_last(bp);
     if (rcp_weights != nullptr && sizeof(T) == 2)
-        return launch_blend_async_impl<T, WRITE_BUF, true>(bp, weights, rcp_weights, out_f32, out_buf, nv_cap, pipelined, pdl, max_ppc, st);
-    return launch_blend_async_impl<T, WRITE_BUF, false>(bp, weights, nullptr, out_f32, out_buf, nv_cap, pipelined, pdl, max_ppc, st);
+        return launch_blend_async_impl<T, WRITE_BUF, true, SPARSE>(bp, weights, rcp_weights, out_f32, out_buf, nv_cap, pipelined, pdl,
+                                                                   max_ppc, st, slot);
+    return launch_blend_async_impl<T, WRITE_BUF, false, SPARSE>(bp, weights, nullptr, out_f32, out_buf, nv_cap, pipelined, pdl, max_ppc, st,
+                                                                slot);
 }
 
-template <typename T, bool WINDOW>
+template <typename T, bool WINDOW, bool SPARSE = false>
 int launch_blend_mod_async(const BlendParams& bp, int smem, const float* tile_weights, const float* rescale, void* out_buf, bool pdl,
-                           cudaStream_t st) {
+                           cudaStream_t st, const int* slot = nullptr) {
     constexpr int BX = kAsX * Vec<T>::kElems;
     const char* what = "td_blend_mixture (cp.async)";
-    int rc = smem_optin(blend_mod_async_kernel<T, WINDOW>, smem, what);
+    int rc = smem_optin(blend_mod_async_kernel<T, WINDOW, SPARSE>, smem, what);
     if (rc != TD_OK) return rc;
     const unsigned gy = (unsigned)(WINDOW ? bp.py_count : (bp.g.H + kAsY - 1) / kAsY), gz = (unsigned)(bp.g.N * bp.g.C);
     dim3 grid((unsigned)((bp.g.W + BX - 1) / BX), bp.sched ? gz : gy, bp.sched ? gy : gz);
-    return launch(what, blend_mod_async_kernel<T, WINDOW>, grid, dim3(kAsThreads), (size_t)smem, st, pdl, bp, tile_weights, rescale,
-                  (T*)out_buf);
+    return launch(what, blend_mod_async_kernel<T, WINDOW, SPARSE>, grid, dim3(kAsThreads), (size_t)smem, st, pdl, bp, tile_weights, rescale,
+                  (T*)out_buf, slot);
 }
 
 // Mixture of Diffusers on the cp.async kernel; 0 launched, 1 not applicable, <0 error
-template <typename T>
+template <typename T, bool SPARSE = false>
 int try_launch_blend_mod_async(const td_grid* g, const BlendParams& bp_in, const float* tile_weights, const float* rescale, void* out_buf,
-                               bool pdl, cudaStream_t st) {
+                               bool pdl, cudaStream_t st, const int* slot = nullptr) {
     constexpr int VEC = Vec<T>::kElems;
     constexpr int BX = kAsX * VEC;
     if (bp_in.g.N * bp_in.g.C > 65535 || (bp_in.g.H + kAsY - 1) / kAsY > 65535 || bp_in.tile_stride >= (1ll << 31)) return 1;
@@ -1307,14 +1374,15 @@ int try_launch_blend_mod_async(const td_grid* g, const BlendParams& bp_in, const
     fill_patch_table(g->ys, g->rows, g->tile_h, g->H, kAsY, bp.prow_lo, bp.prow_n);
     fill_patch_table(g->xs, g->cols, g->tile_w, g->W, BX, bp.pcol_lo, bp.pcol_n);
     schedule_halo_waits_last(bp);
+    if constexpr (SPARSE) return launch_blend_mod_async<T, false, true>(bp, nv_cap * kAsStage, tile_weights, rescale, out_buf, pdl, st, slot);
     return bp.py_count > 0 ? launch_blend_mod_async<T, true>(bp, nv_cap * kAsStage, tile_weights, rescale, out_buf, pdl, st)
                            : launch_blend_mod_async<T, false>(bp, nv_cap * kAsStage, tile_weights, rescale, out_buf, pdl, st);
 }
 
 // returns TD_OK if launched, 1 if the path does not apply (caller falls back), <0 on error
-template <typename T>
+template <typename T, bool SPARSE = false>
 int try_launch_blend_async(const td_grid* g, const BlendParams& bp, const float* weights, const float* rcp_weights, float* out_f32,
-                           void* out_buf, bool pipelined, bool pdl, int max_ppc, cudaStream_t st) {
+                           void* out_buf, bool pipelined, bool pdl, int max_ppc, cudaStream_t st, const int* slot = nullptr) {
     constexpr int VEC = Vec<T>::kElems;
     constexpr int BX = kAsX * VEC;
     if (bp.g.N * bp.g.C > 65535 || (bp.g.H + kAsY - 1) / kAsY > 65535) return 1;
@@ -1323,25 +1391,26 @@ int try_launch_blend_async(const td_grid* g, const BlendParams& bp, const float*
     if (nv_cap <= 0 || nv_cap > kAsMaxVisits || nv_cap > kAsThreads || nv_cap * kAsStage > 200 * 1024) return 1;
     if ((bp.g.H + kAsY - 1) / kAsY > TD_MAX_GRID_DIM || (bp.g.W + BX - 1) / BX > TD_MAX_GRID_DIM) return 1;   // patch tables
     if (pipelined && 2 * nv_cap * kAsStage > 200 * 1024) pipelined = false;
-    return out_buf != nullptr ? launch_blend_async<T, true>(g, bp, weights, rcp_weights, out_f32, out_buf, nv_cap, pipelined, pdl, max_ppc, st)
-                              : launch_blend_async<T, false>(g, bp, weights, rcp_weights, out_f32, out_buf, nv_cap, pipelined, pdl, max_ppc, st);
+    return out_buf != nullptr
+               ? launch_blend_async<T, true, SPARSE>(g, bp, weights, rcp_weights, out_f32, out_buf, nv_cap, pipelined, pdl, max_ppc, st, slot)
+               : launch_blend_async<T, false, SPARSE>(g, bp, weights, rcp_weights, out_f32, out_buf, nv_cap, pipelined, pdl, max_ppc, st, slot);
 }
 
-template <typename TIn, typename TAcc, int MODE>
+template <typename TIn, typename TAcc, int MODE, bool SPARSE>
 int launch_blend_generic(const BlendParams& bp, const float* weights, const float* tile_weights, const float* rescale,
-                         float* out_f32, void* out_buf, cudaStream_t st) {
+                         float* out_f32, void* out_buf, cudaStream_t st, const int* slot) {
     const GeomParams& g = bp.g;
     const long long total = (long long)g.N * g.C * g.H * g.W;
-    blend_grid_generic_kernel<TIn, TAcc, MODE><<<blocks_for(total, 256), 256, 0, st>>>(bp, weights, tile_weights, rescale,
-                                                                                       out_f32, (TAcc*)out_buf, total);
+    blend_grid_generic_kernel<TIn, TAcc, MODE, SPARSE><<<blocks_for(total, 256), 256, 0, st>>>(bp, weights, tile_weights, rescale,
+                                                                                               out_f32, (TAcc*)out_buf, total, slot);
     return launch_status("td_blend (generic)");
 }
 
-template <int MODE>
+template <int MODE, bool SPARSE = false>
 int dispatch_generic(int tile_dtype, int acc_dtype, const BlendParams& bp, const float* w, const float* tw, const float* rs,
-                     float* out_f32, void* out_buf, cudaStream_t st) {
+                     float* out_f32, void* out_buf, cudaStream_t st, const int* slot = nullptr) {
 #define TD_CASE(TI, TA, TIn, TAcc) \
-    if (tile_dtype == TI && acc_dtype == TA) return launch_blend_generic<TIn, TAcc, MODE>(bp, w, tw, rs, out_f32, out_buf, st);
+    if (tile_dtype == TI && acc_dtype == TA) return launch_blend_generic<TIn, TAcc, MODE, SPARSE>(bp, w, tw, rs, out_f32, out_buf, st, slot);
     TD_CASE(TD_F16, TD_F16, __half, __half)
     TD_CASE(TD_F16, TD_BF16, __half, __nv_bfloat16)
     TD_CASE(TD_F16, TD_F32, __half, float)
@@ -1356,18 +1425,24 @@ int dispatch_generic(int tile_dtype, int acc_dtype, const BlendParams& bp, const
     return TD_ERR_INVALID_ARG;
 }
 
+// n_tiles: the tiles the batch table holds, the whole plan's by default (the sparse entries: the active tiles, possibly none -- then
+// num_batches is 0 and batch_ptrs may be null)
 int fill_blend(const td_grid* g, const void* const* batch_ptrs, int num_batches, int tile_bs, int N, int C, int tile_dtype,
-               int acc_dtype, BlendParams* bp) {
+               int acc_dtype, BlendParams* bp, int n_tiles = -1) {
     int st = fill_geom(g, N, C, &bp->g);
     if (st != TD_OK) return st;
+    if (n_tiles < 0) n_tiles = g->num_tiles;
     if (td_dtype_size(tile_dtype) == 0 || td_dtype_size(acc_dtype) == 0) { td_set_error("unknown dtype"); return TD_ERR_INVALID_ARG; }
-    if (batch_ptrs == nullptr || num_batches <= 0 || tile_bs <= 0) { td_set_error("bad batch pointer table"); return TD_ERR_INVALID_ARG; }
+    if (n_tiles == 0 ? (num_batches != 0 || tile_bs <= 0) : (batch_ptrs == nullptr || num_batches <= 0 || tile_bs <= 0)) {
+        td_set_error("bad batch pointer table");
+        return TD_ERR_INVALID_ARG;
+    }
     if (num_batches > TD_MAX_BATCH_PTRS) {
         td_set_error("%d batch tensors exceed TD_MAX_BATCH_PTRS=%d (concatenate them first)", num_batches, TD_MAX_BATCH_PTRS);
         return TD_ERR_UNSUPPORTED;
     }
-    if ((long long)num_batches * tile_bs < g->num_tiles || (long long)(num_batches - 1) * tile_bs >= g->num_tiles) {
-        td_set_error("batch table (%d x %d) does not cover %d tiles exactly", num_batches, tile_bs, g->num_tiles);
+    if ((long long)num_batches * tile_bs < n_tiles || (num_batches > 0 && (long long)(num_batches - 1) * tile_bs >= n_tiles)) {
+        td_set_error("batch table (%d x %d) does not cover %d tiles exactly", num_batches, tile_bs, n_tiles);
         return TD_ERR_INVALID_ARG;
     }
     for (int b = 0; b < num_batches; ++b) {
@@ -1718,4 +1793,140 @@ extern "C" int td_blend_mixture_wrap_rows(const td_grid* g, const void* const* b
     return wrap_rows_entry(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, 1, nullptr, tile_weights, rescale, nullptr,
                            x_buffer, row_begin, row_end, wait_flags, wait_count, wait_value, own_band_begin, own_band_end, flags, stream,
                            "td_blend_mixture_wrap_rows");
+}
+
+// ---------------------------------------------------------------------------
+// Inpainting: the tiles an inpaint mask reaches, and the blends over the compact batches of those tiles only.
+// ---------------------------------------------------------------------------
+namespace {
+
+// One CTA per tile: the tile is active when any element of its window, over all planes, is not exactly 1 (NaN included).
+template <typename T>
+__global__ void __launch_bounds__(256)
+active_tiles_kernel(const __grid_constant__ GeomParams g, const T* __restrict__ mask, int planes, uint8_t* __restrict__ active) {
+    const int t = blockIdx.x;
+    const int r = t / g.cols, c = t - r * g.cols;
+    const long long row0 = g.ys[r], col0 = g.xs[c];
+    const long long n = (long long)planes * g.th * g.tw;
+    int found = 0;
+    for (long long i = threadIdx.x; i < n && !found; i += blockDim.x) {
+        const long long pv = i / g.tw;                       // plane * th + v
+        const long long pl = pv / g.th, v = pv - pl * g.th, u = i - pv * g.tw;
+        found = !(Elem<T>::to_f32(mask[(pl * g.H + row0 + v) * g.W + col0 + u]) == 1.0f);
+    }
+    found = __syncthreads_or(found);
+    if (threadIdx.x == 0) active[t] = found ? 1 : 0;
+}
+
+// The slot table of a sparse blend: n_slots == T, every entry -1 or a position in the compact batches, the positions 0 .. K-1
+// each used exactly once (K = the tiles kept).  Checked on the host copy; the kernels read the device copy.
+int check_slots(const td_grid* g, const int32_t* slot_dev, const int32_t* slot_host, int n_slots, const char* what, int* n_active) {
+    if (g == nullptr) { td_set_error("%s: null grid", what); return TD_ERR_INVALID_ARG; }
+    if (slot_dev == nullptr || slot_host == nullptr || ((uintptr_t)slot_dev & 3u) != 0) {
+        td_set_error("%s: null or misaligned slot table", what);
+        return TD_ERR_INVALID_ARG;
+    }
+    if (g->num_tiles <= 0 || n_slots != g->num_tiles) {
+        td_set_error("%s: slot table of %d entries for a plan of %d tiles", what, n_slots, g->num_tiles);
+        return TD_ERR_INVALID_ARG;
+    }
+    int k = 0;
+    for (int t = 0; t < n_slots; ++t) k += slot_host[t] >= 0;
+    std::vector<unsigned char> seen((size_t)k, 0);
+    for (int t = 0; t < n_slots; ++t) {
+        const int s = slot_host[t];
+        if (s < -1 || s >= k || (s >= 0 && seen[(size_t)s])) {
+            td_set_error("%s: slot[%d] = %d is not -1 or an unused position below %d", what, t, s, k);
+            return TD_ERR_INVALID_ARG;
+        }
+        if (s >= 0) seen[(size_t)s] = 1;
+    }
+    *n_active = k;
+    return TD_OK;
+}
+
+// the sparse entries have the default cp.async form and the generic one: other form flags are refused
+constexpr uint32_t kSparseFlags = TD_FLAG_FORCE_GENERIC | TD_FLAG_NO_PDL | TD_FLAG_ONE_PLANE;
+
+int sparse_common(const td_grid* g, const void* const* batch_ptrs, int num_batches, int tile_bs, int N, int C, int tile_dtype,
+                  int acc_dtype, const int32_t* slot_dev, const int32_t* slot_host, int n_slots, uint32_t flags, const char* what,
+                  BlendParams* bp) {
+    int k = 0;
+    int st = check_slots(g, slot_dev, slot_host, n_slots, what, &k);
+    if (st != TD_OK) return st;
+    if ((st = fill_blend(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, bp, k)) != TD_OK) return st;
+    if (g->wrap != 0) { td_set_error("%s: no form for a periodic plan (wrap=%d)", what, g->wrap); return TD_ERR_UNSUPPORTED; }
+    if (flags & ~kSparseFlags) { td_set_error("%s: flags %#x name a form this entry does not have", what, flags); return TD_ERR_INVALID_ARG; }
+    return TD_OK;
+}
+
+}  // namespace
+
+extern "C" int td_grid_active_tiles(const td_grid* g, const void* mask, int planes, int dtype, uint8_t* active_dev, void* stream) {
+    GeomParams gp;
+    int st = fill_geom(g, 1, 1, &gp);
+    if (st != TD_OK) return st;
+    if (g->wrap != 0) { td_set_error("td_grid_active_tiles: no form for a periodic plan (wrap=%d)", g->wrap); return TD_ERR_UNSUPPORTED; }
+    const int es = td_dtype_size(dtype);
+    if (es == 0) { td_set_error("td_grid_active_tiles: unknown dtype %d", dtype); return TD_ERR_INVALID_ARG; }
+    if (planes <= 0) { td_set_error("td_grid_active_tiles: planes = %d must be positive", planes); return TD_ERR_INVALID_ARG; }
+    if (mask == nullptr || active_dev == nullptr || ((uintptr_t)mask % (uintptr_t)es) != 0) {
+        td_set_error("td_grid_active_tiles: null or misaligned mask / output");
+        return TD_ERR_INVALID_ARG;
+    }
+    cudaStream_t s = (cudaStream_t)stream;
+    switch (dtype) {
+        case TD_F16: active_tiles_kernel<__half><<<g->num_tiles, 256, 0, s>>>(gp, (const __half*)mask, planes, active_dev); break;
+        case TD_BF16: active_tiles_kernel<__nv_bfloat16><<<g->num_tiles, 256, 0, s>>>(gp, (const __nv_bfloat16*)mask, planes, active_dev); break;
+        default: active_tiles_kernel<float><<<g->num_tiles, 256, 0, s>>>(gp, (const float*)mask, planes, active_dev); break;
+    }
+    return launch_status("td_grid_active_tiles");
+}
+
+extern "C" int td_blend_multidiffusion_sparse(const td_grid* g, const void* const* batch_ptrs, int num_batches, int tile_bs, int N, int C,
+                                              int tile_dtype, int acc_dtype, const float* weights, const float* rcp_weights, float* x_out,
+                                              void* x_buffer, const int32_t* slot_dev, const int32_t* slot_host, int n_slots,
+                                              uint32_t flags, void* stream) {
+    const char* what = "td_blend_multidiffusion_sparse";
+    BlendParams bp;
+    int st = sparse_common(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, slot_dev, slot_host, n_slots, flags, what, &bp);
+    if (st != TD_OK) return st;
+    if (weights == nullptr || x_out == nullptr) { td_set_error("%s: null weights / x_out", what); return TD_ERR_INVALID_ARG; }
+    const bool pdl = !(flags & TD_FLAG_NO_PDL);
+    cudaStream_t s = (cudaStream_t)stream;
+    if (!(flags & TD_FLAG_FORCE_GENERIC) && blend_vec_ok(bp, tile_dtype, acc_dtype, {weights, rcp_weights, x_out, x_buffer})) {
+        int rc;
+        switch (tile_dtype) {
+            case TD_F16: rc = try_launch_blend_async<__half, true>(g, bp, weights, rcp_weights, x_out, x_buffer, false, pdl, 1, s, slot_dev); break;
+            case TD_BF16: rc = try_launch_blend_async<__nv_bfloat16, true>(g, bp, weights, rcp_weights, x_out, x_buffer, false, pdl, 1, s, slot_dev); break;
+            default: rc = try_launch_blend_async<float, true>(g, bp, weights, nullptr, x_out, x_buffer, false, pdl, 1, s, slot_dev); break;
+        }
+        if (rc <= 0) return rc;   // launched or hard error; 1 = outside the cp.async kernel's limits -> generic kernel
+    }
+    return dispatch_generic<MODE_MD, true>(tile_dtype, acc_dtype, bp, weights, nullptr, nullptr, x_out, x_buffer, s, slot_dev);
+}
+
+extern "C" int td_blend_mixture_sparse(const td_grid* g, const void* const* batch_ptrs, int num_batches, int tile_bs, int N, int C,
+                                       int tile_dtype, int acc_dtype, const float* tile_weights, const float* rescale, void* x_buffer,
+                                       const int32_t* slot_dev, const int32_t* slot_host, int n_slots, uint32_t flags, void* stream) {
+    const char* what = "td_blend_mixture_sparse";
+    BlendParams bp;
+    int st = sparse_common(g, batch_ptrs, num_batches, tile_bs, N, C, tile_dtype, acc_dtype, slot_dev, slot_host, n_slots, flags, what, &bp);
+    if (st != TD_OK) return st;
+    if (tile_weights == nullptr || rescale == nullptr || x_buffer == nullptr) {
+        td_set_error("%s: null tile_weights / rescale / x_buffer", what);
+        return TD_ERR_INVALID_ARG;
+    }
+    const bool pdl = !(flags & TD_FLAG_NO_PDL);
+    cudaStream_t s = (cudaStream_t)stream;
+    if (!(flags & TD_FLAG_FORCE_GENERIC) && blend_vec_ok(bp, tile_dtype, acc_dtype, {rescale, x_buffer})) {
+        int rc;
+        switch (tile_dtype) {
+            case TD_F16: rc = try_launch_blend_mod_async<__half, true>(g, bp, tile_weights, rescale, x_buffer, pdl, s, slot_dev); break;
+            case TD_BF16: rc = try_launch_blend_mod_async<__nv_bfloat16, true>(g, bp, tile_weights, rescale, x_buffer, pdl, s, slot_dev); break;
+            default: rc = try_launch_blend_mod_async<float, true>(g, bp, tile_weights, rescale, x_buffer, pdl, s, slot_dev); break;
+        }
+        if (rc <= 0) return rc;
+    }
+    return dispatch_generic<MODE_MOD, true>(tile_dtype, acc_dtype, bp, nullptr, tile_weights, rescale, nullptr, x_buffer, s, slot_dev);
 }

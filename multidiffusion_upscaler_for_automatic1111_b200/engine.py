@@ -26,6 +26,15 @@ def make_grid(w: int, h: int, tile_w: int, tile_h: int, overlap: int, tile_bs: i
     return g
 
 
+def rect_grid(w: int, h: int, x: int, y: int, rect_w: int, rect_h: int) -> TdGrid:
+    """A one-tile plan whose tile is the rectangle (x, y, rect_w, rect_h) of a w x h canvas (a custom region for `active_tiles`)."""
+    g = TdGrid()
+    g.H, g.W, g.tile_h, g.tile_w, g.overlap = int(h), int(w), int(rect_h), int(rect_w), 0
+    g.rows = g.cols = g.num_tiles = g.num_batches = g.tile_bs = 1
+    g.ys[0], g.xs[0] = int(y), int(x)
+    return g
+
+
 def grid_bboxes_xywh(g: TdGrid) -> np.ndarray:
     """int32 [T,4] (x, y, w, h) in tile-list order (row outer, col inner)."""
     xs = np.ctypeslib.as_array(g.xs)[:g.cols]
@@ -220,6 +229,90 @@ def blend_mixture(g: TdGrid, batch_outs: Sequence[torch.Tensor], N: int, C: int,
         check(lib.td_blend_mixture(ctypes.byref(g), ptrs, len(keep), int(tile_bs), N, C, dtype_code(tdt),
                                    dtype_code(x_buffer.dtype), tile_weights.data_ptr(), rescale.data_ptr(),
                                    x_buffer.data_ptr(), int(flags), current_stream_ptr(dev)))
+    return x_buffer
+
+
+def active_tiles(g: TdGrid, mask: torch.Tensor) -> np.ndarray:
+    """bool [T]: the tiles of plan g whose window holds at least one mask element, over all leading planes, that is not exactly
+    1.0 (NaN included).  mask: the WebUI's latent inpaint mask (1 = keep the original), [h, w], [C, h, w] or [N, C, h, w] on
+    the device, in fp16, bf16 or fp32 (td_grid_active_tiles, one launch; the T flags are read back here)."""
+    _require_cuda(mask, "mask")
+    if mask.dim() not in (2, 3, 4) or tuple(mask.shape[-2:]) != (g.H, g.W):
+        raise ValueError(f"mask shape {tuple(mask.shape)} does not match the plan's canvas {(g.H, g.W)}")
+    m = mask.contiguous()
+    planes = m.numel() // (g.H * g.W)
+    out = torch.empty(g.num_tiles, dtype=torch.uint8, device=m.device)
+    with torch.cuda.device(m.device):
+        check(lib.td_grid_active_tiles(ctypes.byref(g), m.data_ptr(), int(planes), dtype_code(m.dtype), out.data_ptr(),
+                                       current_stream_ptr(m.device)))
+    return out.cpu().numpy().astype(bool)
+
+
+def slot_table(active: np.ndarray) -> np.ndarray:
+    """int32 [T]: each active tile's position in the compact tile batches (active tiles in tile order), -1 for a skipped tile."""
+    active = np.asarray(active, dtype=bool)
+    slot = np.full(active.shape[0], -1, dtype=np.int32)
+    slot[active] = np.arange(int(active.sum()), dtype=np.int32)
+    return slot
+
+
+def _sparse_table(g: TdGrid, batch_outs: Sequence[torch.Tensor], N: int, C: int, tile_bs: int, slot_dev: torch.Tensor,
+                  slot_host: np.ndarray):
+    """The compact batch table of a sparse blend (concatenated above TD_MAX_BATCH_PTRS batches, as the dense blends do)."""
+    slot_host = np.ascontiguousarray(slot_host, dtype=np.int32)
+    if slot_host.shape != (g.num_tiles,):
+        raise ValueError(f"slot table of shape {slot_host.shape} for a plan of {g.num_tiles} tiles")
+    _require_cuda(slot_dev, "slot table")
+    if slot_dev.dtype != torch.int32 or slot_dev.numel() != g.num_tiles or not slot_dev.is_contiguous():
+        raise ValueError(f"the device slot table must be a contiguous int32 tensor of {g.num_tiles} elements")
+    n_active = int((slot_host >= 0).sum())
+    batch_outs, tile_bs = _fit_batch_table(g, batch_outs, tile_bs)
+    keep, dt = [], None
+    for b, t in enumerate(batch_outs):
+        _require_cuda(t, "tile output")
+        want = (min(tile_bs, n_active - b * tile_bs) * N, C, g.tile_h, g.tile_w)
+        if tuple(t.shape) != want:
+            raise ValueError(f"compact tile batch {b} has shape {tuple(t.shape)}, expected {want}")
+        dt = t.dtype if dt is None else dt
+        keep.append(t.to(dt).contiguous())
+    ptrs = (ctypes.c_void_p * max(1, len(keep)))(*[t.data_ptr() for t in keep])
+    return ptrs, keep, tile_bs, slot_host
+
+
+def blend_multidiffusion_sparse(g: TdGrid, batch_outs: Sequence[torch.Tensor], N: int, C: int, tile_bs: int, weights: torch.Tensor,
+                                acc_dtype: torch.dtype, slot_dev: torch.Tensor, slot_host: np.ndarray,
+                                x_buffer: Optional[torch.Tensor] = None, flags: int = 0, rcp_weights: Optional[torch.Tensor] = None,
+                                tile_dtype: Optional[torch.dtype] = None) -> torch.Tensor:
+    """`blend_multidiffusion` over the active tiles only: batch_outs hold them in tile order (compact batches of tile_bs), slot the
+    tile -> compact position table of `slot_table`.  `tile_dtype` names the tile dtype when there is no batch (no active tile).
+    Returns a fresh fp32 [N,C,H,W] (td_blend_multidiffusion_sparse)."""
+    ptrs, keep, tile_bs, slot_host = _sparse_table(g, batch_outs, N, C, tile_bs, slot_dev, slot_host)
+    tdt = keep[0].dtype if keep else (tile_dtype or acc_dtype)
+    dev = weights.device
+    x_out = torch.empty((N, C, g.H, g.W), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        check(lib.td_blend_multidiffusion_sparse(ctypes.byref(g), ptrs, len(keep), int(tile_bs), N, C, dtype_code(tdt), dtype_code(acc_dtype),
+                                                 weights.data_ptr(), rcp_weights.data_ptr() if rcp_weights is not None else None,
+                                                 x_out.data_ptr(), x_buffer.data_ptr() if x_buffer is not None else None,
+                                                 slot_dev.data_ptr(), slot_host.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)),
+                                                 int(slot_host.shape[0]), int(flags), current_stream_ptr(dev)))
+    return x_out
+
+
+def blend_mixture_sparse(g: TdGrid, batch_outs: Sequence[torch.Tensor], N: int, C: int, tile_bs: int, tile_weights: torch.Tensor,
+                         rescale: torch.Tensor, x_buffer: torch.Tensor, slot_dev: torch.Tensor, slot_host: np.ndarray, flags: int = 0,
+                         tile_dtype: Optional[torch.dtype] = None) -> torch.Tensor:
+    """`blend_mixture` over the active tiles only (see `blend_multidiffusion_sparse`); writes and returns x_buffer
+    (td_blend_mixture_sparse)."""
+    _require_cuda(x_buffer, "x_buffer")
+    ptrs, keep, tile_bs, slot_host = _sparse_table(g, batch_outs, N, C, tile_bs, slot_dev, slot_host)
+    tdt = keep[0].dtype if keep else (tile_dtype or x_buffer.dtype)
+    dev = x_buffer.device
+    with torch.cuda.device(dev):
+        check(lib.td_blend_mixture_sparse(ctypes.byref(g), ptrs, len(keep), int(tile_bs), N, C, dtype_code(tdt), dtype_code(x_buffer.dtype),
+                                          tile_weights.data_ptr(), rescale.data_ptr(), x_buffer.data_ptr(), slot_dev.data_ptr(),
+                                          slot_host.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), int(slot_host.shape[0]), int(flags),
+                                          current_stream_ptr(dev)))
     return x_buffer
 
 

@@ -16,10 +16,12 @@ What differs from the reference by design:
 """
 from __future__ import annotations
 
+import ctypes
 import math
 from types import MethodType
 from typing import Callable, Dict, List, Optional, Tuple, Union
 
+import numpy as np
 import torch
 from torch import Tensor
 
@@ -29,6 +31,30 @@ from ..tile_utils.utils import (BBox, BlendMode, Condition, CustomBBox, Prompt, 
                                 grid_bbox, keep_signature, noise_inverse, controlnet, stablesr)
 
 CondDict = Dict[str, Union[Tensor, List[Tensor]]]
+
+_MASK_DTYPES = (torch.float16, torch.bfloat16, torch.float32)
+
+
+class InpaintPlan:
+    """What `init_inpaint_mask` leaves on a delegate: the grid tiles and custom regions the inpaint mask reaches and the compact
+    tile batches of the sampler loop (active tiles in tile order, `tile_bs` per batch)."""
+
+    def __init__(self, g, active: np.ndarray, regions: List[bool], tile_bs: int, device):
+        self.active = active                                   # bool [T]
+        self.tiles = [int(t) for t in np.flatnonzero(active)]  # active tile indices, ascending
+        self.slot_host = engine.slot_table(active)             # int32 [T]: compact position or -1
+        self.slot_dev = torch.from_numpy(self.slot_host).to(device)
+        xywh = engine.grid_bboxes_xywh(g) if g is not None else np.zeros((0, 4), dtype=np.int32)
+        bboxes = [BBox(*(int(v) for v in xywh[t])) for t in self.tiles]
+        self.batched_bboxes = [bboxes[i:i + tile_bs] for i in range(0, len(bboxes), tile_bs)]
+        flat = [int(v) for t in self.tiles for v in xywh[t, :2]]          # (x, y) per active tile
+        self.origins_host = (ctypes.c_int32 * max(1, len(flat)))(*flat)
+        self.origins_dev = torch.tensor(flat, dtype=torch.int32, device=device)
+        self.regions = regions                                 # per custom region: denoised (True) or skipped
+
+    @property
+    def num_tiles(self) -> int:
+        return len(self.tiles)
 
 
 class AbstractDiffusion:
@@ -116,6 +142,8 @@ class AbstractDiffusion:
         self._strip = None
         self._strip_exchange = None
         self._region_shard = None             # parallel.RegionShard: custom regions under the tile shard
+        self._inpaint: Optional[InpaintPlan] = None   # init_inpaint_mask: the tiles and regions the sampler loop denoises
+        self._full_plan_pass = False          # tiled noise inversion: every tile and region, whatever the inpaint mask
 
     # ----------------------------------------------------------------- helpers
     def _sd_model(self):
@@ -160,6 +188,9 @@ class AbstractDiffusion:
         if self.enable_custom_bbox:
             self.total_bboxes += len(self.custom_bboxes)
         assert self.total_bboxes > 0, "Nothing to paint! No background to draw and no custom bboxes were provided."
+        if self._inpaint is not None:       # progress counts the denoiser calls the sampler loop makes
+            self.total_bboxes = (len(self._inpaint.batched_bboxes) if self.enable_grid_bbox else 0) + \
+                (sum(self._inpaint.regions) if self.enable_custom_bbox else 0)
         self.pbar = None
         if getattr(self.p, "show_tile_progress", False):
             from tqdm import tqdm
@@ -260,6 +291,57 @@ class AbstractDiffusion:
     def get_tile_weights(self) -> Union[Tensor, float]:
         return 1.0
 
+    # ------------------------------------------------------------- inpainting
+    def init_inpaint_mask(self, mask: Tensor):
+        """Denoise only the grid tiles and custom regions the inpaint mask reaches.  Call after init_grid_bbox / init_custom_bbox
+        and before init_done.
+
+        `mask` is the WebUI's latent mask `p.mask` (1 = keep the original): [h, w], [C, h, w] or [N, C, h, w], fp16 / bf16 /
+        fp32, on the device.  A tile (region) is active when at least one mask element in its window (rectangle), over all
+        leading planes, is not exactly 1.0 -- NaN included.  The other tiles cannot change a pixel the host keeps: their windows
+        lie in the kept area, which the host overwrites with the original after every denoiser call.  The weight canvas and the
+        Mixture of Diffusers rescale factor stay those of the full plan, so on every pixel with mask < 1 the step computes what
+        the full plan computes, visiting the same tiles in the same order.  A mask that keeps everything leaves nothing to
+        denoise: the step then returns the blend of nothing (zeros).  Tiled noise inversion (`get_noise`) still runs every tile.
+
+        With a UNet whose output for one sample depends on the batch it runs in, results differ in the last bits, as they do
+        for another tile_bs: the active tiles are batched differently."""
+        self._refuse_inpaint()
+        if not isinstance(mask, Tensor) or mask.dim() not in (2, 3, 4) or tuple(mask.shape[-2:]) != (self.h, self.w):
+            raise ValueError(f"{self.method}: the inpaint mask must be [h, w], [C, h, w] or [N, C, h, w] with (h, w) = {(self.h, self.w)}, "
+                             f"got {tuple(mask.shape) if isinstance(mask, Tensor) else type(mask).__name__}")
+        if mask.dtype not in _MASK_DTYPES:
+            raise ValueError(f"{self.method}: the inpaint mask must be fp16, bf16 or fp32, got {mask.dtype}")
+        grid = self._grid if self.enable_grid_bbox else None
+        active = engine.active_tiles(grid, mask) if grid is not None else np.zeros(0, dtype=bool)
+        regions = [bool(engine.active_tiles(engine.rect_grid(self.w, self.h, b.x, b.y, b.w, b.h), mask)[0]) for b in self.custom_bboxes]
+        self._inpaint = InpaintPlan(grid, active, regions, self.tile_bs or 1, mask.device)
+        # side-input caches built before this call hold the full plan's tiles
+        if self.control_tensor_batch is not None:
+            self.prepare_controlnet_tensors(refresh=True)
+        if self.stablesr_tensor is not None:
+            self.stablesr_tensor_batch, _ = self._side_input_tiles(self.stablesr_tensor, 1, False)
+
+    def _refuse_inpaint(self):
+        """NotImplementedError for a plan init_inpaint_mask has no form for (raised before any state changes)."""
+        if self._grid is not None and self._grid.wrap:
+            raise NotImplementedError(f"{self.method}: init_inpaint_mask() does not take a wrapped plan (wrap_x / wrap_y)")
+        if self._shard is not None:
+            raise NotImplementedError(f"{self.method}: init_inpaint_mask() does not run under the multi-GPU tile shard")
+
+    def _active_plan(self) -> Optional[InpaintPlan]:
+        """The inpaint plan the sampler loop runs, or None for the full plan."""
+        return None if self._full_plan_pass else self._inpaint
+
+    def _region_skipped(self, bbox_id: int) -> bool:
+        ip = self._active_plan()
+        return ip is not None and not ip.regions[bbox_id]
+
+    def _scatter_active(self, x: Tensor, ip: InpaintPlan) -> Tensor:
+        """The active tiles of x, compact and in tile order (td_scatter_bboxes: the same copy as td_scatter_tiles)."""
+        self._tiles = engine.scatter_bboxes(x, ip.origins_dev, ip.origins_host, ip.num_tiles, self.tile_h, self.tile_w, out=self._tiles)
+        return self._tiles
+
     # ------------------------------------------------------------- multi-GPU
     def init_tile_shard(self, group=None, fused: bool = True, mode: Optional[str] = None):
         """Shard the tiles over the ranks of `group` (one process per GPU).  Call after init_grid_bbox.
@@ -282,6 +364,8 @@ class AbstractDiffusion:
         wrap_y the strips close into a ring (StripShard(wrap_y=True)); both modes stay bit-identical to one GPU."""
         import torch.distributed as dist
         from .. import parallel
+        if self._inpaint is not None:
+            raise NotImplementedError(f"{self.method}: init_tile_shard() does not run with an inpaint mask (init_inpaint_mask)")
         if self._grid is None and not self.enable_custom_bbox:
             raise RuntimeError("init_tile_shard() must follow init_grid_bbox() or init_custom_bbox()")
         if self._grid is not None and self._grid.wrap and mode is None:
@@ -599,6 +683,8 @@ class AbstractDiffusion:
         done = []
         use_networks = not getattr(self.p, "disable_extra_networks", False)
         for bbox_id, bbox in enumerate(self.custom_bboxes):
+            if self._region_skipped(bbox_id):     # inpaint mask: the region lies in the kept area, it and its composite terms drop out
+                continue
             if poll_interrupt and host.interrupted():
                 return self._INTERRUPTED
             if use_networks:
@@ -776,9 +862,10 @@ class AbstractDiffusion:
         raise NotImplementedError
 
     # ------------------------------------ side-input tile caches (ControlNet, StableSR)
-    def _crop_side_input(self, t: Tensor, scale: int) -> Tensor:
+    def _crop_side_input(self, t: Tensor, scale: int, ip: Optional[InpaintPlan] = None) -> Tensor:
         """Every grid tile of a side input [B, C, H*scale, W*scale] in one scatter launch: [T*B, C, th*scale, tw*scale],
-        tile-major -- what the reference builds with T slice views and one `cat` per batch (abstractdiffusion.py:494-503)."""
+        tile-major -- what the reference builds with T slice views and one `cat` per batch (abstractdiffusion.py:494-503).
+        With an inpaint plan `ip`: its active tiles only, compact, in tile order."""
         dev = host.device()
         if t.device != dev:
             t = t.to(dev)
@@ -793,20 +880,31 @@ class AbstractDiffusion:
             # canvas (p.width not a multiple of 8, hints resized by the extension: the reference's slicing tolerates
             # both, abstractdiffusion.py:494-503): plain slicing, same tile order
             s = scale
-            return torch.cat([t[:, :, b[1] * s:b[3] * s, b[0] * s:b[2] * s] for batch in self.batched_bboxes for b in batch], dim=0)
+            batches = self.batched_bboxes if ip is None else ip.batched_bboxes
+            return torch.cat([t[:, :, b[1] * s:b[3] * s, b[0] * s:b[2] * s] for batch in batches for b in batch], dim=0)
+        if ip is not None:
+            origins = ip.origins_dev * scale
+            host_origins = (ctypes.c_int32 * len(ip.origins_host))(*[v * scale for v in ip.origins_host])
+            return engine.scatter_bboxes(t.contiguous(), origins, host_origins, ip.num_tiles, self._grid.tile_h * scale,
+                                         self._grid.tile_w * scale)
         g = self._grid if scale == 1 else engine.scaled_grid(self._grid, scale)
         return engine.scatter_tiles(g, t.contiguous(), flags=self._blend_flags)
 
-    def _batch_rows(self, tiles: Tensor, batch_id: int, rows_per_tile: int) -> Tensor:
+    def _batch_rows(self, tiles: Tensor, batch_id: int, rows_per_tile: int, num_tiles: Optional[int] = None) -> Tensor:
         lo = batch_id * self.tile_bs * rows_per_tile
-        hi = min((batch_id + 1) * self.tile_bs, self.num_tiles) * rows_per_tile
+        hi = min((batch_id + 1) * self.tile_bs, self.num_tiles if num_tiles is None else num_tiles) * rows_per_tile
         return tiles[lo:hi]
 
     def _side_input_tiles(self, full: Tensor, scale: int, park_on_cpu: bool):
         """(per tile batch, per custom region) crops of one side input living at `scale` x the latent resolution."""
         park = (lambda t: t.cpu()) if park_on_cpu else (lambda t: t)
         per_batch, per_region = [], []
-        if self.batched_bboxes:
+        ip = self._inpaint
+        if ip is not None and self.batched_bboxes:      # inpaint mask: the active tiles only, in the compact batches of the loop
+            if ip.batched_bboxes:
+                tiles = self._crop_side_input(full, scale, ip)
+                per_batch = [park(self._batch_rows(tiles, b, full.shape[0], ip.num_tiles)) for b in range(len(ip.batched_bboxes))]
+        elif self.batched_bboxes:
             tiles = self._crop_side_input(full, scale)
             rows = full.shape[0]
             per_batch = [park(self._batch_rows(tiles, b, rows)) for b in range(len(self.batched_bboxes))]
@@ -866,12 +964,21 @@ class AbstractDiffusion:
         replicates the latent (abstractdiffusion.py:520-535): k-diffusion keeps the x_batch_size copies of a tile
         adjacent, the DDIM family repeats the whole tile batch (twice more when cond and uncond run together)."""
         for unit_id, unit in enumerate(self._control_params()):
-            crops = self.control_tensor_batch[unit_id][batch_id]
+            crops = self._side_batch(self.control_tensor_batch[unit_id], self.org_control_tensor_batch[unit_id], opt_f, batch_id)
             if self.is_kdiff:
                 crops = crops[:tile_batch_size].repeat_interleave(x_batch_size, dim=0)
             else:
                 crops = crops.repeat([x_batch_size * (1 if is_denoise else 2), 1, 1, 1])
             unit.hint_cond = crops.to(host.device())
+
+    def _side_batch(self, per_batch: list, full: Tensor, scale: int, batch_id: int) -> Tensor:
+        """A side input's crops for tile batch `batch_id` of the loop that runs.  The caches hold the inpaint plan's active tiles;
+        the full-plan pass of noise inversion crops its batch from the whole side input instead."""
+        if self._inpaint is None or not self._full_plan_pass:
+            return per_batch[batch_id]
+        bboxes = self.batched_bboxes[batch_id]
+        s = scale
+        return torch.cat([full[:, :, b.y * s:(b.y + b.h) * s, b.x * s:(b.x + b.w) * s] for b in bboxes], dim=0)
 
     @controlnet
     def set_custom_controlnet_tensors(self, bbox_id: int, repeat_size: int):
@@ -914,7 +1021,7 @@ class AbstractDiffusion:
     def switch_stablesr_tensors(self, batch_id: int):
         model = self._stablesr_model()
         if model is not None and self.stablesr_tensor_batch is not None:
-            model.latent_image = self.stablesr_tensor_batch[batch_id]
+            model.latent_image = self._side_batch(self.stablesr_tensor_batch, self.stablesr_tensor, 1, batch_id)
 
     @stablesr
     def set_custom_stablesr_tensors(self, bbox_id: int):

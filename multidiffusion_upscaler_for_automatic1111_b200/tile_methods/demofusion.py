@@ -206,6 +206,9 @@ class DemoFusion(AbstractDiffusion):
         if self._shard_on:
             self._derive_shards()
 
+    def init_inpaint_mask(self, *args, **kwargs):
+        raise NotImplementedError("DemoFusion does not support the inpaint mask: its global views cover the whole canvas")
+
     # ------------------------------------------------------------------ multi-GPU
     def init_tile_shard(self, group=None, fused: bool = False):
         """Shard the local windows AND the s*s global views over the ranks of `group` (one process per GPU): contiguous

@@ -129,8 +129,8 @@ class MixtureOfDiffusers(AbstractDiffusion):
         # mixtureofdiffusers.py:145-175 in one launch: BACKGROUND adds weighted by the pre-rescaled custom weights, no
         # normalisation, FOREGROUND feather overlay
         out = self._composite_regions(self.x_buffer, None, done, background_aux=lambda bbox_id: self.custom_weights[bbox_id])
-        if any(b.blend_mode == BlendMode.FOREGROUND for _, b, _ in done):
-            return out                       # the reference's overlay promotes to fp32 (fp32 mask)
+        if any(b.blend_mode == BlendMode.FOREGROUND for b in self.custom_bboxes):
+            return out                       # the reference's overlay promotes to fp32 (fp32 mask; so also when the inpaint mask skips it)
         self.x_buffer.copy_(out)             # BACKGROUND only: the reference returns x_buffer itself (x_in.dtype; lossless)
         return self.x_buffer
 
@@ -159,6 +159,9 @@ class MixtureOfDiffusers(AbstractDiffusion):
         if self._shard is not None:
             return self._grid_pass_sharded(x, t_in, c_in, sd_model, N, C)
 
+        ip = self._active_plan()
+        if ip is not None:
+            return self._grid_pass_active(ip, x, t_in, c_in, sd_model, N, C)
         tiles = self._scatter_all(x)
         icond_tiles = None
         if isinstance(c_in, dict):
@@ -179,6 +182,32 @@ class MixtureOfDiffusers(AbstractDiffusion):
 
         return engine.blend_mixture(self._grid, outs, N, C, self.tile_bs, self.tile_weights, self.rescale_factor,
                                     self.x_buffer, flags=self._blend_flags)
+
+    def _grid_pass_active(self, ip, x: Tensor, t_in: Tensor, c_in: CondDict, sd_model, N: int, C: int):
+        """`_grid_pass` under an inpaint mask: the active tiles in compact batches (latent and spatial image cond through the list
+        scatter), then the sparse gaussian blend, which drops the skipped tiles' visits.  Returns x_buffer, or None when
+        interrupted."""
+        outs = []
+        if ip.num_tiles:
+            tiles = self._scatter_active(x, ip)
+            icond_tiles, n_icond = None, 0
+            if isinstance(c_in, dict):
+                icond_full = self.get_icond(c_in)
+                if tuple(icond_full.shape[2:]) == (self.h, self.w):
+                    icond_tiles = engine.scatter_bboxes(icond_full.contiguous(), ip.origins_dev, ip.origins_host, ip.num_tiles,
+                                                        self.tile_h, self.tile_w)
+                    n_icond = icond_full.shape[0]
+            off = 0
+            for batch_id, bboxes in enumerate(ip.batched_bboxes):
+                if host.interrupted():
+                    return None
+                n_rep = len(bboxes)
+                icond_tile = icond_tiles[off * n_icond:(off + n_rep) * n_icond] if icond_tiles is not None else None
+                outs.append(self._denoise_tile_batch(sd_model, tiles[off * N:(off + n_rep) * N], n_rep, t_in, c_in, icond_tile, batch_id, N))
+                off += n_rep
+                self.update_pbar()
+        return engine.blend_mixture_sparse(self._grid, outs, N, C, self.tile_bs, self.tile_weights, self.rescale_factor, self.x_buffer,
+                                           ip.slot_dev, ip.slot_host, flags=self._blend_flags, tile_dtype=x.dtype)
 
     def _blend_inputs_to(self, device):
         if self.rescale_factor.device != device:
@@ -292,4 +321,9 @@ class MixtureOfDiffusers(AbstractDiffusion):
 
     @torch.no_grad()
     def get_noise(self, x_in: Tensor, sigma_in: Tensor, cond_in: CondDict, step: int) -> Tensor:
-        return self.apply_model_hijack(x_in, sigma_in, cond=cond_in, noise_inverse_step=step)
+        # the inverted latent is the full plan's: there is no host mask here, and an active tile reads kept pixels too
+        self._full_plan_pass = True
+        try:
+            return self.apply_model_hijack(x_in, sigma_in, cond=cond_in, noise_inverse_step=step)
+        finally:
+            self._full_plan_pass = False

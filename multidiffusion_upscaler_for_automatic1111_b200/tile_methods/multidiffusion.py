@@ -10,6 +10,7 @@ kernel (pointer table, no concatenation copy).
 """
 from __future__ import annotations
 
+import ctypes
 from typing import Callable, List, Optional, Union
 
 import torch
@@ -128,7 +129,12 @@ class MultiDiffusion(AbstractDiffusion):
         return (id(t), t._version, id(i), i._version, None if v is None else (id(v), v._version))
 
     def _crop_icond(self, icond: Tensor, bboxes: List[BBox]) -> Tensor:
-        """Spatial icond -> tile batch with the same scatter kernel as the latent."""
+        """Spatial icond -> tile batch with the same scatter kernel as the latent (a batch of the inpaint plan's active tiles need
+        not be a contiguous tile range: its windows go through the list scatter)."""
+        if self._active_plan() is not None:
+            flat = [v for b in bboxes for v in (b.x, b.y)]
+            return engine.scatter_bboxes(icond.contiguous(), torch.tensor(flat, dtype=torch.int32, device=icond.device),
+                                         (ctypes.c_int32 * len(flat))(*flat), len(bboxes), self.tile_h, self.tile_w)
         first = self._bbox_index(bboxes[0])
         return engine.scatter_tiles(self._grid, icond, tile_begin=first, tile_end=first + len(bboxes),
                                     flags=self._blend_flags)
@@ -158,7 +164,31 @@ class MultiDiffusion(AbstractDiffusion):
             return self._sample_one_step_sharded(x_in, x, repeat_func, custom_func if regions else None, N, C)
 
         x_out = None
-        if self.enable_grid_bbox:
+        ip = self._active_plan()
+        if self.enable_grid_bbox and ip is not None:
+            # inpaint mask: the active tiles only, in compact batches; the sparse blend drops the skipped tiles' visits
+            outs = []
+            tiles = self._scatter_active(x, ip) if ip.num_tiles else None
+            side_inputs = self.enable_controlnet or self.enable_stablesr
+            off = 0
+            for batch_id, bboxes in enumerate(ip.batched_bboxes):
+                if host.interrupted():
+                    return x_in
+                if side_inputs:
+                    self.switch_controlnet_tensors(batch_id, N, len(bboxes))
+                    self.switch_stablesr_tensors(batch_id)
+                outs.append(repeat_func(tiles[off * N:(off + len(bboxes)) * N], bboxes))
+                off += len(bboxes)
+                if self.pbar is not None:
+                    self.update_pbar()
+            if regions:
+                self.reset_buffer(x)
+            x_out = engine.blend_multidiffusion_sparse(self._grid, outs, N, C, self.tile_bs, self.weights, x.dtype, ip.slot_dev, ip.slot_host,
+                                                       x_buffer=self.x_buffer if regions else None, flags=self._blend_flags,
+                                                       rcp_weights=self._rcp_weights, tile_dtype=x.dtype)
+            if not regions:
+                return x_out
+        elif self.enable_grid_bbox:
             tiles = self._scatter_all(x)
             views = self._tile_batch_views(tiles, N)
             state = getattr(host.get_shared(), "state", None)      # polled per tile batch (multidiffusion.py:152)
@@ -263,4 +293,9 @@ class MultiDiffusion(AbstractDiffusion):
                 icond = icond[bbox.slicer]
             return sd_model.apply_model(x, sigma_in, cond=self.make_cond_dict(cond_in, tcond, icond))
 
-        return self.sample_one_step(x_in, org_func, repeat_func, custom_func)
+        # the inverted latent is the full plan's: there is no host mask here, and an active tile reads kept pixels too
+        self._full_plan_pass = True
+        try:
+            return self.sample_one_step(x_in, org_func, repeat_func, custom_func)
+        finally:
+            self._full_plan_pass = False

@@ -65,6 +65,9 @@ class SpotDiffusion(MultiDiffusion):
     def init_noise_inverse(self, *args, **kwargs):
         raise NotImplementedError("SpotDiffusion does not support noise inversion")
 
+    def init_inpaint_mask(self, *args, **kwargs):
+        raise NotImplementedError("SpotDiffusion does not support the inpaint mask: its windows move every step")
+
     # ------------------------------------------------------------- per call
     def draw_shift(self):
         """(shift_x, shift_y) of the next call: randrange(lo, hi) for x, then for y; an axis with one allowed shift draws nothing."""
