@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define TD_ABI_VERSION 17
+#define TD_ABI_VERSION 18
 
 typedef enum td_status {
     TD_OK = 0,
@@ -244,6 +244,16 @@ int td_vae_best_tile_size(int lowerbound, int upperbound);
  * (td_nchw_to_nhwc_wrap, or td_copy_region per piece). */
 int td_vae_split_tiles(int h, int w, int tile_size, int pad, int is_decoder, int wrap,
                        int32_t* in_bboxes, int32_t* out_bboxes, int cap);
+
+/* Tiled-VAE inpainting (new: the reference decodes every tile).  active_dev[t] = 1 when at least one element of rectangle t,
+ * over all `planes` leading planes of the mask, is not exactly 1.0 (NaN is not 1.0), else 0.  mask: DEVICE [planes, H, W]
+ * contiguous in `dtype` (image-space, 1 = keep the original), aligned to its element size.  rects_host: HOST int32
+ * [n_rects][4] = [x1, x2, y1, y2] (td_vae_split_tiles' output bboxes), each non-empty and inside [0, W) x [0, H).
+ * active_dev: DEVICE uint8 [n_rects], zeroed on the stream by this call.  Refused before any work, output untouched: a null or
+ * misaligned pointer, planes / H / W / n_rects <= 0, an unknown dtype, an empty or outside rectangle (TD_ERR_INVALID_ARG);
+ * planes * H > INT32_MAX (TD_ERR_UNSUPPORTED). */
+int td_vae_active_tiles(const void* mask, int planes, int H, int W, int dtype, const int32_t* rects_host, int n_rects,
+                        uint8_t* active_dev, void* stream);
 
 /* Statistics of `nseg` contiguous segments of `seg_len` elements each, ONE read:
  * get_var_mean -- tilevae.py:207-215 with nseg = B*32, seg_len = (C/32)*H*W (the

@@ -33,7 +33,7 @@ TD_MAX_GRID_DIM = 256
 TD_MAX_BATCH_PTRS = 128
 TD_MAX_PEERS = 16
 TD_IPC_HANDLE_BYTES = 64
-ABI_VERSION = 17
+ABI_VERSION = 18
 
 DTYPE_CODE = {torch.float16: TD_F16, torch.bfloat16: TD_BF16, torch.float32: TD_F32}
 
@@ -112,6 +112,7 @@ _SIGNATURES = {
     "td_debug_check_fast_div": (c_int, [c_int, c_int, c_void_p, c_void_p]),
     "td_vae_best_tile_size": (c_int, [c_int, c_int]),
     "td_vae_split_tiles": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_int32), POINTER(c_int32), c_int]),
+    "td_vae_active_tiles": (c_int, [c_void_p, c_int, c_int, c_int, c_int, POINTER(c_int32), c_int, c_void_p, c_void_p]),
     "td_nchw_to_nhwc_wrap": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int64, c_int64, c_int64,
                                      c_int, c_int, c_void_p]),
     "td_gn_stats_workspace_bytes": (c_int64, [c_int64, c_int64, c_int]),

@@ -7,6 +7,7 @@
 //                         crop_valid_region+paste tilevae.py:248-259,632
 //   td_resample_nearest, td_affine_clamp <- fast-mode estimator input  tilevae.py:545-559
 //   td_vae_split_tiles <- split_tiles / get_best_tile_size             tilevae.py:390-462
+//   td_vae_active_tiles   (new) the output rectangles an image-space inpaint mask reaches
 //
 // All HBM-bound streaming kernels: 128-bit vector access, fp32 statistics merged with
 // warp shuffles (Chan's parallel update: no E[x^2]-E[x]^2 cancellation), grids sized to
@@ -398,6 +399,108 @@ extern "C" int td_affine_clamp(void* x, int B, int C, int64_t HW, int dtype, con
     else if (dtype == TD_F32) affine_clamp_kernel<float><<<grid, 256, 0, s>>>((float*)x, C, HW, mean_new, std_new, mean_old, std_old, lo, hi);
     else { td_set_error("td_affine_clamp: unknown dtype %d", dtype); return TD_ERR_INVALID_ARG; }
     return launch_status("td_affine_clamp");
+}
+
+// ---- inpainting: the output rectangles an image-space mask reaches ---------------------------
+namespace {
+
+constexpr int kActiveThreads = 256;
+constexpr int kActiveRows = 16;                 // mask rows (over all planes) per CTA: ~24 KB of a cfg4 fp16 rectangle
+constexpr int kActiveRectsPerLaunch = 128;      // rectangles passed by value per launch (2 KB of parameters)
+
+struct ActiveRects {
+    int32_t r[kActiveRectsPerLaunch][4];        // [x1, x2, y1, y2]
+};
+
+// 1.0 in two packed 16-bit elements / one fp32: an element equals 1.0 exactly when its bits are these (1.0 has one encoding
+// and a NaN never has it), so a 16-byte vector is tested with four integer compares
+template <typename T> struct OneWord;
+template <> struct OneWord<__half> { static constexpr uint32_t kBits = 0x3C003C00u; };
+template <> struct OneWord<__nv_bfloat16> { static constexpr uint32_t kBits = 0x3F803F80u; };
+template <> struct OneWord<float> { static constexpr uint32_t kBits = 0x3F800000u; };
+
+// CTA (x, y): rows [x * kActiveRows, +kActiveRows) of rectangle y's planes * (y2 - y1) rows, one warp per row.  A row segment
+// is read with 16-byte loads from its first 16-byte boundary on, its ragged ends element by element.  A CTA that finds an
+// element != 1.0 stores 1; a CTA whose rectangle is already flagged reads nothing.
+template <typename T>
+__global__ void __launch_bounds__(kActiveThreads)
+vae_active_tiles_kernel(const __grid_constant__ ActiveRects rects, const T* __restrict__ mask, int planes, int H, int W,
+                        uint8_t* __restrict__ active) {
+    constexpr int VEC = Vec<T>::kElems;
+    constexpr uint32_t kOne = OneWord<T>::kBits;
+    __shared__ int s_done;
+    const int32_t* b = rects.r[blockIdx.y];
+    const int x1 = b[0], n = b[1] - b[0], y1 = b[2], h = b[3] - b[2];
+    const long long rows = (long long)planes * h;
+    const long long j0 = (long long)blockIdx.x * kActiveRows, j1 = min(j0 + kActiveRows, rows);
+    if (j0 >= rows) return;
+    if (threadIdx.x == 0) s_done = *(volatile const uint8_t*)&active[blockIdx.y];
+    __syncthreads();
+    if (s_done) return;
+    const int lane = threadIdx.x & 31;
+    int found = 0;
+    for (long long j = j0 + (threadIdx.x >> 5); j < j1; j += kActiveThreads / 32) {
+        const long long pl = j / h, y = y1 + (j - pl * h);
+        const T* row = mask + (pl * H + y) * W + x1;
+        const int head = min(n, (int)(((16u - ((uintptr_t)row & 15u)) & 15u) / sizeof(T)));
+        const int nv = (n - head) / VEC;
+        const T* body = row + head;
+        for (int v = lane; v < nv; v += 32) {
+            const uint4 q = ldg128(body + (long long)v * VEC);
+            found |= (q.x != kOne) | (q.y != kOne) | (q.z != kOne) | (q.w != kOne);
+        }
+        for (int i = lane; i < head; i += 32) found |= !(Elem<T>::to_f32(row[i]) == 1.0f);
+        for (int i = head + nv * VEC + lane; i < n; i += 32) found |= !(Elem<T>::to_f32(row[i]) == 1.0f);
+    }
+    if (__syncthreads_or(found) && threadIdx.x == 0) active[blockIdx.y] = 1;
+}
+
+}  // namespace
+
+extern "C" int td_vae_active_tiles(const void* mask, int planes, int H, int W, int dtype, const int32_t* rects_host, int n_rects,
+                                   uint8_t* active_dev, void* stream) {
+    const int es = td_dtype_size(dtype);
+    if (es == 0) { td_set_error("td_vae_active_tiles: unknown dtype %d", dtype); return TD_ERR_INVALID_ARG; }
+    if (mask == nullptr || active_dev == nullptr || rects_host == nullptr || ((uintptr_t)mask % (uintptr_t)es) != 0) {
+        td_set_error("td_vae_active_tiles: null or misaligned mask / rectangles / output");
+        return TD_ERR_INVALID_ARG;
+    }
+    if (planes <= 0 || H <= 0 || W <= 0 || n_rects <= 0) {
+        td_set_error("td_vae_active_tiles: planes = %d, H = %d, W = %d, n_rects = %d must be positive", planes, H, W, n_rects);
+        return TD_ERR_INVALID_ARG;
+    }
+    for (int t = 0; t < n_rects; ++t) {
+        const int32_t* b = rects_host + 4LL * t;
+        if (!(0 <= b[0] && b[0] < b[1] && b[1] <= W && 0 <= b[2] && b[2] < b[3] && b[3] <= H)) {
+            td_set_error("td_vae_active_tiles: rectangle %d = [%d, %d) x [%d, %d) is empty or leaves the %d x %d mask", t, b[0], b[1],
+                         b[2], b[3], W, H);
+            return TD_ERR_INVALID_ARG;
+        }
+    }
+    if ((long long)planes * H > INT32_MAX) {
+        td_set_error("td_vae_active_tiles: %lld mask rows exceed the grid limit", (long long)planes * H);
+        return TD_ERR_UNSUPPORTED;
+    }
+    cudaStream_t s = (cudaStream_t)stream;
+    int st = launch_status("td_vae_active_tiles (zero)", cudaMemsetAsync(active_dev, 0, (size_t)n_rects, s));
+    if (st != TD_OK) return st;
+    for (int r0 = 0; r0 < n_rects; r0 += kActiveRectsPerLaunch) {
+        const int k = std::min(kActiveRectsPerLaunch, n_rects - r0);
+        ActiveRects p;
+        long long rows = 0;
+        for (int t = 0; t < k; ++t) {
+            for (int e = 0; e < 4; ++e) p.r[t][e] = rects_host[4LL * (r0 + t) + e];
+            rows = std::max(rows, (long long)planes * (p.r[t][3] - p.r[t][2]));
+        }
+        const dim3 grid((unsigned)((rows + kActiveRows - 1) / kActiveRows), (unsigned)k);
+#define TD_LAUNCH(T) vae_active_tiles_kernel<T><<<grid, kActiveThreads, 0, s>>>(p, (const T*)mask, planes, H, W, active_dev + r0)
+        if (dtype == TD_F16) TD_LAUNCH(__half);
+        else if (dtype == TD_BF16) TD_LAUNCH(__nv_bfloat16);
+        else TD_LAUNCH(float);
+#undef TD_LAUNCH
+        if ((st = launch_status("td_vae_active_tiles")) != TD_OK) return st;
+    }
+    return TD_OK;
 }
 
 // ---- host bookkeeping ----------------------------------------------------------------------

@@ -248,6 +248,22 @@ def active_tiles(g: TdGrid, mask: torch.Tensor) -> np.ndarray:
     return out.cpu().numpy().astype(bool)
 
 
+def vae_active_tiles(mask: torch.Tensor, rects) -> np.ndarray:
+    """bool [T]: the rectangles (int32 [T, 4] of [x1, x2, y1, y2], the tiled VAE's output bboxes) that hold at least one
+    element of the image-space mask, over all leading planes, that is not exactly 1.0 (NaN included).  mask: [..., H, W] on
+    the device, in fp16, bf16 or fp32 (td_vae_active_tiles; the T flags are read back here)."""
+    _require_cuda(mask, "mask")
+    m = mask.contiguous()
+    H, W = m.shape[-2], m.shape[-1]
+    r = np.ascontiguousarray(np.asarray(rects, dtype=np.int32).reshape(-1, 4))
+    out = torch.empty(r.shape[0], dtype=torch.uint8, device=m.device)
+    with torch.cuda.device(m.device):
+        check(lib.td_vae_active_tiles(m.data_ptr(), int(m.numel() // max(H * W, 1)), int(H), int(W), dtype_code(m.dtype),
+                                      r.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), int(r.shape[0]), out.data_ptr(),
+                                      current_stream_ptr(m.device)))
+    return out.cpu().numpy().astype(bool)
+
+
 def slot_table(active: np.ndarray) -> np.ndarray:
     """int32 [T]: each active tile's position in the compact tile batches (active tiles in tile order), -1 for a skipped tile."""
     active = np.asarray(active, dtype=bool)

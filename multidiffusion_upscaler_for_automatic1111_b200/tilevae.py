@@ -34,7 +34,7 @@ import numpy as np
 import torch
 import torch.nn.functional as F
 
-from . import host
+from . import engine, host
 from ._cabi import check, current_stream_ptr, dtype_code, lib
 
 NUM_GROUPS = 32
@@ -414,6 +414,12 @@ def pick_images_per_pass(n: int, fits: Callable[[int], bool]) -> int:
     return 1
 
 
+def shard_tiles(tiles, world: int, rank: int) -> List[int]:
+    """The tiles rank `rank` of a `world`-rank tile shard runs out of the tiles a pass runs (in order): every world-th, so
+    the ranks stay balanced when an inpaint mask skips tiles."""
+    return list(tiles)[rank::world]
+
+
 class VAEHook:
 
     def __init__(self, net, tile_size, is_decoder: bool, fast_decoder: bool, fast_encoder: bool, color_fix: bool, to_gpu: bool = False):
@@ -439,6 +445,10 @@ class VAEHook:
         # their halo from the opposite edge, so a wrapped decode of a seamless latent has no seam (td_vae_split_tiles' `wrap`).
         self.wrap_x: bool = False
         self.wrap_y: bool = False
+        # Inpainting (fast-mode decoder): [P, 1, oh, ow] image-space mask, 1 = keep the original, and the [P, out_c, oh, ow]
+        # canvas the skipped tiles keep (None: zeros).  Set with `set_inpaint_mask`.
+        self.inpaint_mask: Optional[torch.Tensor] = None
+        self.inpaint_fill: Optional[torch.Tensor] = None
         self._program = None
         self._shard_group = None
         self._shard_world = 1
@@ -452,6 +462,56 @@ class VAEHook:
         self._shard_group = group
         self._shard_world = dist.get_world_size(group)
         self._shard_rank = dist.get_rank(group)
+
+    def set_inpaint_mask(self, mask: Optional[torch.Tensor], fill: Optional[torch.Tensor] = None) -> None:
+        """Decode only the tiles an inpaint mask reaches, in every later call until `set_inpaint_mask(None)`.  New: the
+        reference decodes every tile.
+
+        mask: image-space, 1 = keep the original (the host's blurred overlay mask, inverted and scaled to [0, 1]), [oh, ow],
+        [1, oh, ow] or [N, 1, oh, ow], fp16 / bf16 / fp32 on the device.  A tile runs when one mask element in its output
+        rectangle is not exactly 1.0 (NaN included); with per-image masks, when one image of its pass reaches it.
+        fill: None (zeros) or [N or 1, out_c, oh, ow] in the network's dtype on its device, e.g. the init image in [-1, 1]:
+        what the skipped rectangles of the result hold.  An active tile's rectangle is bit-identical to an unmasked call.
+
+        Fast-mode decoders only: every GroupNorm site is then frozen before the tiles run, so skipping a tile changes no
+        other tile.  An image whose estimate met a NaN (slow mode) runs all its tiles.  Refused before any change:
+        NotImplementedError for an encoder or slow mode, ValueError for a bad shape or dtype."""
+        if mask is None:
+            self.inpaint_mask = self.inpaint_fill = None
+            return
+        if not self.is_decoder:
+            raise NotImplementedError("[Tiled VAE]: inpainting skips decoder tiles only; the encoder needs the whole latent")
+        if not self.fast_mode:
+            raise NotImplementedError("[Tiled VAE]: inpainting needs the fast decoder: slow mode's GroupNorm barriers need every tile")
+        floats = (torch.float16, torch.bfloat16, torch.float32)
+        if not isinstance(mask, torch.Tensor) or mask.dtype not in floats:
+            raise ValueError(f"inpaint mask must be an fp16 / bf16 / fp32 tensor, got {getattr(mask, 'dtype', type(mask))}")
+        shape = tuple(mask.shape)
+        ok = (len(shape) == 2 or (len(shape) == 3 and shape[0] == 1) or (len(shape) == 4 and shape[1] == 1 and shape[0] >= 1))
+        if not ok or mask.numel() == 0:
+            raise ValueError(f"inpaint mask shape {shape}: expected [oh, ow], [1, oh, ow] or [N, 1, oh, ow]")
+        if fill is not None:
+            if not isinstance(fill, torch.Tensor) or fill.dtype not in floats:
+                raise ValueError(f"inpaint fill must be an fp16 / bf16 / fp32 tensor, got {getattr(fill, 'dtype', type(fill))}")
+            if fill.dim() != 4 or fill.numel() == 0 or tuple(fill.shape[-2:]) != shape[-2:]:
+                raise ValueError(f"inpaint fill shape {tuple(fill.shape)}: expected [N or 1, out_c, {shape[-2]}, {shape[-1]}]")
+        for what, t in (("mask", mask), ("fill", fill)):
+            if t is not None and not t.is_cuda:
+                raise ValueError(f"inpaint {what} must be on the device, got {t.device}")
+        self.inpaint_mask = mask.reshape(-1, 1, shape[-2], shape[-1]).contiguous()
+        self.inpaint_fill = fill.contiguous() if fill is not None else None
+
+    def _inpaint_inputs(self, N, out_c, oh, ow, device, dtype):
+        """(mask, fill) checked against this call, before any tile runs."""
+        mask, fill = self.inpaint_mask, self.inpaint_fill
+        if mask.shape[0] not in (1, N) or tuple(mask.shape[-2:]) != (oh, ow) or mask.device != device:
+            raise ValueError(f"inpaint mask {tuple(mask.shape)} on {mask.device} does not match this call: {N} images of {oh} x {ow} "
+                             f"on {device}")
+        if fill is not None and (fill.shape[0] not in (1, N) or tuple(fill.shape[1:]) != (out_c, oh, ow) or fill.dtype != dtype
+                                 or fill.device != device):
+            raise ValueError(f"inpaint fill {tuple(fill.shape)} {fill.dtype} on {fill.device} does not match this call: "
+                             f"[{N} or 1, {out_c}, {oh}, {ow}] {dtype} on {device}")
+        return mask, fill
 
     def __call__(self, x):
         original_device = next(self.net.parameters()).device
@@ -517,18 +577,28 @@ class VAEHook:
         est_in = fast_mode_estimator_input(z, tile_size) if self.fast_mode else None
 
         sharded = self._shard_world > 1
-        mine = [i for i in range(len(in_bboxes)) if i % self._shard_world == self._shard_rank] if sharded else list(range(len(in_bboxes)))
-        my_in, my_out = [in_bboxes[i] for i in mine], [out_bboxes[i] for i in mine]
+        num_tiles = len(in_bboxes)
+        mine = shard_tiles(range(num_tiles), self._shard_world, self._shard_rank)
+        my_in = [in_bboxes[i] for i in mine]
         out_c = [op for op in program.ops if isinstance(op, ve.Conv)][-1].module.out_channels
         oh, ow = (height * 8, width * 8) if is_decoder else (height // 8, width // 8)
-        result = torch.zeros((N, out_c, oh, ow), dtype=dtype, device=device)   # zeros: a partial (interrupted) result reads 0 elsewhere
+        mask, fill = self._inpaint_inputs(N, out_c, oh, ow, device, dtype) if self.inpaint_mask is not None else (None, None)
+        if fill is None:
+            result = torch.zeros((N, out_c, oh, ow), dtype=dtype, device=device)   # zeros: a partial (interrupted) result reads 0 elsewhere
+        else:
+            result = torch.empty((N, out_c, oh, ow), dtype=dtype, device=device)
+            for n in range(N) if fill.shape[0] == 1 and N > 1 else (None,):
+                copy_region(fill, result if n is None else result[n:n + 1])
         # budget / reserve: bytes (None when no barrier); host_bytes: pinned host memory (its peak: buffers live until the
         # call ends); d2h / h2d_bytes: bytes copied each way; pin_s: seconds spent pinning; tiles_parked: {site: tiles}
-        # images_per_pass: images that went through the tiles together
+        # images_per_pass: images that went through the tiles together; tiles_run: tiles this rank ran, summed over the
+        # passes; tiles_skipped: tiles no rank ran because the inpaint mask does not reach them, summed over the passes
         self.last_park_stats = {"budget": None, "reserve": None, "host_bytes": 0, "d2h_bytes": 0, "h2d_bytes": 0, "pin_s": 0.0,
-                                "tiles_parked": {}}
+                                "tiles_parked": {}, "tiles_run": 0, "tiles_skipped": 0}
         k = self._images_per_pass(program, backend, z, my_in) if isinstance(backend, ve.TensorCoreBackend) else N
         self.last_park_stats["images_per_pass"] = k
+        # (images, tiles) whose output regions the shard exchanges: every tile of the batch, or per pass the tiles it ran
+        exchanged = [] if mask is not None else [(slice(0, N), list(range(num_tiles)))]
 
         def one_pass(img):
             """Tiles finished by one pass over images `img`; None when the estimate of a batched pass met a NaN."""
@@ -539,7 +609,17 @@ class VAEHook:
                         return None
                 else:
                     ex.estimate(backend.load(est_in[img]), self.color_fix)
-            return self._run_tiles(ex, backend, z[img], result[img], my_in, my_out)
+            tiles = list(range(num_tiles))
+            if mask is not None:
+                # frozen sites only: a tile's output then depends on its own input and the pass's images.  A pass with a
+                # barrier (an estimate that met a NaN) needs every tile's statistics and runs them all
+                if ex.barrier_sites() == 0:
+                    tiles = np.flatnonzero(engine.vae_active_tiles(mask if mask.shape[0] == 1 else mask[img], out_bboxes)).tolist()
+                exchanged.append((img, tiles))
+            run = shard_tiles(tiles, self._shard_world, self._shard_rank)
+            self.last_park_stats["tiles_run"] += len(run)
+            self.last_park_stats["tiles_skipped"] += num_tiles - len(tiles)
+            return self._run_tiles(ex, backend, z[img], result[img], [in_bboxes[i] for i in run], [out_bboxes[i] for i in run])
 
         finished = 0
         for start in range(0, N, k):
@@ -557,7 +637,7 @@ class VAEHook:
                 break
         interrupted = host.interrupted()
         if sharded:
-            self._exchange_regions(result, in_bboxes, out_bboxes)
+            self._exchange_regions(result, out_bboxes, exchanged)
         if finished == 0 and mine and interrupted:
             return self._cheap_fallback(z, device, dtype)
         if not interrupted and torch.isnan(result).any():
@@ -714,30 +794,37 @@ class VAEHook:
             k = int(t.item())
         return k
 
-    def _exchange_regions(self, result, in_bboxes, out_bboxes):
+    def _exchange_regions(self, result, out_bboxes, exchanged):
         """Tile shard: every rank pasted its own tiles; gather the disjoint output regions (one all-gather of the
-        packed regions -- each byte crosses NVLink once; the round-1 all_reduce of the whole canvas moved it twice)."""
+        packed regions -- each byte crosses NVLink once; the round-1 all_reduce of the whole canvas moved it twice).
+        exchanged: (images, tiles) per pass; rank r owns shard_tiles(tiles, world, r) of those images.  A tile the inpaint
+        mask skipped is in no list: every rank holds its fill already."""
         import torch.distributed as dist
         world, rank = self._shard_world, self._shard_rank
-        owners = [[i for i in range(len(out_bboxes)) if i % world == r] for r in range(world)]
-        sizes = [sum((out_bboxes[i][1] - out_bboxes[i][0]) * (out_bboxes[i][3] - out_bboxes[i][2]) for i in own) for own in owners]
-        plane = result.shape[0] * result.shape[1]
-        cap = max(sizes) * plane
+        planes = lambda img: len(range(*img.indices(result.shape[0]))) * result.shape[1]
+        area = lambda b: (b[1] - b[0]) * (b[3] - b[2])
+        owners = [[(img, shard_tiles(tiles, world, r)) for img, tiles in exchanged] for r in range(world)]
+        sizes = [sum(planes(img) * area(out_bboxes[i]) for img, own in jobs for i in own) for jobs in owners]
+        cap = max(sizes)
+        if cap == 0:
+            return
         send = torch.zeros(cap, dtype=result.dtype, device=result.device)
         off = 0
-        for i in owners[rank]:
-            b = out_bboxes[i]
-            blk = result[:, :, b[2]:b[3], b[0]:b[1]]
-            send[off:off + blk.numel()].view(blk.shape).copy_(blk)
-            off += blk.numel()
+        for img, own in owners[rank]:
+            for i in own:
+                b = out_bboxes[i]
+                blk = result[img, :, b[2]:b[3], b[0]:b[1]]
+                send[off:off + blk.numel()].view(blk.shape).copy_(blk)
+                off += blk.numel()
         recv = torch.empty(world * cap, dtype=result.dtype, device=result.device)
         dist.all_gather_into_tensor(recv, send, group=self._shard_group)
         for r in range(world):
             if r == rank:
                 continue
             off = r * cap
-            for i in owners[r]:
-                b = out_bboxes[i]
-                dst = result[:, :, b[2]:b[3], b[0]:b[1]]
-                dst.copy_(recv[off:off + dst.numel()].view(dst.shape))
-                off += dst.numel()
+            for img, own in owners[r]:
+                for i in own:
+                    b = out_bboxes[i]
+                    dst = result[img, :, b[2]:b[3], b[0]:b[1]]
+                    dst.copy_(recv[off:off + dst.numel()].view(dst.shape))
+                    off += dst.numel()
