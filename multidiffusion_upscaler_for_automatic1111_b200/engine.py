@@ -126,7 +126,8 @@ def _batch_table(g: TdGrid, batch_outs: Sequence[torch.Tensor], N: int, C: int, 
 def _fit_batch_table(g: TdGrid, batch_outs: Sequence[torch.Tensor], tile_bs: int):
     """The kernels take at most TD_MAX_BATCH_PTRS output tensors per launch (pointers travel in the kernel parameter
     block).  The reference accepts any batch count (e.g. 441 tiles with tile_bs 3 = 147 batches): concatenate groups of
-    k consecutive full batches into one tensor each and report the new tile_bs = k * tile_bs.  Tile order is unchanged."""
+    k consecutive full batches into one tensor each and report the new tile_bs = k * tile_bs.  Tile order is unchanged.
+    The plan `g` is not read: the window-list blend (`blend_bboxes`, g None) fits its table the same way."""
     from ._cabi import TD_MAX_BATCH_PTRS
     n = len(batch_outs)
     if n <= TD_MAX_BATCH_PTRS:
@@ -450,18 +451,36 @@ def scatter_bboxes(x: torch.Tensor, origins_dev: torch.Tensor, origins_host, n_t
 def blend_bboxes(batch_outs: Sequence[torch.Tensor], tile_bs: int, origins_dev: torch.Tensor, origins_host, n_tiles: int, N: int, C: int,
                  H: int, W: int, tile_h: int, tile_w: int, wrap: int = 0) -> torch.Tensor:
     """Window LIST count-normalised blend (demofusion.py:259-264): fp32 [N,C,H,W] = ordered sum (rounded through the tile
-    dtype per add) / max(count, 1).  `wrap` as in `scatter_bboxes`: coverage is modular on those axes, and window pixels
-    off the canvas on a bounded axis are dropped (td_blend_bboxes_wrap)."""
+    dtype per add) / max(count, 1), the count exact (an int per pixel, not the tile dtype).  `wrap` as in `scatter_bboxes`:
+    coverage is modular on those axes, and window pixels off the canvas on a bounded axis are dropped (td_blend_bboxes_wrap).
+
+    batch_outs: ceil(n_tiles / tile_bs) tensors, batch b of shape (min(tile_bs, n_tiles - b*tile_bs)*N, C, tile_h, tile_w), one
+    dtype, one CUDA device; above TD_MAX_BATCH_PTRS batches they are concatenated in groups as the grid blends do."""
+    n_tiles, tile_bs = int(n_tiles), int(tile_bs)
+    if tile_bs <= 0 or n_tiles <= 0 or len(batch_outs) != -(-n_tiles // tile_bs):
+        raise ValueError(f"{len(batch_outs)} tile batches of {tile_bs} for {n_tiles} windows")
     dev, dt = batch_outs[0].device, batch_outs[0].dtype
-    _require_cuda(batch_outs[0], "tile output")
-    ptrs = (ctypes.c_void_p * len(batch_outs))(*[t.data_ptr() for t in batch_outs])
+    keep = []
+    for b, t in enumerate(batch_outs):
+        if not t.is_cuda or t.dtype != dt or t.device != dev:
+            raise ValueError(f"tile batch {b} is {t.dtype} on {t.device}, batch 0 is {dt} on {dev}: one dtype, one CUDA device")
+        want = (min(tile_bs, n_tiles - b * tile_bs) * N, C, tile_h, tile_w)
+        if tuple(t.shape) != want:
+            raise ValueError(f"tile batch {b} has shape {tuple(t.shape)}, expected {want}")
+        keep.append(t.contiguous())
+    if origins_dev.device != dev or origins_dev.dtype != torch.int32 or origins_dev.numel() != 2 * n_tiles or not origins_dev.is_contiguous():
+        raise ValueError(f"origins_dev must be a contiguous int32 tensor of {2 * n_tiles} elements on {dev}")
+    if origins_host is None or len(origins_host) < 2 * n_tiles:
+        raise ValueError(f"origins_host must hold {2 * n_tiles} values")
+    keep, tile_bs = _fit_batch_table(None, keep, tile_bs)
+    ptrs = (ctypes.c_void_p * len(keep))(*[t.data_ptr() for t in keep])
     out = torch.empty((N, C, H, W), dtype=torch.float32, device=dev)
     with torch.cuda.device(dev):
         if wrap:
-            check(lib.td_blend_bboxes_wrap(ptrs, len(batch_outs), int(tile_bs), origins_dev.data_ptr(), origins_host, int(n_tiles), N, C, H,
+            check(lib.td_blend_bboxes_wrap(ptrs, len(keep), int(tile_bs), origins_dev.data_ptr(), origins_host, n_tiles, N, C, H,
                                            W, int(tile_h), int(tile_w), int(wrap), dtype_code(dt), out.data_ptr(), current_stream_ptr(dev)))
         else:
-            check(lib.td_blend_bboxes(ptrs, len(batch_outs), int(tile_bs), origins_dev.data_ptr(), origins_host, int(n_tiles), N, C, H, W,
+            check(lib.td_blend_bboxes(ptrs, len(keep), int(tile_bs), origins_dev.data_ptr(), origins_host, n_tiles, N, C, H, W,
                                       int(tile_h), int(tile_w), dtype_code(dt), out.data_ptr(), current_stream_ptr(dev)))
     return out
 

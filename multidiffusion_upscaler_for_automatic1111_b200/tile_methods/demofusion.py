@@ -368,7 +368,7 @@ class DemoFusion(AbstractDiffusion):
         dt, dev = x.dtype, x.device
         s = int(p.current_scale_num)
 
-        # ---- local windows: count-normalised blend (buffer / count, both in x.dtype) ----------------------------
+        # ---- local windows: count-normalised blend (buffer in x.dtype / exact count, in fp32, rounded to x.dtype) ------
         if self._shard_on:
             x_local = self._local_pass_sharded(x, repeat_func)
             if x_local is None:

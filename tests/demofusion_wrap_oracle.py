@@ -46,11 +46,11 @@ def demofusion_views(w: int, h: int, window_size: int, overlap: int, wrap: int, 
     return out, jr
 
 
-def axis_indices(o: int, n: int, L: int, wrapped: bool):
+def axis_indices(o: int, n: int, L: int, wrapped: bool, device=None):
     """Canvas indices of o .. o + n - 1 on one axis (mod L when wrapped) and which of them lie on the canvas."""
-    i = torch.arange(o, o + n)
+    i = torch.arange(o, o + n, device=device)
     if wrapped:
-        return i % L, torch.ones(n, dtype=torch.bool)
+        return i % L, torch.ones(n, dtype=torch.bool, device=device)
     ok = (i >= 0) & (i < L)
     return i.clamp(0, L - 1), ok
 
@@ -58,8 +58,8 @@ def axis_indices(o: int, n: int, L: int, wrapped: bool):
 def demofusion_crop(x: torch.Tensor, b: BBox, wrap: int) -> torch.Tensor:
     """One window of x [N,C,H,W]: modular on a wrapped axis, zeros off a bounded one."""
     H, W = x.shape[2], x.shape[3]
-    iy, oky = axis_indices(b[1], b[3], H, bool(wrap & WRAP_Y))
-    ix, okx = axis_indices(b[0], b[2], W, bool(wrap & WRAP_X))
+    iy, oky = axis_indices(b[1], b[3], H, bool(wrap & WRAP_Y), x.device)
+    ix, okx = axis_indices(b[0], b[2], W, bool(wrap & WRAP_X), x.device)
     t = x[:, :, iy][:, :, :, ix].clone()
     t[:, :, ~oky] = 0
     t[:, :, :, ~okx] = 0
@@ -81,6 +81,24 @@ def demofusion_gaussian_filter(latents: torch.Tensor, kernel_size: int, sigma, w
     return y.to(latents.dtype)
 
 
+def local_blend(x_like: torch.Tensor, windows: Sequence[BBox], outs: Sequence[torch.Tensor], wrap: int) -> torch.Tensor:
+    """demofusion_step's local blend for windows (x, y, w, h) and their outputs outs[t] [N,C,h,w], in list order, from
+    explicit modular index arrays: modular on the wrapped axes, window pixels off a bounded axis dropped.  The buffer is
+    accumulated window by window in x_like.dtype and divided by the exact fp32 count (1 where no window covers a pixel);
+    returns that fp32 quotient, on x_like's device (oracle/demofusion.local_blend on a periodic canvas)."""
+    assert len(windows) == len(outs)
+    H, W = x_like.shape[2], x_like.shape[3]
+    x_buffer = torch.zeros_like(x_like)
+    count = torch.zeros((H, W), dtype=torch.float32, device=x_like.device)
+    for b, out in zip(windows, outs):
+        iy, oky = axis_indices(b[1], b[3], H, bool(wrap & WRAP_Y), x_like.device)
+        ix, okx = axis_indices(b[0], b[2], W, bool(wrap & WRAP_X), x_like.device)
+        iy, ix = iy[oky][:, None], ix[okx][None, :]
+        x_buffer[:, :, iy, ix] = x_buffer[:, :, iy, ix] + out[:, :, oky][:, :, :, okx]
+        count[iy, ix] = count[iy, ix] + 1
+    return x_buffer.float() / torch.where(count == 0, 1.0, count)
+
+
 def demofusion_step(x: torch.Tensor, local_batches: Sequence[Sequence[BBox]], global_batches: Sequence[Sequence[Tuple[int, int]]],
                     scale: int, mixture: bool, use_gaussian: bool, sig: float, cos_factor: torch.Tensor, cs2: float, cs3: float,
                     denoise_local: Callable, denoise_global: Callable, wrap: int = 0, jitter_range: int = 0) -> torch.Tensor:
@@ -92,7 +110,9 @@ def demofusion_step(x: torch.Tensor, local_batches: Sequence[Sequence[BBox]], gl
     wrap == 0 with jitter_range > 0 is the reference's padded path: x is zero-padded by jitter_range, the windows move
     by +jitter_range, the views start at jitter_range and stop at `end = W_padded - jitter_range` on both axes, and the
     result is cropped back.  Written with explicit per-window loops and modular index arrays; every op rounds in x.dtype
-    where the reference's eager ops do (oracle/demofusion.py)."""
+    where the reference's eager ops do (oracle/demofusion.py), except the local window count: that is an exact fp32 count
+    and the quotient buffer / count is rounded to x.dtype.  The reference's x.dtype count saturates at 256 (bf16) and
+    2048 (fp16) and would scale x_local by coverage / 256 past them; up to those coverages both rules give the same bits."""
     F = torch.nn.functional
     jr = jitter_range if wrap == 0 else 0
     H0, W0 = x.shape[2], x.shape[3]
@@ -100,20 +120,13 @@ def demofusion_step(x: torch.Tensor, local_batches: Sequence[Sequence[BBox]], gl
         x = F.pad(x, (jr, jr, jr, jr), "constant", value=0)
         local_batches = [[(bx + jr, by + jr, bw, bh) for (bx, by, bw, bh) in bb] for bb in local_batches]
     N, H, W = x.shape[0], x.shape[2], x.shape[3]
-    wy, wx = bool(wrap & WRAP_Y), bool(wrap & WRAP_X)
 
-    x_buffer = torch.zeros_like(x)
-    weights = torch.zeros_like(x)
+    windows, outs = [], []
     for bboxes in local_batches:
         out = denoise_local(torch.cat([demofusion_crop(x, b, wrap) for b in bboxes], dim=0), bboxes)
-        for i, b in enumerate(bboxes):
-            iy, oky = axis_indices(b[1], b[3], H, wy)
-            ix, okx = axis_indices(b[0], b[2], W, wx)
-            idx = (slice(None), slice(None), iy[oky][:, None], ix[okx][None, :])
-            x_buffer[idx] = x_buffer[idx] + out[i * N:(i + 1) * N][:, :, oky][:, :, :, okx]
-            weights[idx] = weights[idx] + 1
-    weights = torch.where(weights == 0, torch.tensor(1), weights)
-    x_local = x_buffer / weights
+        windows += list(bboxes)
+        outs += [out[i * N:(i + 1) * N] for i in range(len(bboxes))]
+    x_local = local_blend(x, windows, outs, wrap).to(x.dtype)
 
     std_, mean_ = x.std(), x.mean()
     c3 = 0.99 * cos_factor ** cs3 + 1e-2
